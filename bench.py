@@ -2,7 +2,7 @@
 """Benchmark of the GLAMR global-optimisation hot path (BASELINE.json metric: global-opt iterations/sec over
 frames x persons), one process per GPU.
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--extras all|none|a,b,..]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--extras all|none|a,b,..] [--dump-outputs DIR]
     python -m torch.distributed.run --nnodes=1 --nproc-per-node N --master-addr 127.0.0.1 --master-port P bench.py --gpus N ...
 
 One "step" = one optimiser iteration of GlobalReconOptimizer.optimize_main (trajectory codec + camera + full SMPL
@@ -13,9 +13,13 @@ same line (`extras`): the north-star video (glamr_static_multi, 4 persons x 300 
 N GPUs = strong scaling), configs[3] (8 x 500 glamr_static_multi), configs[2] (prior networks, 64 x 120) and configs[4]
 (32 independent 300-frame sequences through run_dataset, replicas over the N GPUs).
 
---impl reference times the reference algorithm's CPU path on this box's host cores: the oracle port under oracle/
-(torch-CPU restatement pinned to the executed reference by tests/golden), because /root/reference is not on the
-GPU box.  It is the only place besides tests/ and smoke() that executes oracle/ code.
+--steps K sets the number of timed iterations of the headline workload: K with L2 flushed before each (ms_per_step), then K
+back to back (ms_per_step_l2_warm).  --dump-outputs DIR writes, after them, what the last timed iteration computed (see
+dump_outputs) so that two builds can be compared output for output; the inputs are seeded and identical from run to run.
+
+--impl reference times the reference algorithm's CPU path on the host cores: the oracle port under oracle/
+(torch-CPU restatement pinned to the executed reference by tests/golden), so that the benchmark needs nothing outside
+this repository.  It is the only place besides tests/ and smoke() that executes oracle/ code.
 """
 import argparse
 import copy
@@ -43,9 +47,6 @@ T_START = time.perf_counter()
 # is spent, so that the headline line is always printed within minutes even on a host that is busy with other jobs
 BENCH_BUDGET_S = float(os.environ.get('GLAMR_BENCH_BUDGET_S', 480.0))
 REF_BUDGET_S = float(os.environ.get('GLAMR_REF_BUDGET_S', 150.0))   # wall-clock bound (s) of the CPU reference arm (--impl reference)
-# dram__bytes_read.sum + dram__bytes_write.sum of one LBS launch, keyed by frame-persons per launch (ncu capture, profiles/)
-NCU_BLEND_DRAM_BYTES = {300: 37911808 + 2394624}               # lbs_blend_tc_kernel alone
-NCU_LBS_DRAM_BYTES = {300: 37911808 + 2394624 + 26944768}     # blend (read + write) + tensor-core skinning (read), profiles/lbs_tc_kernels_r02_final.md
 # switches that change what the library executes: the bench refuses to run with any of them set
 FORBIDDEN_ENV = ['GLAMR_B200_SO', 'GLAMR_LBS_DEBUG', 'GLAMR_TC_DEBUG', 'GLAMR_PDL', 'GLAMR_LBS_STAGES', 'GLAMR_TC_NTILE']
 ECHO_ENV = FORBIDDEN_ENV + ['GLAMR_ITER_PATH', 'GLAMR_LBS_PATH', 'GLAMR_PRIOR_GRAPH', 'GLAMR_NET_WIMG', 'GLAMR_NET_SKINNY', 'GLAMR_ALLREDUCE', 'OMP_NUM_THREADS', 'NCCL_ALGO', 'NCCL_PROTO']
@@ -63,6 +64,8 @@ def parse():
     ap.add_argument('--extras', default='all', help="'all', 'none' or a comma list of " + ','.join(ALL_EXTRAS))
     ap.add_argument('--cpu-sample-iters', type=int, default=20)
     ap.add_argument('--no-cpu-baseline', action='store_true')
+    ap.add_argument('--dump-outputs', metavar='DIR', default=None,
+                    help='write what the last timed iteration computed as DIR/<name>.npy (float32 / float64, <= 64 MB in all)')
     return ap.parse_args()
 
 
@@ -74,7 +77,7 @@ def refuse_experiment_switches():
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons during the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks / throttle reasons during the timed region."""
     Q = 'index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,clocks_event_reasons.hw_thermal_slowdown,' \
         'clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap'
 
@@ -206,8 +209,8 @@ class CpuPort:
     def sweep_threads(self, warm=1, probe=3, budget_s=40.0):
         """median seconds per iteration for each candidate thread count, smallest count first.  Bounded three ways (boxes exist
         where many-thread torch CPU runs are 25-250x slower than 8 threads, and hosts shared with other jobs where they take
-        minutes): the all-threads candidate only runs on hosts with <= 64 threads (128 threads measured 4.5 - 12 s per iteration
-        against 45 - 100 ms at 16 - 32, profiles/README_r02.md); a candidate is abandoned as soon as one of its iterations takes
+        minutes): the all-threads candidate only runs on hosts with <= 64 threads (128 threads have taken seconds per iteration
+        against tens of ms at 16 - 32); a candidate is abandoned as soon as one of its iterations takes
         > 3x the best median so far; the sweep stops when a candidate is slower than the one before it (the scaling has turned
         over), when `budget_s` is spent, or when a candidate hits its own wall-clock limit.  -> (best_threads, {threads: median})"""
         cands = sorted({t for t in (8, 16, 32) if t <= host_threads()} | ({host_threads()} if host_threads() <= 64 else set()))
@@ -434,7 +437,7 @@ class StageLoop:
         evs = [(torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)) for _ in range(K)]
         ctx.barrier()
         for a, b in evs:
-            ctx.flush.fill_(1)                   # evict L2 (126 MB) between timed iterations
+            ctx.flush.fill_(1)                   # evict L2 (50 MB on an H100) between timed iterations
             a.record()
             self.step()
             b.record()
@@ -658,6 +661,30 @@ def c5_sweep(ctx, n_seq=32, frames=300):
             'sequences_this_rank': len(done), 'ms_per_sequence_this_rank': float(np.mean([d[3] for d in done]) * 1e3) if done else None}
 
 
+DUMP_BUDGET_BYTES = 64 * 1024 * 1024
+
+
+def dump_outputs(out_dir, model, data):
+    """what a caller of the timed iteration receives after its last step: the optimisation variables after the Adam update
+    (theta) and the per-frame outputs of the evaluation that produced the gradient (the entries optimize_main leaves in the
+    data dict), as DIR/<name>.npy in float32 (float64 where the library computes in float64).  An array whose share of the
+    64 MB budget is too small is replaced by a fixed strided sample of its flattened values."""
+    arrays = {'theta': model._theta, 'cam_pose': data['cam_pose'], 'cam_pose_inv': data['cam_pose_inv']}
+    for pid, d in enumerate(data['person_data'].values()):
+        for k in ['smpl_orient_world', 'root_trans_world', 'smpl_orient_world_base', 'root_trans_world_base', 'kp_2d_pred',
+                  'smpl_orient_cam_in_world', 'root_trans_cam_in_world', 'traj_local', 'joints_world']:
+            arrays[f'person{pid}_{k}'] = d[k]
+    arrays = {k: v.detach().cpu().numpy() for k, v in arrays.items()}
+    arrays = {k: v.astype(np.float64 if v.dtype == np.float64 else np.float32) for k, v in arrays.items()}
+    total = sum(a.nbytes for a in arrays.values())
+    os.makedirs(out_dir, exist_ok=True)
+    for k, a in arrays.items():
+        cap = DUMP_BUDGET_BYTES * a.nbytes // max(total, 1) // a.itemsize
+        if a.size > cap:
+            a = np.ascontiguousarray(a.reshape(-1)[::-(-a.size // max(cap, 1))])
+        np.save(os.path.join(out_dir, k + '.npy'), a)
+
+
 def run_ours(args):
     refuse_experiment_switches()
     # all CPU legs of this run (main cpu_baseline + the north-star one) share one wall-clock budget: the GPU numbers must not wait for a busy host
@@ -679,6 +706,10 @@ def run_ours(args):
         sampler.start()
     cold_ms, warm_ms = loop.time(K)
     clocks = sampler.stop() if rank == 0 else None
+    if args.dump_outputs:
+        model._scatter_outputs(data)          # collective when the frame-persons are sharded
+        if rank == 0:
+            dump_outputs(args.dump_outputs, model, data)
     _dbg('timed loops done')
     lbs_ms = loop.lbs_ms(min(K, 50))
     blend_ms = loop.blend_ms()
@@ -731,30 +762,28 @@ def run_ours(args):
             peaks = json.load(open(os.path.join(REPO, 'MEASURED_PEAKS.json')))
         except Exception:
             pass
-        hbm_peak = peaks.get('hbm_gbs', 6650.0)
+        hbm_peak = peaks.get('hbm_gbs', 3350.0)
         alg_bytes = BYTES_CONST + n_local * BYTES_PER_FP
         achieved = alg_bytes / (lbs_ms * 1e-3) / 1e9
         fp32_tf = FLOPS_PER_FP * n_local / (lbs_ms * 1e-3) / 1e12
         fp32_exec = FLOPS_PER_FP_EXECUTED * n_local / (lbs_ms * 1e-3) / 1e12
         hbm_roofline = {'bound': 'hbm', 'kernel': 'LBS of the iteration: lbs_blend_tc_kernel (+ feature kernel) + lbs_skin_tc_kernel', 'achieved': achieved, 'peak': hbm_peak, 'unit': 'GB/s', 'frac': achieved / hbm_peak,
-                         'traffic': NCU_LBS_DRAM_BYTES.get(n_local), 'traffic_source': 'profiles/ (ncu --set full, dram__bytes_read + write, per launch)' if n_local in NCU_LBS_DRAM_BYTES else None,
-                         'peak_source': 'MEASURED_PEAKS.json hbm_gbs' if 'hbm_gbs' in peaks else 'fallback 6650 GB/s',
+                         'peak_source': 'MEASURED_PEAKS.json hbm_gbs' if 'hbm_gbs' in peaks else 'H100 SXM data sheet, 3350 GB/s',
                          'algorithmic_bytes': alg_bytes, 'kernel_ms': lbs_ms, 'kernel_share_of_step': lbs_ms / cold_ms,
                          'kernel_parts': {**lbs_parts,
                                           'note': 'kernel_ms = skinning (on the critical path) + blend timed in situ on its side stream, where it overlaps the other kernels of the evaluation, '
-                                                  'so kernel_share_of_step counts overlapped time; both with L2 flushed. traffic (ncu, cold) is 3.3x the algorithmic bytes: the 3xTF32 hi/lo '
-                                                  'constant image is 2 x 18.6 MB and v_posed makes one 25 MB round trip through L2/HBM between the two kernels; back-to-back iterations keep both in the 126 MB L2'},
+                                                  'so kernel_share_of_step counts overlapped time; both with L2 flushed. The 3xTF32 hi/lo constant image is 2 x 18.6 MB and v_posed '
+                                                  'makes one 25 MB round trip between the two kernels, together more than the 50 MB L2 of an H100 holds'},
                          'tensor': None if blend_ms is None else {
                              'kernel': 'blend_features_kernel + lbs_blend_tc_kernel launched alone (warm L2)', 'kernel_ms': blend_ms,
                              'achieved_tflops_tf32': 3 * 2 * 224 * 20736 * (-(-n_local // 128) * 128) / (blend_ms * 1e-3) / 1e12,
-                             'peak_tflops_tf32': peaks.get('bf16_tflops', 2250.0) / 2,
-                             'frac': 3 * 2 * 224 * 20736 * (-(-n_local // 128) * 128) / (blend_ms * 1e-3) / 1e12 / (peaks.get('bf16_tflops', 2250.0) / 2),
-                             'note': '3xTF32: three kind::tf32 MMAs per product; peak = half of the measured dense bf16 throughput (MEASURED_PEAKS.json); '
-                                     'ncu: sm__pipe_tensor_cycles_active 56.6 % of peak, 167 MB L2->SM per launch (profiles/lbs_tc_kernels_r02_final.md)'},
+                             'peak_tflops_tf32': peaks.get('bf16_tflops', 989.0) / 2,
+                             'frac': 3 * 2 * 224 * 20736 * (-(-n_local // 128) * 128) / (blend_ms * 1e-3) / 1e12 / (peaks.get('bf16_tflops', 989.0) / 2),
+                             'note': '3xTF32: three tf32 wgmma per product; peak = half of the dense bf16 throughput (MEASURED_PEAKS.json, else the H100 SXM data sheet at 700 W)'},
                          'fp32': {'achieved_tflops': fp32_tf, 'executed_tflops': fp32_exec, 'peak_tflops': fp32_peak, 'frac': fp32_tf / fp32_peak, 'frac_executed': fp32_exec / fp32_peak,
                                   'peak_source': 'glamr_fp32_probe: register-resident FFMA loop timed in this run (best of 5)',
                                   'note': 'algorithmic LBS flops (15.85 MFLOP per frame-person, dense skinning) over the LBS time (blend GEMM timed in situ on its side stream + skinning kernel) against the measured FP32 FFMA peak; '
-                                          'both LBS kernels run on the tensor cores now (3xTF32: the top-level roofline is the blend; the skinning is a K = 24 GEMM whose time is its TMEM epilogue and operand loads), so this FP32-FMA fraction is a comparison figure against the round-1 SIMT kernel, not a bound; the HBM fraction is small by construction (constants stay L2-resident)'}}
+                                          'both LBS kernels run on the tensor cores (3xTF32: the top-level roofline is the blend; the skinning is a K = 24 GEMM whose time is its epilogue and operand loads), so this FP32-FMA fraction is a comparison figure against the SIMT kernel, not a bound'}}
         tensor = hbm_roofline.pop('tensor')
         if tensor is not None:
             # the dominant kernel of the iteration is the tensor-core blend GEMM: quote the roofline against the tensor pipe.  Algorithmic flops =
@@ -766,12 +795,10 @@ def run_ours(args):
             ach = alg_flops / (tensor['kernel_ms'] * 1e-3) / 1e12
             roofline = {'bound': 'tensor', 'kernel': 'lbs_blend_tc_kernel (+ blend_features_kernel): the longest kernel of the iteration, launched alone (warm L2)',
                         'achieved': ach, 'peak': tf32_peak, 'unit': 'TFLOP/s', 'frac': ach / tf32_peak,
-                        'traffic': NCU_BLEND_DRAM_BYTES.get(n_local), 'traffic_source': 'profiles/lbs_tc_kernels_r02_final.md (ncu --set full, dram read + write of the blend kernel, cold)' if n_local in NCU_BLEND_DRAM_BYTES else None,
-                        'peak_source': ('MEASURED_PEAKS.json bf16_tflops / 2' if 'bf16_tflops' in peaks else 'fallback: nominal 2250 / 2') + ' = dense TF32',
+                        'peak_source': ('MEASURED_PEAKS.json bf16_tflops / 2' if 'bf16_tflops' in peaks else 'H100 SXM data sheet: 989 / 2') + ' = dense TF32',
                         'algorithmic_flops': alg_flops, 'kernel_ms': tensor['kernel_ms'],
                         'issued_tflops_tf32': tensor['achieved_tflops_tf32'], 'issued_frac': tensor['frac'],
-                        'note': 'frac = algorithmic blend flops / time / dense TF32 peak; issued_frac counts the three kind::tf32 MMAs per product (3xTF32) on 128 x 256 tiles '
-                                '(ncu: tensor pipe active 48 % of the cycles at 300 frames, 0.71 of peak issue at 1200 frames, profiles/chain_analysis_r02.md)',
+                        'note': 'frac = algorithmic blend flops / time / dense TF32 peak; issued_frac counts the three tf32 wgmma per product (3xTF32) on 128 x 256 tiles',
                         'hbm': hbm_roofline, 'fp32': hbm_roofline.pop('fp32'), 'kernel_parts': hbm_roofline.pop('kernel_parts')}
         else:
             roofline = hbm_roofline

@@ -1,4 +1,4 @@
-// Shared device/host helpers for the glamr_b200 CUDA library (sm_100a only).
+// Shared device/host helpers for the glamr_b200 CUDA library (sm_90a only).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -28,12 +28,12 @@
 #endif
 
 // Which implementation runs when the environment does not say otherwise.  A path becomes the default only after its parity
-// tests passed on a B200 (GLAMR_ITER_PATH=fused|legacy, GLAMR_LBS_PATH=tc|simt select explicitly for A/B runs).
+// tests passed on the GPU (GLAMR_ITER_PATH=fused|legacy, GLAMR_LBS_PATH=tc|simt select explicitly for A/B runs).
 #define GLAMR_DEFAULT_ITER_FUSED 0
-#define GLAMR_DEFAULT_LBS_TC 2        /* 2 = tensor-core blend + tensor-core skinning (verified on B200: all GPU tests green, memcheck clean), 1 = tensor-core blend + SIMT skinning, 0 = FP32 SIMT kernel */
-#define GLAMR_DEFAULT_BLEND_EARLY 0    /* 1: pipelined blend at the top of the evaluation into a second v_posed buffer -- measured slower (it takes the SMs the skinning needs: 98.8 vs 88.0 us at 1 x 300), kept selectable (GLAMR_BLEND_EARLY=1) */
+#define GLAMR_DEFAULT_LBS_TC 2        /* 2 = tensor-core blend + tensor-core skinning, 1 = tensor-core blend + SIMT skinning, 0 = FP32 SIMT kernel */
+#define GLAMR_DEFAULT_BLEND_EARLY 0    /* 1: pipelined blend at the top of the evaluation into a second v_posed buffer (GLAMR_BLEND_EARLY=1) */
 #define GLAMR_DEFAULT_BLEND_SPLIT 0    /* percent of the pipelined blend launched at the top of the evaluation (GLAMR_BLEND_SPLIT) */
-#define GLAMR_DEFAULT_SMEM_CARVEOUT 3   /* bit mask, see smem_carveout_mask() in smpl_kernels.cu: measured 193.0 -> 157.4 us per iteration at 4 x 300, neutral at 1 x 300 */
+#define GLAMR_DEFAULT_SMEM_CARVEOUT 3   /* bit mask, see smem_carveout_mask() in smpl_kernels.cu */
 #define GLAMR_DEFAULT_NET_WIMG 0       /* prior-network GEMMs: weight operand as a pre-split image fetched by bulk TMA (GLAMR_NET_WIMG=1) */
 
 namespace glamr {
@@ -53,17 +53,17 @@ constexpr int kNChunks = kPF / kChunkK;      // 23
 // k = 0..206 pose feature x posedirs, 207..216 betas x shapedirs, 217 = 1 x v_template, zero padded to 224
 constexpr int kTcFeat = kPF + kNB + 1;       // 218
 constexpr int kTcK = 224;                    // K padded to a multiple of the per-stage chunk
-constexpr int kTcChunkK = 8;                 // one tcgen05 kind::tf32 MMA step per pipeline stage
+constexpr int kTcChunkK = 8;                 // one wgmma tf32 step (k8) per pipeline stage
 constexpr int kTcChunks = kTcK / kTcChunkK;  // 28
-constexpr int kTcM = 128;                    // frames per CTA tile (= TMEM lanes)
-constexpr int kTcN = 256;                    // basis columns per CTA tile (= TMEM columns)
+constexpr int kTcM = 128;                    // frames per CTA tile (two consumer warpgroups of 64 rows)
+constexpr int kTcN = 256;                    // basis columns per CTA tile (wgmma N)
 constexpr int kTcNTiles = (kV * 3 + kTcN - 1) / kTcN;   // 81
 constexpr int kTcCols = kTcNTiles * kTcN;    // 20736
 constexpr int kTcAStageFloats = 2 * (kTcChunkK / 4) * kTcM * 4;   // hi | lo images of a [128 x 8] K-major core-matrix tile: 2048 floats
 constexpr int kTcBStageFloats = 2 * (kTcChunkK / 4) * kTcN * 4;   // 4096 floats
 // tensor-core skinning (lbs_skin_tc_kernel): T[vertex][frame x 12] = W[vertex][24 joints] . A[24 joints][frame x 12]
 constexpr int kSkF = 20;                     // frames per CTA tile
-constexpr int kSkN = kSkF * 12;              // 240 TMEM columns: the 3x4 blended transform of each frame
+constexpr int kSkN = kSkF * 12;              // 240 accumulator columns (wgmma N): the 3x4 blended transform of each frame
 constexpr int kSkKGroups = kNJ / 4;          // 6 groups of 4 joints (K = 24 = 3 MMA steps of 8)
 constexpr int kSkWHalf = kSkKGroups * kVTile * 4;     // 3072 floats: hi (or lo) image of a [128 vertices x 24] K-major tile
 constexpr int kSkWImageFloats = 2 * kSkWHalf;          // 6144 floats = 24,576 B per vertex tile
@@ -114,25 +114,101 @@ __device__ __forceinline__ void tma_bulk_g2s(void* smem_dst, const void* gsrc, u
 __device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
 __device__ __forceinline__ void pdl_launch_dependents() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
 
-// ---- tcgen05 (UMMA) helpers: shared-memory descriptor of a K-major, un-swizzled operand tile and one kind::tf32 MMA ----
-// rows = rows of the operand tile (128 for X, NT for W): fixes the leading byte offset between 16-byte K groups
-__device__ __forceinline__ uint64_t umma_desc_kmajor_noswizzle(const void* smem_ptr, int rows) {
-  // cute::UMMA::SmemDescriptor: start[0,14) | LBO[16,30) | SBO[32,46) | version=1 [46,48) | layout_type=0 [61,64)
+// ---- wgmma helpers: shared-memory descriptor of a K-major, un-swizzled operand tile and one m64nNk8 tf32 MMA --------
+// The operand tile is stored as 8-row x 16-byte core matrices: element (r, k) at ((k / 4) * rows + r) * 16 + (k % 4) * 4 bytes.
+// rows = rows of the whole stored tile (it fixes the leading byte offset between 16-byte K groups); a warpgroup's 64-row slice
+// starts 64 * 16 bytes further in.
+__device__ __forceinline__ uint64_t wgmma_desc_kmajor_noswizzle(const void* smem_ptr, int rows) {
+  // GMMA matrix descriptor: start[0,14) | LBO[16,30) | SBO[32,46) | base offset[49,52) = 0 | layout type[62,64) = 0 (no swizzle)
   const uint32_t addr = smem_u32(smem_ptr);
   uint64_t d = 0;
   d |= (uint64_t)((addr >> 4) & 0x3FFF);
   d |= (uint64_t)((rows * 16) >> 4) << 16;     // leading byte offset: next 16-byte K group
   d |= (uint64_t)(128 >> 4) << 32;             // stride byte offset: next 8-row group
-  d |= (uint64_t)1 << 46;                      // descriptor version (Blackwell)
   return d;
 }
-__device__ __forceinline__ void umma_tf32(uint32_t tmem_d, uint64_t da, uint64_t db, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n\t}\n" ::"r"(tmem_d),
-      "l"(da), "l"(db), "r"(idesc), "r"(accumulate)
-      : "memory");
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+// keeps the compiler from moving accesses of accumulator registers across wgmma issue / wait
+template <int R>
+__device__ __forceinline__ void wgmma_fence_acc(float (&d)[R]) {
+#pragma unroll
+  for (int i = 0; i < R; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
+// D[64 x N] (+)= A[64 x 8] B[N x 8]^T, both operands tf32 in shared memory.  Accumulator fragment of thread t of the warpgroup:
+// d[4 i + 2 h + e] = D[16 (t / 32) + (t % 32) / 4 + 8 h][8 i + 2 (t % 4) + e]
+__device__ __forceinline__ void wgmma_m64n32k8_tf32(float (&d)[16], uint64_t da, uint64_t db, uint32_t accumulate) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %18, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n32k8.f32.tf32.tf32 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, %16, %17, p, 1, 1;\n\t}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+        "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+      : "l"(da), "l"(db), "r"(accumulate));
+}
+__device__ __forceinline__ void wgmma_m64n128k8_tf32(float (&d)[64], uint64_t da, uint64_t db, uint32_t accumulate) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %66, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n128k8.f32.tf32.tf32 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, %64, %65, p, 1, 1;\n\t}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+        "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+        "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+        "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]),
+        "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]),
+        "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),
+        "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]),
+        "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+      : "l"(da), "l"(db), "r"(accumulate));
+}
+__device__ __forceinline__ void wgmma_m64n240k8_tf32(float (&d)[120], uint64_t da, uint64_t db, uint32_t accumulate) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %122, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n240k8.f32.tf32.tf32 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63, %64, %65, %66, %67, %68, %69, %70, %71, %72, %73, %74, %75, %76, %77, %78, %79, %80, %81, %82, %83, %84, %85, %86, %87, %88, %89, %90, %91, %92, %93, %94, %95, %96, %97, %98, %99, %100, %101, %102, %103, %104, %105, %106, %107, %108, %109, %110, %111, %112, %113, %114, %115, %116, %117, %118, %119}, %120, %121, p, 1, 1;\n\t}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+        "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+        "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+        "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]),
+        "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]),
+        "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),
+        "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]),
+        "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63]),
+        "+f"(d[64]), "+f"(d[65]), "+f"(d[66]), "+f"(d[67]), "+f"(d[68]), "+f"(d[69]), "+f"(d[70]), "+f"(d[71]),
+        "+f"(d[72]), "+f"(d[73]), "+f"(d[74]), "+f"(d[75]), "+f"(d[76]), "+f"(d[77]), "+f"(d[78]), "+f"(d[79]),
+        "+f"(d[80]), "+f"(d[81]), "+f"(d[82]), "+f"(d[83]), "+f"(d[84]), "+f"(d[85]), "+f"(d[86]), "+f"(d[87]),
+        "+f"(d[88]), "+f"(d[89]), "+f"(d[90]), "+f"(d[91]), "+f"(d[92]), "+f"(d[93]), "+f"(d[94]), "+f"(d[95]),
+        "+f"(d[96]), "+f"(d[97]), "+f"(d[98]), "+f"(d[99]), "+f"(d[100]), "+f"(d[101]), "+f"(d[102]), "+f"(d[103]),
+        "+f"(d[104]), "+f"(d[105]), "+f"(d[106]), "+f"(d[107]), "+f"(d[108]), "+f"(d[109]), "+f"(d[110]), "+f"(d[111]),
+        "+f"(d[112]), "+f"(d[113]), "+f"(d[114]), "+f"(d[115]), "+f"(d[116]), "+f"(d[117]), "+f"(d[118]), "+f"(d[119])
+      : "l"(da), "l"(db), "r"(accumulate));
+}
+__device__ __forceinline__ void wgmma_m64n256k8_tf32(float (&d)[128], uint64_t da, uint64_t db, uint32_t accumulate) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %130, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n256k8.f32.tf32.tf32 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63, %64, %65, %66, %67, %68, %69, %70, %71, %72, %73, %74, %75, %76, %77, %78, %79, %80, %81, %82, %83, %84, %85, %86, %87, %88, %89, %90, %91, %92, %93, %94, %95, %96, %97, %98, %99, %100, %101, %102, %103, %104, %105, %106, %107, %108, %109, %110, %111, %112, %113, %114, %115, %116, %117, %118, %119, %120, %121, %122, %123, %124, %125, %126, %127}, %128, %129, p, 1, 1;\n\t}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+        "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+        "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+        "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]),
+        "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]),
+        "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),
+        "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]),
+        "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63]),
+        "+f"(d[64]), "+f"(d[65]), "+f"(d[66]), "+f"(d[67]), "+f"(d[68]), "+f"(d[69]), "+f"(d[70]), "+f"(d[71]),
+        "+f"(d[72]), "+f"(d[73]), "+f"(d[74]), "+f"(d[75]), "+f"(d[76]), "+f"(d[77]), "+f"(d[78]), "+f"(d[79]),
+        "+f"(d[80]), "+f"(d[81]), "+f"(d[82]), "+f"(d[83]), "+f"(d[84]), "+f"(d[85]), "+f"(d[86]), "+f"(d[87]),
+        "+f"(d[88]), "+f"(d[89]), "+f"(d[90]), "+f"(d[91]), "+f"(d[92]), "+f"(d[93]), "+f"(d[94]), "+f"(d[95]),
+        "+f"(d[96]), "+f"(d[97]), "+f"(d[98]), "+f"(d[99]), "+f"(d[100]), "+f"(d[101]), "+f"(d[102]), "+f"(d[103]),
+        "+f"(d[104]), "+f"(d[105]), "+f"(d[106]), "+f"(d[107]), "+f"(d[108]), "+f"(d[109]), "+f"(d[110]), "+f"(d[111]),
+        "+f"(d[112]), "+f"(d[113]), "+f"(d[114]), "+f"(d[115]), "+f"(d[116]), "+f"(d[117]), "+f"(d[118]), "+f"(d[119]),
+        "+f"(d[120]), "+f"(d[121]), "+f"(d[122]), "+f"(d[123]), "+f"(d[124]), "+f"(d[125]), "+f"(d[126]), "+f"(d[127])
+      : "l"(da), "l"(db), "r"(accumulate));
+}
+
 
 // x = hi + lo with hi = tf32(x), lo = tf32(x - hi): the operands of the 3xTF32 tensor-core products (hi*hi + lo*hi + hi*lo)
 __device__ __forceinline__ void split_tf32(float x, float& hi, float& lo) {

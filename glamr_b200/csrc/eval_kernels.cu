@@ -1,6 +1,6 @@
 // Evaluation kernels (global_recon/utils/evaluator.py:202-327): sparse joint regression from the skinned vertices
 // (evaluator.py:263,306  joint_h36m = J_regressor @ vertices) and the per-frame similarity Procrustes alignment
-// (lib/utils/torch_transform.py:282-345 batch_compute_similarity_transform_torch).  sm_100a.
+// (lib/utils/torch_transform.py:282-345 batch_compute_similarity_transform_torch).  sm_90a.
 #include <math.h>
 
 #include "common.cuh"

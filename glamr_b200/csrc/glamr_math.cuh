@@ -5,7 +5,7 @@
 //
 // The header is plain C++ (no CUDA intrinsics) so that tests/host_harness can compile the very same code with
 // g++ and check each primitive against torch autograd on the CPU-only build box; the product only ever runs it
-// inside the sm_100a kernels of this directory.
+// inside the sm_90a kernels of this directory.
 #pragma once
 #include <math.h>
 

@@ -1,4 +1,4 @@
-// One global-optimisation iteration of GLAMR on sm_100a (global_recon/models/global_recon_model.py:547-570):
+// One global-optimisation iteration of GLAMR on sm_90a (global_recon/models/global_recon_model.py:547-570):
 //   traj_forward    (1 CTA / person: trajectory codec with two block-wide prefix scans)
 //   cam_forward     (1 thread / frame)
 //   pose_prep + lbs + joints_finalize   (smpl_kernels.cu: the full SMPL evaluation for every frame-person)
@@ -733,10 +733,10 @@ extern "C" int glamr_opt_create(glamr_opt_t** out, const glamr_smpl_t* smpl, con
     if (st->blend_split < 0 || st->blend_split > 100) st->blend_split = 0;
     // GLAMR_FEATURES_EARLY=0|1: the feature kernel of the pipelined blend (its A operand; body pose / betas only) runs at the top of the
     // evaluation on the side stream, so that only the GEMM is left after the skinning
-    // (default: only while this rank's per-frame kernels have fewer CTAs than the GPU has SMs -- measured 102.8 -> 94.8 us per L2-flushed
-    // iteration at 1 x 300, but 154 -> 180 us at 4 x 300, where the GEMM then no longer follows a kernel with its own shared-memory split)
+    // (default: only while this rank's per-frame kernels have fewer CTAs than the GPU has SMs; with more, the GEMM would no longer
+    // follow a kernel with its own shared-memory split)
     const char* fe = getenv("GLAMR_FEATURES_EARLY");
-    int sms = 148, dev = 0;
+    int sms = 132, dev = 0;
     cudaGetDevice(&dev);
     cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
     const int frame_ctas = (pb->n_end - pb->n_begin + kFrameThreads / 32 - 1) / (kFrameThreads / 32);

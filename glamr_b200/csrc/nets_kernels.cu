@@ -1,8 +1,8 @@
-// Learned-prior inference on sm_100a: the motion infiller (CVAE, transformer encoder/decoder over 50-frame windows,
+// Learned-prior inference on sm_90a: the motion infiller (CVAE, transformer encoder/decoder over 50-frame windows,
 // motion_infiller/models/motion_infiller_vae.py:22-123,252-421,564-632) and the trajectory predictor (CVAE, MLP +
 // 2-layer bidirectional LSTM, traj_pred/models/traj_pred_vae.py:20-92,202-333; lib/models/{mlp,rnn,pos_encoding}.py).
-// Every Linear (QKV / out-proj / FFN / MLP / LSTM input projections) runs on the tensor cores: tcgen05.mma kind::tf32
-// with a 3xTF32 split and the accumulator in TMEM (gemm_tf32x3_tcgen05_kernel); LayerNorm, softmax attention (S <= 64,
+// Every Linear (QKV / out-proj / FFN / MLP / LSTM input projections) runs on the tensor cores: wgmma.mma_async tf32
+// with a 3xTF32 split and the accumulator in registers (gemm_tf32x3_wgmma_kernel); LayerNorm, softmax attention (S <= 64,
 // shared memory) and the LSTM recurrence (W_hh resident in registers + shared memory for the whole sequence) are FP32
 // SIMT kernels.  Outputs match the reference's fp32 networks to <= 1e-4 (tests/golden/nets.npz).
 // Weights are addressed by their reference state-dict names so Lightning checkpoints map 1:1.
@@ -75,16 +75,15 @@ __global__ void __launch_bounds__(256) gemm_bias_act_kernel(int M, int N, int K,
   }
 }
 
-// ------------------------------------------------------------------------------------------------ tcgen05 GEMM (3xTF32)
-// Y = act(X W^T + b) on the 5th-generation tensor cores: tcgen05.mma.kind::tf32 with the accumulator in TMEM.
+// ------------------------------------------------------------------------------------------------ wgmma GEMM (3xTF32)
+// Y = act(X W^T + b) on the Hopper tensor cores: wgmma.mma_async tf32 with the accumulator in registers.
 // FP32 accuracy is kept with the 3xTF32 split  x = hi + lo (hi = tf32(x), lo = tf32(x - hi)):
 //   X W^T ~= Xhi Whi^T + Xlo Whi^T + Xhi Wlo^T     (error ~2^-21 relative: the 1e-4 parity bar of the infilled pose holds)
-// CTA = 128 threads, tile 128 (M) x 128 (N), K step 32.  Both operands are K-major (X [M,K] and W [N,K] row-major), written
-// by the CTA into shared memory in the canonical no-swizzle UMMA layout (8-row x 16-byte core matrices: element (r,k) at
-// ((k/4)*128 + r)*16 + (k%4)*4 bytes => LBO = 2048 B between K groups, SBO = 128 B between 8-row groups), made visible to
-// the async proxy with fence.proxy.async, multiplied by one elected thread (12 MMAs per K step), completion tracked with
-// tcgen05.commit -> mbarrier; the epilogue reads the 128x128 fp32 accumulator with tcgen05.ld (32x32b.x32), adds the
-// bias, applies the activation and stores.
+// CTA = 256 threads = two warpgroups, tile 128 (M) x NT (N), K step 32; warpgroup g computes rows 64 g .. 64 g + 63 (m64nNTk8).
+// Both operands are K-major (X [M,K] and W [N,K] row-major), written by the CTA into shared memory in the canonical no-swizzle
+// layout (8-row x 16-byte core matrices: element (r,k) at ((k/4)*128 + r)*16 + (k%4)*4 bytes => LBO = 2048 B between K groups,
+// SBO = 128 B between 8-row groups) and made visible to the async proxy with fence.proxy.async; the epilogue adds the bias to the
+// accumulator fragment, applies the activation and stores.
 constexpr int TCM = 128, TCK = 32;                              // N tile (NT) is a template parameter: 128, or 32 for one-tile-high problems
 constexpr int kTcATileFloats = TCM * TCK;                       // 4096 floats = 16 KB (hi or lo of the X tile)
 
@@ -105,7 +104,7 @@ struct TcCfg {
   static constexpr int kStageFloats = 2 * kTcATileFloats + 2 * kBTileFloats;            // Xhi | Xlo | Whi | Wlo
   static constexpr int kXVec = (TCM * TCK / 4) / kTcThreads;                            // 16-byte loads per thread and K step
   static constexpr int kWVec = (NT * TCK / 4) / kTcThreads;
-  static constexpr size_t kSmemBytes = (size_t)kTcStages * kStageFloats * sizeof(float) + 64;
+  static constexpr size_t kSmemBytes = (size_t)kTcStages * kStageFloats * sizeof(float) + 16;
   static_assert(kWVec >= 1, "W tile smaller than one 16-byte load per thread");
 };
 
@@ -141,7 +140,7 @@ __device__ __forceinline__ void tc_load_tiles(TcRegs<NT>& r, int tid, int M, int
     }
   }
 }
-// split into tf32 hi / lo and store as K-major 8x16-byte core matrices (the layout umma_desc_kmajor_noswizzle describes)
+// split into tf32 hi / lo and store as K-major 8x16-byte core matrices (the layout wgmma_desc_kmajor_noswizzle describes)
 template <int NT, bool WIMG = false>
 __device__ __forceinline__ void tc_store_tiles(float* st, int tid, const TcRegs<NT>& r) {
   float* Ahi = st;
@@ -193,35 +192,34 @@ __global__ void build_w_image_kernel(const float* __restrict__ W, int N, int K, 
   }
 }
 
-// 256 threads; two shared-memory stages: while the tensor core works on stage s (12 UTCHMMA per K step, tracked by
-// tcgen05.commit -> mbarrier[s]) all threads split and store K step it+1 into stage s^1 and already have the global
-// loads of step it+2 in flight in registers, so the L2 latency never sits on the critical path of these small GEMMs.
-// NT = 128: 128x128 tiles (one CTA per SM).  NT = 32: 128x32 tiles for problems one tile high (M <= 128, a single
-// 120-frame window): 4x more CTAs, each with a quarter of the W traffic, split work and epilogue.
+// 256 threads; two shared-memory stages: while the tensor core works on stage s (12 wgmma per K step and warpgroup, one commit
+// group) all threads split and store K step it+1 into stage s^1 and already have the global loads of step it+2 in flight in
+// registers, so the L2 latency never sits on the critical path of these small GEMMs.
+// NT = 128: 128x128 tiles.  NT = 32: 128x32 tiles for problems one tile high (M <= 128, a single 120-frame window): 4x more
+// CTAs, each with a quarter of the W traffic, split work and epilogue.
 // WIMG: W points at the pre-split operand image of the weight (build_w_image_kernel) and arrives by bulk TMA (wbar[s]).
+template <int NT>
+__device__ __forceinline__ void wgmma_tf32_nt(float (&d)[NT / 2], uint64_t da, uint64_t db, uint32_t accumulate) {
+  if constexpr (NT == 128) wgmma_m64n128k8_tf32(d, da, db, accumulate);
+  else wgmma_m64n32k8_tf32(d, da, db, accumulate);
+}
 template <int ACT, bool VEC, int NT, bool WIMG>
-__global__ void __launch_bounds__(kTcThreads) gemm_tf32x3_tcgen05_kernel(int M, int N, int K, const float* __restrict__ X, int ldx,
-                                                                         const float* __restrict__ W, const float* __restrict__ bias,
-                                                                         const float* __restrict__ bias2, float* __restrict__ Y, int ldy) {
+__global__ void __launch_bounds__(kTcThreads) gemm_tf32x3_wgmma_kernel(int M, int N, int K, const float* __restrict__ X, int ldx,
+                                                                       const float* __restrict__ W, const float* __restrict__ bias,
+                                                                       const float* __restrict__ bias2, float* __restrict__ Y, int ldy) {
+  static_assert(NT == 128 || NT == 32, "N tile");
   using Cfg = TcCfg<NT>;
   extern __shared__ __align__(128) unsigned char tc_smem[];
   float* stage0 = reinterpret_cast<float*>(tc_smem);
-  uint64_t* bar = reinterpret_cast<uint64_t*>(stage0 + kTcStages * Cfg::kStageFloats);   // [2] MMA completion per stage
-  uint64_t* wbar = bar + 2;                                                              // [2] weight image landed (WIMG)
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(wbar + 2);
+  uint64_t* wbar = reinterpret_cast<uint64_t*>(stage0 + kTcStages * Cfg::kStageFloats);   // [2] weight image landed (WIMG)
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+  const int g = warp >> 2;                                                                // warpgroup: rows 64 g .. 64 g + 63
   const int m0 = blockIdx.y * TCM, n0 = blockIdx.x * NT;
 
-  if (warp == 0) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)), "r"(NT));
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::);
-  }
   const int nk = (K + TCK - 1) / TCK;
   constexpr uint32_t kWBytes = 2 * Cfg::kBTileFloats * sizeof(float);
   const float* wimg = W + (size_t)blockIdx.x * nk * (2 * Cfg::kBTileFloats);            // this column tile's K steps, contiguous
   if (tid == 0) {
-    mbar_init(&bar[0], 1);
-    mbar_init(&bar[1], 1);
     mbar_init(&wbar[0], 1);
     mbar_init(&wbar[1], 1);
     mbar_fence_init();
@@ -236,34 +234,31 @@ __global__ void __launch_bounds__(kTcThreads) gemm_tf32x3_tcgen05_kernel(int M, 
   tc_store_tiles<NT, WIMG>(stage0, tid, regs);
   if (nk > 1) tc_load_tiles<NT, VEC, WIMG>(regs, tid, M, N, K, X, ldx, W, m0, n0, TCK);
   asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // generic-proxy smem writes -> visible to the tensor core
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
   __syncthreads();
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-  const uint32_t tmem_d = *tmem_slot;
-  // instruction descriptor (cute::UMMA::InstrDescriptor): D=F32 [4,6)=1, A=TF32 [7,10)=2, B=TF32 [10,13)=2, K-major A/B, N>>3 [17,23), M>>4 [24,29)
-  const uint32_t idesc = (1u << 4) | (2u << 7) | (2u << 10) | ((uint32_t)(NT >> 3) << 17) | ((uint32_t)(TCM >> 4) << 24);
 
+  float acc[NT / 2];
+#pragma unroll
+  for (int i = 0; i < NT / 2; ++i) acc[i] = 0.0f;
   for (int it = 0; it < nk; ++it) {
     const int s = it & 1;
     float* st = stage0 + s * Cfg::kStageFloats;
-    if (tid == 0) {
-      if (WIMG) mbar_wait(&wbar[s], (it >> 1) & 1);                       // this stage's weight image has landed
+    if (WIMG) mbar_wait(&wbar[s], (it >> 1) & 1);                         // this stage's weight image has landed
+    wgmma_fence();
 #pragma unroll
-      for (int k8 = 0; k8 < ((dbg & 1) ? 0 : TCK / 8); ++k8) {           // one tf32 MMA consumes K = 8 (two 16-byte K groups)
-        const size_t koa = (size_t)k8 * 2 * TCM * 4, kob = (size_t)k8 * 2 * NT * 4;   // floats
-        const uint64_t dah = umma_desc_kmajor_noswizzle(st + koa, TCM), dal = umma_desc_kmajor_noswizzle(st + kTcATileFloats + koa, TCM);
-        const uint64_t dbh = umma_desc_kmajor_noswizzle(st + 2 * kTcATileFloats + kob, NT);
-        const uint64_t dbl = umma_desc_kmajor_noswizzle(st + 2 * kTcATileFloats + Cfg::kBTileFloats + kob, NT);
-        umma_tf32(tmem_d, dah, dbh, idesc, (it > 0 || k8 > 0) ? 1u : 0u);
-        umma_tf32(tmem_d, dal, dbh, idesc, 1u);
-        umma_tf32(tmem_d, dah, dbl, idesc, 1u);
-      }
-      // arrive on mbarrier[s] when every MMA issued so far has completed (implies fence::before_thread_sync)
-      asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(&bar[s])) : "memory");
+    for (int k8 = 0; k8 < ((dbg & 1) ? 0 : TCK / 8); ++k8) {             // one tf32 wgmma consumes K = 8 (two 16-byte K groups)
+      const size_t koa = (size_t)k8 * 2 * TCM * 4 + g * 64 * 4, kob = (size_t)k8 * 2 * NT * 4;   // floats
+      const uint64_t dah = wgmma_desc_kmajor_noswizzle(st + koa, TCM), dal = wgmma_desc_kmajor_noswizzle(st + kTcATileFloats + koa, TCM);
+      const uint64_t dbh = wgmma_desc_kmajor_noswizzle(st + 2 * kTcATileFloats + kob, NT);
+      const uint64_t dbl = wgmma_desc_kmajor_noswizzle(st + 2 * kTcATileFloats + Cfg::kBTileFloats + kob, NT);
+      wgmma_tf32_nt<NT>(acc, dah, dbh, (it > 0 || k8 > 0) ? 1u : 0u);
+      wgmma_tf32_nt<NT>(acc, dal, dbh, 1u);
+      wgmma_tf32_nt<NT>(acc, dah, dbl, 1u);
     }
+    wgmma_commit();
     if (it + 1 < nk) {
-      // stage s^1 was consumed by the MMAs of step it-1: wait for their commit, then refill it while step `it` computes
-      if (it >= 1) mbar_wait(&bar[s ^ 1], ((it - 1) >> 1) & 1);
+      // stage s^1 was read by both warpgroups' wgmmas of step it-1: retire them, then refill it while step `it` computes
+      wgmma_wait<1>();
+      __syncthreads();
       if (WIMG && tid == 0) {                                            // stage s^1 is free: fetch the weight image of step it+1
         mbar_expect_tx(&wbar[s ^ 1], kWBytes);
         tma_bulk_g2s(stage0 + (s ^ 1) * Cfg::kStageFloats + 2 * kTcATileFloats, wimg + (size_t)(it + 1) * (2 * Cfg::kBTileFloats), kWBytes, &wbar[s ^ 1]);
@@ -274,69 +269,39 @@ __global__ void __launch_bounds__(kTcThreads) gemm_tf32x3_tcgen05_kernel(int M, 
       __syncthreads();
     }
   }
-  mbar_wait(&bar[(nk - 1) & 1], ((nk - 1) >> 1) & 1);      // all MMAs done: the accumulator is final
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
+  wgmma_wait<0>();                                         // all wgmmas done: the accumulator is final
+  wgmma_fence_acc(acc);
 
-  // ---- epilogue: a warp may read TMEM lanes (= rows) 32 (w % 4) .. +31; 32-column chunks alternate between warps 0-3 and 4-7
+  // ---- epilogue: acc[4 i + 2 h + e] = Y[m0 + 64 g + 16 (warp % 4) + lane / 4 + 8 h][n0 + 8 i + 2 (lane % 4) + e]
   if (!(dbg & 4)) {
-    const int wq = warp & 3, wh = warp >> 2;
-    const int m = m0 + wq * 32 + lane;
-#pragma unroll 1
-    for (int cc = wh; cc < NT / 32; cc += 2) {
-      if (n0 + cc * 32 >= N) break;
-      uint32_t v[32];
-      const uint32_t taddr = tmem_d + ((uint32_t)(wq * 32) << 16) + (uint32_t)(cc * 32);
-      asm volatile(
-          "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-          "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, "
-          "%28, %29, %30, %31}, [%32];\n"
-          : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]), "=r"(v[8]), "=r"(v[9]), "=r"(v[10]),
-            "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15]), "=r"(v[16]), "=r"(v[17]), "=r"(v[18]), "=r"(v[19]), "=r"(v[20]),
-            "=r"(v[21]), "=r"(v[22]), "=r"(v[23]), "=r"(v[24]), "=r"(v[25]), "=r"(v[26]), "=r"(v[27]), "=r"(v[28]), "=r"(v[29]), "=r"(v[30]),
-            "=r"(v[31])
-          : "r"(taddr));
-      asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-      const int nb = n0 + cc * 32;
-      if (m < M && nb + 32 <= N && (ldy & 3) == 0 && (reinterpret_cast<uintptr_t>(Y) & 15) == 0) {
-        float4* yrow = reinterpret_cast<float4*>(Y + (size_t)m * ldy + nb);          // this lane's 128 contiguous bytes
-        const bool bvec = ((reinterpret_cast<uintptr_t>(bias) | reinterpret_cast<uintptr_t>(bias2)) & 15) == 0 && (nb & 3) == 0;
+    const bool yvec = (ldy & 1) == 0 && (reinterpret_cast<uintptr_t>(Y) & 7) == 0;
 #pragma unroll
-        for (int j = 0; j < 32; j += 4) {
-          float bsum[4] = {0.f, 0.f, 0.f, 0.f};
-          if (bvec) {
-            if (bias) { const float4 t = __ldg(reinterpret_cast<const float4*>(bias + nb + j)); bsum[0] += t.x; bsum[1] += t.y; bsum[2] += t.z; bsum[3] += t.w; }
-            if (bias2) { const float4 t = __ldg(reinterpret_cast<const float4*>(bias2 + nb + j)); bsum[0] += t.x; bsum[1] += t.y; bsum[2] += t.z; bsum[3] += t.w; }
-          } else {
+    for (int i = 0; i < NT / 8; ++i) {
+      const int n = n0 + 8 * i + 2 * (lane & 3);
+      if (n >= N) continue;
+      const bool pair = n + 1 < N;
+      float b0 = 0.0f, b1 = 0.0f;
+      if (bias) { b0 += __ldg(bias + n); if (pair) b1 += __ldg(bias + n + 1); }
+      if (bias2) { b0 += __ldg(bias2 + n); if (pair) b1 += __ldg(bias2 + n + 1); }
 #pragma unroll
-            for (int q = 0; q < 4; ++q) bsum[q] = (bias ? __ldg(bias + nb + j + q) : 0.0f) + (bias2 ? __ldg(bias2 + nb + j + q) : 0.0f);
-          }
-          float o[4];
-#pragma unroll
-          for (int q = 0; q < 4; ++q) {
-            o[q] = __uint_as_float(v[j + q]) + bsum[q];
-            if (ACT == 1) o[q] = fmaxf(o[q], 0.0f);
-          }
-          yrow[j >> 2] = make_float4(o[0], o[1], o[2], o[3]);
-        }
-      } else if (m < M) {
-#pragma unroll
-        for (int j = 0; j < 32; ++j) {
-          const int n = nb + j;
-          if (n < N) {
-            float o = __uint_as_float(v[j]) + (bias ? bias[n] : 0.0f) + (bias2 ? bias2[n] : 0.0f);
-            if (ACT == 1) o = fmaxf(o, 0.0f);
-            Y[(size_t)m * ldy + n] = o;
-          }
+      for (int h = 0; h < 2; ++h) {
+        const int m = m0 + g * 64 + (warp & 3) * 16 + (lane >> 2) + 8 * h;
+        if (m >= M) continue;
+        float o0 = acc[4 * i + 2 * h] + b0, o1 = acc[4 * i + 2 * h + 1] + b1;
+        if (ACT == 1) { o0 = fmaxf(o0, 0.0f); o1 = fmaxf(o1, 0.0f); }
+        float* y = Y + (size_t)m * ldy + n;
+        if (pair && yvec) {
+          *reinterpret_cast<float2*>(y) = make_float2(o0, o1);
+        } else {
+          y[0] = o0;
+          if (pair) y[1] = o1;
         }
       }
     }
   }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-  __syncthreads();
-  if (warp == 0) asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_d), "r"(NT));
 }
 
-static int g_gemm_mode = 1;   // 1 = tcgen05 3xTF32 for the transformer (default), 0 = FP32 SIMT everywhere (A/B verification)
+static int g_gemm_mode = 1;   // 1 = wgmma 3xTF32 for the transformer (default), 0 = FP32 SIMT everywhere (A/B verification)
 // The trajectory predictor (MLP + LSTM, M = T*B rows, outputs integrated over T frames by the trajectory codec) stays on the
 // FP32 SIMT GEMM: its matrices are launch-latency sized and its per-frame heading error accumulates through the prefix sum.
 struct ScopedFp32Gemm {
@@ -368,7 +333,7 @@ static int wimg_get(cudaStream_t s, const float* W, int N, int K, const float** 
   float* img = nullptr;
   GLAMR_CUDA_TRY(cudaMalloc(&img, (size_t)tiles * ksteps * 2 * TcCfg<NT>::kBTileFloats * sizeof(float)));
   const size_t total = (size_t)tiles * ksteps * NT * TCK;
-  build_w_image_kernel<NT><<<(unsigned)((total + 255) / 256 < 1184 ? (total + 255) / 256 : 1184), 256, 0, s>>>(W, N, K, ksteps, img);
+  build_w_image_kernel<NT><<<(unsigned)((total + 255) / 256 < 1056 ? (total + 255) / 256 : 1056), 256, 0, s>>>(W, N, K, ksteps, img);
   GLAMR_LAUNCH_CHECK();
   g_wimg[key] = img;
   *out = img;
@@ -381,14 +346,14 @@ static int gemm_tc_launch(cudaStream_t s, int M, int N, int K, const float* X, i
   static bool attr = false;
   constexpr size_t smem = TcCfg<NT>::kSmemBytes;
   if (!attr) {
-    GLAMR_CUDA_TRY(cudaFuncSetAttribute(gemm_tf32x3_tcgen05_kernel<0, true, NT, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    GLAMR_CUDA_TRY(cudaFuncSetAttribute(gemm_tf32x3_tcgen05_kernel<1, true, NT, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    GLAMR_CUDA_TRY(cudaFuncSetAttribute(gemm_tf32x3_tcgen05_kernel<0, false, NT, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    GLAMR_CUDA_TRY(cudaFuncSetAttribute(gemm_tf32x3_tcgen05_kernel<1, false, NT, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    GLAMR_CUDA_TRY(cudaFuncSetAttribute(gemm_tf32x3_tcgen05_kernel<0, true, NT, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    GLAMR_CUDA_TRY(cudaFuncSetAttribute(gemm_tf32x3_tcgen05_kernel<1, true, NT, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    GLAMR_CUDA_TRY(cudaFuncSetAttribute(gemm_tf32x3_tcgen05_kernel<0, false, NT, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    GLAMR_CUDA_TRY(cudaFuncSetAttribute(gemm_tf32x3_tcgen05_kernel<1, false, NT, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    GLAMR_CUDA_TRY(cudaFuncSetAttribute(gemm_tf32x3_wgmma_kernel<0, true, NT, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    GLAMR_CUDA_TRY(cudaFuncSetAttribute(gemm_tf32x3_wgmma_kernel<1, true, NT, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    GLAMR_CUDA_TRY(cudaFuncSetAttribute(gemm_tf32x3_wgmma_kernel<0, false, NT, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    GLAMR_CUDA_TRY(cudaFuncSetAttribute(gemm_tf32x3_wgmma_kernel<1, false, NT, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    GLAMR_CUDA_TRY(cudaFuncSetAttribute(gemm_tf32x3_wgmma_kernel<0, true, NT, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    GLAMR_CUDA_TRY(cudaFuncSetAttribute(gemm_tf32x3_wgmma_kernel<1, true, NT, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    GLAMR_CUDA_TRY(cudaFuncSetAttribute(gemm_tf32x3_wgmma_kernel<0, false, NT, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    GLAMR_CUDA_TRY(cudaFuncSetAttribute(gemm_tf32x3_wgmma_kernel<1, false, NT, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     attr = true;
   }
   if (g_wimg_enabled < 0) {
@@ -407,12 +372,12 @@ static int gemm_tc_launch(cudaStream_t s, int M, int N, int K, const float* X, i
   };
   if (img) {
     const bool xvec = (K % 4 == 0) && (ldx % 4 == 0) && ((uintptr_t)X % 16 == 0);
-    if (xvec) { if (act == 1) go(gemm_tf32x3_tcgen05_kernel<1, true, NT, true>, img); else go(gemm_tf32x3_tcgen05_kernel<0, true, NT, true>, img); }
-    else { if (act == 1) go(gemm_tf32x3_tcgen05_kernel<1, false, NT, true>, img); else go(gemm_tf32x3_tcgen05_kernel<0, false, NT, true>, img); }
+    if (xvec) { if (act == 1) go(gemm_tf32x3_wgmma_kernel<1, true, NT, true>, img); else go(gemm_tf32x3_wgmma_kernel<0, true, NT, true>, img); }
+    else { if (act == 1) go(gemm_tf32x3_wgmma_kernel<1, false, NT, true>, img); else go(gemm_tf32x3_wgmma_kernel<0, false, NT, true>, img); }
   } else if (vec) {
-    if (act == 1) go(gemm_tf32x3_tcgen05_kernel<1, true, NT, false>, W); else go(gemm_tf32x3_tcgen05_kernel<0, true, NT, false>, W);
+    if (act == 1) go(gemm_tf32x3_wgmma_kernel<1, true, NT, false>, W); else go(gemm_tf32x3_wgmma_kernel<0, true, NT, false>, W);
   } else {
-    if (act == 1) go(gemm_tf32x3_tcgen05_kernel<1, false, NT, false>, W); else go(gemm_tf32x3_tcgen05_kernel<0, false, NT, false>, W);
+    if (act == 1) go(gemm_tf32x3_wgmma_kernel<1, false, NT, false>, W); else go(gemm_tf32x3_wgmma_kernel<0, false, NT, false>, W);
   }
   GLAMR_LAUNCH_CHECK();
   return GLAMR_OK;
@@ -424,8 +389,8 @@ static int gemm_tc_launch(cudaStream_t s, int M, int N, int K, const float* X, i
 // in dependent order per sequence, so the figure of merit is the LATENCY of one launch, not its throughput.  One warp owns an
 // 8 x 4 output tile and splits K across its lanes: every lane issues all its 16-byte loads of the 8 X rows and 4 W rows at once
 // (no shared memory, no block barrier, one global round trip), accumulates 32 partial dot products in FP32 and the warp folds
-// them with a 31-shuffle transpose-reduction that leaves output (r, c) on lane 4 r + c.  ~2 us per launch against ~12 us for the
-// one-tile tcgen05 kernel at M = 50 (profiles/init_breakdown_r02d_p1.txt), exact FP32 FMA arithmetic.
+// them with a 31-shuffle transpose-reduction that leaves output (r, c) on lane 4 r + c: one launch of a few us instead of the
+// one-tile tensor-core kernel's staged pipeline, exact FP32 FMA arithmetic.
 constexpr int kSkinnyMaxM = 256;
 template <int ACT, bool VEC>
 __global__ void __launch_bounds__(128) gemm_skinny_kernel(int M, int N, int K, const float* __restrict__ X, int ldx, const float* __restrict__ W,
@@ -868,7 +833,7 @@ int decoder_layer(cudaStream_t s, Arena& A, const DecLayer& L, int B, int S, int
 }  // namespace
 
 // Y[M,N] = act(X[M,K] W[N,K]^T + bias) -- stand-alone entry for the GEMM used by every Linear of the prior networks
-// (nn.Linear in lib/models/mlp.py:32-41, nn.MultiheadAttention projections, FFN).  mode: 1 tcgen05 3xTF32, 0 FP32 SIMT.
+// (nn.Linear in lib/models/mlp.py:32-41, nn.MultiheadAttention projections, FFN).  mode: 1 wgmma 3xTF32, 0 FP32 SIMT.
 extern "C" int glamr_linear_forward(int M, int N, int K, const float* X, const float* W, const float* bias, int relu, float* Y, int mode,
                                     void* stream) {
   if (M <= 0 || N <= 0 || K <= 0 || !X || !W || !Y) return GLAMR_EINVAL;

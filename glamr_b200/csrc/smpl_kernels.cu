@@ -1,4 +1,4 @@
-// SMPL forward on sm_100a: Rodrigues + kinematic chain (pose_prep), blend shapes + pose blend + linear blend skinning
+// SMPL forward on sm_90a: Rodrigues + kinematic chain (pose_prep), blend shapes + pose blend + linear blend skinning
 // (lbs_kernel: 1-D bulk-TMA / mbarrier double-buffered posedirs slabs, FP32 FMA, K-sparse skinning), extra joint
 // regression + joint remap + re-rooting (joints_finalize).  Reference arithmetic: smplx.lbs as stated in-tree at
 // HybrIK/hybrik/models/layers/smpl/lbs.py:195-288,402-548 and GLAMR's wrapper lib/models/smpl.py:289-343.
@@ -37,7 +37,7 @@ __global__ void __launch_bounds__(128) pose_prep_kernel(SmplDev m, int n, const 
 // Why this shape: the kernel is shared-memory-bandwidth bound unless the register tile is large.  Per k a thread reads
 // 12 posedirs values (3 LDS.128, distinct per lane) + 8 pose-feature values (2 LDS.128, warp-broadcast) = 20 wavefronts
 // per warp for 96 FFMA (0.21 wavefronts/FFMA, below the 0.25 the LSU can sustain next to 4 FFMA/clk); the first
-// version (3 x 16 tile) needed 19 wavefronts per 48 FFMA and stalled on the LSU (profiles/lbs_kernel_r01.md).
+// version (3 x 16 tile) needed 19 wavefronts per 48 FFMA and stalled on the LSU.
 // All operands arrive by 1-D bulk TMA (cp.async.bulk + mbarrier): the CTA's posedirs slab [207][384] in 23 chunks of
 // 9 rows (13,824 B contiguous thanks to the tile-major re-layout), the matching [9][32] pose-feature chunk, and the
 // A tile [24][32][12]; a 3-stage full/empty mbarrier ring replaces __syncthreads in the main loop.
@@ -299,7 +299,7 @@ lbs_kernel(SmplDev m, int n_begin, int n_end, const float* __restrict__ betas, S
 
 // ------------------------------------------------------------------------------------------------ blend features
 // The A operand of the blend GEMM for frame-person f: (R_j - I) of the 23 body joints (lbs.py:256-258), the betas, the constant 1
-// that multiplies v_template and zero padding, as tf32 hi / lo in the UMMA image (see pose_prep_frame).  It depends on the body
+// that multiplies v_template and zero padding, as tf32 hi / lo in the wgmma image (see pose_prep_frame).  It depends on the body
 // pose and the betas only -- NOT on the root orientation -- so the optimiser evaluates it (and the blend GEMM behind it) off the
 // critical path of the iteration.  One warp per frame-person.
 __global__ void __launch_bounds__(128) blend_features_kernel(int n, const float* __restrict__ body_pose, const float* __restrict__ betas, SmplWorkspace w) {
@@ -333,47 +333,37 @@ __global__ void __launch_bounds__(128) blend_features_kernel(int n, const float*
 // ------------------------------------------------------------------------------------------------ tensor-core LBS
 // The shape blend + pose blend of SMPL is one contraction  v_posed[frame, col] = sum_k feat[frame, k] basis[col, k]
 // (k: 207 pose features x posedirs | 10 betas x shapedirs | 1 x v_template; lbs.py:240,256-267), i.e. a [n x 218] x [218 x 20670]
-// GEMM.  lbs_blend_tc_kernel runs it on the 5th-generation tensor cores with FP32 accuracy (3xTF32: hi*hi + lo*hi + hi*lo,
-// |error| ~ 2e-7 on the blended vertex): both operands are PRE-SPLIT into tf32 hi / lo and pre-tiled in global memory as the UMMA
-// K-major core-matrix image (basis once at glamr_smpl_create, features by pose_prep_frame), so a pipeline stage is two 1-D bulk
-// TMA copies (8 KB of A, 16 KB of B) with no SIMT work on the operand path.  CTA tile = 128 frames (TMEM lanes) x 256 basis columns
-// (TMEM columns), K in 28 steps of 8; warp 0 = TMA producer, warp 1 = MMA issuer (one elected thread, tcgen05.commit -> mbarrier),
-// warps 2-5 = epilogue: tcgen05.ld the accumulator and store it TRANSPOSED ([column][frame]) so that lbs_skin_kernel (lanes =
-// frames) reads 128 contiguous bytes per vertex coordinate.  4 stages x 24 KB = 96 KB of shared memory and 256 TMEM columns per
-// CTA: two CTAs per SM overlap one's epilogue with the other's main loop.
+// GEMM.  lbs_blend_tc_kernel runs it on the Hopper tensor cores (wgmma) with FP32 accuracy (3xTF32: hi*hi + lo*hi + hi*lo,
+// |error| ~ 2e-7 on the blended vertex): both operands are PRE-SPLIT into tf32 hi / lo and pre-tiled in global memory as the
+// K-major core-matrix image wgmma reads from shared memory (basis once at glamr_smpl_create, features by pose_prep_frame), so a
+// pipeline stage is two 1-D bulk TMA copies (8 KB of A, 16 KB of B) with no SIMT work on the operand path.  CTA tile = 128 frames x
+// 256 basis columns, K in 28 steps of 8; warp 8 = TMA producer, warpgroups 0 and 1 = consumers (64 frames each, m64n256k8, the
+// accumulator in 128 registers per thread), which release a stage once the wgmma group that read it has retired and finally store
+// the accumulator TRANSPOSED ([column][frame]) so that lbs_skin_kernel (lanes = frames) reads contiguous bytes per vertex
+// coordinate.  4 stages x 24 KB = 96 KB of shared memory per CTA.
 constexpr int kTcStages = 4;
-constexpr int kTcThreads = 192;
+constexpr int kTcThreads = 288;           // warpgroups 0-1 consume, warp 8 produces
 constexpr uint32_t kTcABytes = kTcAStageFloats * sizeof(float);      // 8,192
 constexpr uint32_t kTcBBytes = kTcBStageFloats * sizeof(float);      // 16,384
 constexpr size_t kTcSmemBytes = (size_t)kTcStages * (kTcABytes + kTcBBytes) + 128;
 
-__global__ void __launch_bounds__(kTcThreads) lbs_blend_tc_kernel(SmplDev m, SmplWorkspace w, int mtile0) {
+__global__ void __launch_bounds__(kTcThreads, 1) lbs_blend_tc_kernel(SmplDev m, SmplWorkspace w, int mtile0) {
   extern __shared__ __align__(128) unsigned char tc_raw[];
   float* As = reinterpret_cast<float*>(tc_raw);                                   // [stages][hi | lo][2][128][4]
   float* Bs = As + kTcStages * kTcAStageFloats;                                   // [stages][hi | lo][2][256][4]
   uint64_t* full = reinterpret_cast<uint64_t*>(Bs + kTcStages * kTcBStageFloats); // [stages]
   uint64_t* empty = full + kTcStages;                                             // [stages]
-  uint64_t* acc_full = empty + kTcStages;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(acc_full + 1);
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const int ntile = blockIdx.x, mtile = blockIdx.y + mtile0;     // mtile0: first 128-frame tile of this launch (the optimiser splits the blend in two launches)
   pdl_launch_dependents();
-  if (warp == 1) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)), "r"(kTcN));
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::);
-  }
   if (tid == 0) {
 #pragma unroll
-    for (int s = 0; s < kTcStages; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], 1); }
-    mbar_init(acc_full, 1);
+    for (int s = 0; s < kTcStages; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], 8); }   // empty: one arrival per consumer warp
     mbar_fence_init();
   }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
   __syncthreads();
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-  const uint32_t tmem_d = *tmem_slot;
 
-  if (warp == 0) {
+  if (warp == 8) {
     if (lane == 0) {
       const float* gA = w.tcA + (size_t)mtile * kTcChunks * kTcAStageFloats;
       const float* gB = m.tcB + (size_t)ntile * kTcChunks * kTcBStageFloats;
@@ -386,7 +376,7 @@ __global__ void __launch_bounds__(kTcThreads) lbs_blend_tc_kernel(SmplDev m, Smp
       for (int c = 0; c < kTcChunks; ++c) {
         const int s = c % kTcStages;
         if (c >= kTcStages) {
-          mbar_wait(&empty[s], ((c / kTcStages) - 1) & 1);                       // the MMAs that read this stage have completed
+          mbar_wait(&empty[s], ((c / kTcStages) - 1) & 1);                       // the wgmma groups that read this stage have retired
           mbar_expect_tx(&full[s], kTcABytes + kTcBBytes);
           tma_bulk_g2s(Bs + s * kTcBStageFloats, gB + (size_t)c * kTcBStageFloats, kTcBBytes, &full[s]);
         } else {
@@ -395,58 +385,47 @@ __global__ void __launch_bounds__(kTcThreads) lbs_blend_tc_kernel(SmplDev m, Smp
         tma_bulk_g2s(As + s * kTcAStageFloats, gA + (size_t)c * kTcAStageFloats, kTcABytes, &full[s]);
       }
     }
-  } else if (warp == 1) {
-    if (lane == 0) {
-      // instruction descriptor (cute::UMMA::InstrDescriptor): D=F32 [4,6)=1, A=TF32 [7,10)=2, B=TF32 [10,13)=2, K-major A/B, N>>3 [17,23), M>>4 [24,29)
-      const uint32_t idesc = (1u << 4) | (2u << 7) | (2u << 10) | ((uint32_t)(kTcN >> 3) << 17) | ((uint32_t)(kTcM >> 4) << 24);
-      for (int c = 0; c < kTcChunks; ++c) {
-        const int s = c % kTcStages;
-        mbar_wait(&full[s], (c / kTcStages) & 1);
-        asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-        const float* a = As + s * kTcAStageFloats;
-        const float* b = Bs + s * kTcBStageFloats;
-        const uint64_t dah = umma_desc_kmajor_noswizzle(a, kTcM), dal = umma_desc_kmajor_noswizzle(a + kTcAStageFloats / 2, kTcM);
-        const uint64_t dbh = umma_desc_kmajor_noswizzle(b, kTcN), dbl = umma_desc_kmajor_noswizzle(b + kTcBStageFloats / 2, kTcN);
-        umma_tf32(tmem_d, dah, dbh, idesc, c > 0 ? 1u : 0u);
-        umma_tf32(tmem_d, dal, dbh, idesc, 1u);
-        umma_tf32(tmem_d, dah, dbl, idesc, 1u);
-        // arrives on empty[s] once every MMA issued so far has completed (implies tcgen05.fence::before_thread_sync)
-        asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(&empty[s])) : "memory");
-      }
-      asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(acc_full)) : "memory");
-    }
-  } else {
-    // ---- epilogue: warp q = warp % 4 may read TMEM lanes 32 q .. 32 q + 31 (= frames of this tile)
-    mbar_wait(acc_full, 0);
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    const int q = warp & 3;
-    const int frame = mtile * kTcM + q * 32 + lane;                              // < w.mpad by construction
-    // v_posed^T [column][frame], or frame-tiled [frame / 20][column][frame % 20] for the tensor-core skinning
-    float* const vpb = vp_buffer(w);
-    float* out = w.vp_tiled ? vpb + ((size_t)(frame / kSkF) * kTcCols + (size_t)ntile * kTcN) * kSkF + frame % kSkF
-                            : vpb + (size_t)ntile * kTcN * w.mpad + frame;
-    const size_t cstride = w.vp_tiled ? (size_t)kSkF : (size_t)w.mpad;
-#pragma unroll 1
-    for (int cc = 0; cc < kTcN / 32; ++cc) {
-      uint32_t v[32];
-      const uint32_t taddr = tmem_d + ((uint32_t)(q * 32) << 16) + (uint32_t)(cc * 32);
-      asm volatile(
-          "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-          "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, "
-          "%28, %29, %30, %31}, [%32];\n"
-          : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]), "=r"(v[8]), "=r"(v[9]), "=r"(v[10]),
-            "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15]), "=r"(v[16]), "=r"(v[17]), "=r"(v[18]), "=r"(v[19]), "=r"(v[20]),
-            "=r"(v[21]), "=r"(v[22]), "=r"(v[23]), "=r"(v[24]), "=r"(v[25]), "=r"(v[26]), "=r"(v[27]), "=r"(v[28]), "=r"(v[29]), "=r"(v[30]),
-            "=r"(v[31])
-          : "r"(taddr));
-      asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
+    return;
+  }
+  // ---- consumers: warpgroup g owns frames 64 g .. 64 g + 63 of the tile
+  const int g = warp >> 2;
+  float acc[kTcN / 2];
 #pragma unroll
-      for (int j = 0; j < 32; ++j) out[(size_t)(cc * 32 + j) * cstride] = __uint_as_float(v[j]);   // 32 lanes = 32 consecutive frames: 128 B per column (2-3 runs when tiled)
+  for (int i = 0; i < kTcN / 2; ++i) acc[i] = 0.0f;
+#pragma unroll 1
+  for (int c = 0; c < kTcChunks; ++c) {
+    const int s = c % kTcStages;
+    mbar_wait(&full[s], (c / kTcStages) & 1);
+    const float* a = As + s * kTcAStageFloats + g * 64 * 4;
+    const float* b = Bs + s * kTcBStageFloats;
+    const uint64_t dah = wgmma_desc_kmajor_noswizzle(a, kTcM), dal = wgmma_desc_kmajor_noswizzle(a + kTcAStageFloats / 2, kTcM);
+    const uint64_t dbh = wgmma_desc_kmajor_noswizzle(b, kTcN), dbl = wgmma_desc_kmajor_noswizzle(b + kTcBStageFloats / 2, kTcN);
+    wgmma_fence();
+    wgmma_m64n256k8_tf32(acc, dah, dbh, c > 0 ? 1u : 0u);
+    wgmma_m64n256k8_tf32(acc, dal, dbh, 1u);
+    wgmma_m64n256k8_tf32(acc, dah, dbl, 1u);
+    wgmma_commit();
+    wgmma_wait<1>();                                                              // the group of chunk c - 1 has retired
+    if (c > 0 && lane == 0) mbar_arrive(&empty[(c - 1) % kTcStages]);
+  }
+  wgmma_wait<0>();
+  wgmma_fence_acc(acc);
+  // ---- epilogue: d[4 i + 2 h + e] = D[16 (warp % 4) + lane / 4 + 8 h][8 i + 2 (lane % 4) + e]
+  // v_posed^T [column][frame], or frame-tiled [frame / 20][column][frame % 20] for the tensor-core skinning; a store instruction
+  // writes 8 consecutive frames (32 bytes) of 4 columns
+  float* const vpb = vp_buffer(w);
+  const size_t cstride = w.vp_tiled ? (size_t)kSkF : (size_t)w.mpad;
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    const int frame = mtile * kTcM + g * 64 + (warp & 3) * 16 + (lane >> 2) + 8 * h;   // < w.mpad by construction
+    float* out = (w.vp_tiled ? vpb + ((size_t)(frame / kSkF) * kTcCols + (size_t)ntile * kTcN) * kSkF + frame % kSkF
+                             : vpb + (size_t)ntile * kTcN * w.mpad + frame) + (size_t)(2 * (lane & 3)) * cstride;
+#pragma unroll
+    for (int i = 0; i < kTcN / 8; ++i) {
+      out[(size_t)(8 * i) * cstride] = acc[4 * i + 2 * h];
+      out[(size_t)(8 * i + 1) * cstride] = acc[4 * i + 2 * h + 1];
     }
   }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-  __syncthreads();
-  if (warp == 1) asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_d), "r"(kTcN));
 }
 
 // Skinning of the blended vertices (lbs.py:273-284): CTA = 128 vertices x 32 frames, warp = 32 vertices, lane = frame.
@@ -554,34 +533,23 @@ __global__ void __launch_bounds__(kLbsThreads) lbs_skin_kernel(SmplDev m, int n_
 
 // ------------------------------------------------------------------------------------------------ tensor-core skinning
 // lbs.py:273-284 as a GEMM with a fused epilogue.  The blended transform of vertex v in frame f is T[v][f] = sum_j W[v][j] A_j[f]
-// (12 numbers), i.e. [128 vertices x 24 joints] x [24 joints x (20 frames x 12)] per CTA: M = 128 (TMEM lanes = vertices), N = 240
-// (TMEM columns), K = 24 in three kind::tf32 steps, 3xTF32 (hi*hi + lo*hi + hi*lo) like the blend.  Both operands are pre-tiled
-// UMMA images (W: model constant built at glamr_smpl_create; A: written by pose_prep_frame), so the whole operand traffic of a
-// CTA is three bulk copies: W image 24 KB, A image 45 KB, and the 128 x 20 v_posed block 30 KB (the blend stores v_posed frame-
-// tiled for this).  Epilogue: thread = vertex reads its 12 x 20 transform entries with tcgen05.ld, its v_posed with conflict-free
-// LDS.128 (80-byte row pitch, 240-byte lane stride) and applies T to it -- no shared-memory traffic for the joint transforms,
-// which bounded the SIMT skinning (12 LDS.128 per vertex-frame).  warp 0 = producer, warp 1 = TMEM + MMA, warps 2-5 = epilogue;
-// 101 KB of shared memory and 256 TMEM columns per CTA: two CTAs per SM overlap one's epilogue with the other's loads.
+// (12 numbers), i.e. [128 vertices x 24 joints] x [24 joints x (20 frames x 12)] per CTA: two consumer warpgroups of 64 vertices,
+// each m64n240k8 with the accumulator in 120 registers per thread, K = 24 in three steps, 3xTF32 (hi*hi + lo*hi + hi*lo) like the
+// blend.  Both operands are pre-tiled wgmma images (W: model constant built at glamr_smpl_create; A: written by pose_prep_frame), so
+// the whole operand traffic of a CTA is three bulk copies: W image 24 KB, A image 45 KB, and the 128 x 20 v_posed block 30 KB (the
+// blend stores v_posed frame-tiled for this).  Epilogue straight from the accumulator fragment: the quad of lanes that holds a
+// vertex row owns all 24 columns of a frame pair; each lane dots its column pairs with (x, y) or (z, 1) of v_posed and one
+// shuffle with the neighbouring lane completes an output coordinate -- no shared-memory traffic for the joint transforms, which
+// bounded the SIMT skinning (12 LDS.128 per vertex-frame).  warp 8 = producer; 99 KB of shared memory per CTA.
 constexpr uint32_t kSkWBytes = kSkWImageFloats * sizeof(float);       // 24,576
 constexpr uint32_t kSkBBytes = kSkBImageFloats * sizeof(float);       // 46,080
 constexpr uint32_t kSkVBytes = kSkVpTileFloats * sizeof(float);       // 30,720
 constexpr size_t kSkinTcSmemBytes = (size_t)kSkWBytes + kSkBBytes + kSkVBytes + 128;
 
-#define GLAMR_TMEM_LD_X16(v, taddr)                                                                                                  \
-  asm volatile("tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];\n" \
-               : "=r"((v)[0]), "=r"((v)[1]), "=r"((v)[2]), "=r"((v)[3]), "=r"((v)[4]), "=r"((v)[5]), "=r"((v)[6]), "=r"((v)[7]),      \
-                 "=r"((v)[8]), "=r"((v)[9]), "=r"((v)[10]), "=r"((v)[11]), "=r"((v)[12]), "=r"((v)[13]), "=r"((v)[14]), "=r"((v)[15])  \
-               : "r"(taddr))
+constexpr int kSkinTcThreads = 288;     // warpgroups 0-1 consume (64 vertices each), warp 8 produces
+constexpr int kSkTilesPerCta = 3;       // frame tiles one CTA sweeps (W stays in shared memory)
 
-#define GLAMR_TMEM_LD_X8(v, taddr)                                                                                  \
-  asm volatile("tcgen05.ld.sync.aligned.32x32b.x8.b32 {%0, %1, %2, %3, %4, %5, %6, %7}, [%8];\n"                      \
-               : "=r"((v)[0]), "=r"((v)[1]), "=r"((v)[2]), "=r"((v)[3]), "=r"((v)[4]), "=r"((v)[5]), "=r"((v)[6]), "=r"((v)[7]) \
-               : "r"(taddr))
-
-constexpr int kSkinTcThreads = 320;     // warp 0 producer, warp 1 TMEM + MMA, warps 2-9 epilogue (two warps per TMEM lane quarter)
-constexpr int kSkTilesPerCta = 3;       // frame tiles one CTA sweeps (W stays in shared memory; 54 x 5 CTAs = one wave at 300 frames)
-
-__global__ void __launch_bounds__(kSkinTcThreads) lbs_skin_tc_kernel(SmplDev m, int n, SmplWorkspace w, float* __restrict__ vertices) {
+__global__ void __launch_bounds__(kSkinTcThreads, 1) lbs_skin_tc_kernel(SmplDev m, int n, SmplWorkspace w, float* __restrict__ vertices) {
   extern __shared__ __align__(128) unsigned char sk_raw[];
   float* Ws = reinterpret_cast<float*>(sk_raw);                       // [hi | lo][6][128][4]
   float* Bs = Ws + kSkWImageFloats;                                   // [hi | lo][6][240][4]
@@ -589,36 +557,24 @@ __global__ void __launch_bounds__(kSkinTcThreads) lbs_skin_tc_kernel(SmplDev m, 
   uint64_t* full_w = reinterpret_cast<uint64_t*>(Vs + kSkVpTileFloats);
   uint64_t* full_b = full_w + 1;          // A image of the current frame tile has landed
   uint64_t* full_v = full_w + 2;          // v_posed block has landed
-  uint64_t* acc_full = full_w + 3;        // the tile's MMAs have completed (accumulator readable)
-  uint64_t* b_empty = full_w + 4;         // ... and no longer read Bs: the next A image may be fetched
-  uint64_t* v_empty = full_w + 5;         // the 4 epilogue warps are done with Vs
-  uint64_t* acc_empty = full_w + 6;       // ... and with the accumulator
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(full_w + 7);
+  uint64_t* b_empty = full_w + 3;         // the 8 consumer warps' wgmmas no longer read Bs: the next A image may be fetched
+  uint64_t* v_empty = full_w + 4;         // the 8 consumer warps are done with Vs
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const int vtile = blockIdx.x;
   const int ftile0 = blockIdx.y * kSkTilesPerCta;
   const int ntiles = min(kSkTilesPerCta, (n + kSkF - 1) / kSkF - ftile0);
   pdl_launch_dependents();
-  if (warp == 1) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)), "r"(256));
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::);
-  }
   if (tid == 0) {
     mbar_init(full_w, 1);
     mbar_init(full_b, 1);
     mbar_init(full_v, 1);
-    mbar_init(acc_full, 1);
-    mbar_init(b_empty, 1);
+    mbar_init(b_empty, 8);
     mbar_init(v_empty, 8);
-    mbar_init(acc_empty, 8);
     mbar_fence_init();
   }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
   __syncthreads();
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-  const uint32_t tmem_d = *tmem_slot;
 
-  if (warp == 0) {
+  if (warp == 8) {
     if (lane == 0) {
       mbar_expect_tx(full_w, kSkWBytes);
       tma_bulk_g2s(Ws, m.skW + (size_t)vtile * kSkWImageFloats, kSkWBytes, full_w);          // model constant: before the dependency wait
@@ -634,86 +590,80 @@ __global__ void __launch_bounds__(kSkinTcThreads) lbs_skin_tc_kernel(SmplDev m, 
         tma_bulk_g2s(Vs, vpb + ((size_t)ftile * kTcCols + (size_t)vtile * kTileCols) * kSkF, kSkVBytes, full_v);
       }
     }
-  } else if (warp == 1) {
-    if (lane == 0) {
-      const uint32_t idesc = (1u << 4) | (2u << 7) | (2u << 10) | ((uint32_t)(kSkN >> 3) << 17) | ((uint32_t)(kVTile >> 4) << 24);
-      mbar_wait(full_w, 0);
-      for (int it = 0; it < ntiles; ++it) {
-        mbar_wait(full_b, it & 1);
-        if (it > 0) mbar_wait(acc_empty, (it - 1) & 1);
-        asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
+    return;
+  }
+  // ---- consumers: warpgroup g owns vertices 64 g .. 64 g + 63 of the tile
+  const int g = warp >> 2, q = lane & 3;
+  int gv[2], ci[2];
+  const float* vrow[2];
 #pragma unroll
-        for (int c = 0; c < kNJ / 8; ++c) {
-          const float* a = Ws + c * 2 * kVTile * 4;
-          const float* b = Bs + c * 2 * kSkN * 4;
-          const uint64_t dah = umma_desc_kmajor_noswizzle(a, kVTile), dal = umma_desc_kmajor_noswizzle(a + kSkWHalf, kVTile);
-          const uint64_t dbh = umma_desc_kmajor_noswizzle(b, kSkN), dbl = umma_desc_kmajor_noswizzle(b + kSkBHalf, kSkN);
-          umma_tf32(tmem_d, dah, dbh, idesc, c > 0 ? 1u : 0u);
-          umma_tf32(tmem_d, dal, dbh, idesc, 1u);
-          umma_tf32(tmem_d, dah, dbl, idesc, 1u);
-        }
-        // both arrive once every MMA issued so far has completed
-        asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(b_empty)) : "memory");
-        asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(acc_full)) : "memory");
-      }
+  for (int h = 0; h < 2; ++h) {
+    const int vl = g * 64 + (warp & 3) * 16 + (lane >> 2) + 8 * h;   // accumulator rows of this thread
+    gv[h] = vtile * kVTile + vl;
+    ci[h] = m.compact_of_vertex[min(gv[h], kVPad - 1)];
+    vrow[h] = Vs + (size_t)vl * 3 * kSkF;
+  }
+  // column pair j of a frame pair (24 columns) this lane holds: 8 j + 2 q = 12 fr + 4 row + (0: x, y | 2: z, 1)
+  int jf[3], jrow[3];
+  bool jxy[3];
+#pragma unroll
+  for (int j = 0; j < 3; ++j) {
+    const int c0 = 8 * j + 2 * q;
+    jf[j] = c0 >= 12 ? 1 : 0;
+    jrow[j] = (c0 - 12 * jf[j]) >> 2;
+    jxy[j] = (c0 & 3) == 0;
+  }
+  mbar_wait(full_w, 0);
+  for (int it = 0; it < ntiles; ++it) {
+    const int ftile = ftile0 + it;
+    mbar_wait(full_b, it & 1);
+    float acc[kSkN / 2];
+#pragma unroll
+    for (int i = 0; i < kSkN / 2; ++i) acc[i] = 0.0f;
+    wgmma_fence();
+#pragma unroll
+    for (int c = 0; c < kNJ / 8; ++c) {
+      const float* a = Ws + c * 2 * kVTile * 4 + g * 64 * 4;
+      const float* b = Bs + c * 2 * kSkN * 4;
+      const uint64_t dah = wgmma_desc_kmajor_noswizzle(a, kVTile), dal = wgmma_desc_kmajor_noswizzle(a + kSkWHalf, kVTile);
+      const uint64_t dbh = wgmma_desc_kmajor_noswizzle(b, kSkN), dbl = wgmma_desc_kmajor_noswizzle(b + kSkBHalf, kSkN);
+      wgmma_m64n240k8_tf32(acc, dah, dbh, c > 0 ? 1u : 0u);
+      wgmma_m64n240k8_tf32(acc, dal, dbh, 1u);
+      wgmma_m64n240k8_tf32(acc, dah, dbl, 1u);
     }
-  } else {
-    // ---- epilogue: warp q = warp % 4 may read TMEM lanes 32 q .. 32 q + 31 (= vertices of this tile); the two warps of a quarter take
-    // alternate pairs of frames (24 accumulator columns each)
-    const int q = warp & 3, half = (warp - 2) >> 2;
-    const int vl = q * 32 + lane;
-    const int gv = vtile * kVTile + vl;
-    const bool v_ok = gv < kV;
-    const int ci = m.compact_of_vertex[min(gv, kVPad - 1)];
-    const float* vrow = Vs + (size_t)vl * 3 * kSkF;
-    for (int it = 0; it < ntiles; ++it) {
-      const int ftile = ftile0 + it;
-      mbar_wait(full_v, it & 1);
-      mbar_wait(acc_full, it & 1);
-      asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-#pragma unroll 1
-      for (int g = half; g < kSkF / 2; g += 2) {                   // 2 frames = 24 accumulator columns per step
-        uint32_t t[24];
-        const uint32_t taddr = tmem_d + ((uint32_t)(q * 32) << 16) + (uint32_t)(g * 24);
-        GLAMR_TMEM_LD_X16(t, taddr);
-        GLAMR_TMEM_LD_X8(t + 16, taddr + 16);
-        const float2 xs = *reinterpret_cast<const float2*>(vrow + g * 2);
-        const float2 ys = *reinterpret_cast<const float2*>(vrow + kSkF + g * 2);
-        const float2 zs = *reinterpret_cast<const float2*>(vrow + 2 * kSkF + g * 2);
-        asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-        const float x[2] = {xs.x, xs.y}, y[2] = {ys.x, ys.y}, z[2] = {zs.x, zs.y};
+    wgmma_commit();
+    wgmma_wait<0>();
+    wgmma_fence_acc(acc);
+    __syncwarp();
+    if (lane == 0) mbar_arrive(b_empty);
+    mbar_wait(full_v, it & 1);
 #pragma unroll
-        for (int ff = 0; ff < 2; ++ff) {
-          const int fl = ftile * kSkF + g * 2 + ff;                // local frame-person index
-#define GLAMR_T(k) __uint_as_float(t[ff * 12 + (k)])
-          const float ox = fmaf(GLAMR_T(0), x[ff], fmaf(GLAMR_T(1), y[ff], fmaf(GLAMR_T(2), z[ff], GLAMR_T(3))));
-          const float oy = fmaf(GLAMR_T(4), x[ff], fmaf(GLAMR_T(5), y[ff], fmaf(GLAMR_T(6), z[ff], GLAMR_T(7))));
-          const float oz = fmaf(GLAMR_T(8), x[ff], fmaf(GLAMR_T(9), y[ff], fmaf(GLAMR_T(10), z[ff], GLAMR_T(11))));
-#undef GLAMR_T
+    for (int h = 0; h < 2; ++h) {
+      const bool v_ok = gv[h] < kV;
+#pragma unroll
+      for (int p = 0; p < kSkF / 2; ++p) {
+        float part[3];
+#pragma unroll
+        for (int j = 0; j < 3; ++j) {
+          const float t0 = acc[4 * (3 * p + j) + 2 * h], t1 = acc[4 * (3 * p + j) + 2 * h + 1];
+          const int f = 2 * p + jf[j];
+          part[j] = jxy[j] ? fmaf(t0, vrow[h][f], t1 * vrow[h][kSkF + f]) : fmaf(t0, vrow[h][2 * kSkF + f], t1);
+          part[j] += __shfl_xor_sync(0xffffffffu, part[j], 1);      // the neighbouring lane holds the other half of the row
+        }
+#pragma unroll
+        for (int j = 0; j < 3; ++j) {
+          if ((j == 2) != ((q & 1) == 1)) continue;                  // even lanes store j = 0, 1; odd lanes j = 2
+          const int fl = ftile * kSkF + 2 * p + jf[j];               // local frame-person index
           if (fl < n && v_ok) {
-            if (vertices) {
-              float* o = vertices + ((size_t)fl * kV + gv) * 3;
-              o[0] = ox; o[1] = oy; o[2] = oz;
-            }
-            if (ci >= 0) {
-              float* o = w.vcompact + ((size_t)fl * m.S + ci) * 3;
-              o[0] = ox; o[1] = oy; o[2] = oz;
-            }
+            if (vertices) vertices[((size_t)fl * kV + gv[h]) * 3 + jrow[j]] = part[j];
+            if (ci[h] >= 0) w.vcompact[((size_t)fl * m.S + ci[h]) * 3 + jrow[j]] = part[j];
           }
         }
       }
-      // release the accumulator and the v_posed block for the next frame tile
-      asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-      __syncwarp();
-      if (lane == 0) {
-        mbar_arrive(acc_empty);
-        mbar_arrive(v_empty);
-      }
     }
+    __syncwarp();
+    if (lane == 0) mbar_arrive(v_empty);
   }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-  __syncthreads();
-  if (warp == 1) asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_d), "r"(256));
 }
 
 // ------------------------------------------------------------------------------------------------ joints_finalize
@@ -943,7 +893,7 @@ int launch_reroot_vertices(int n, const float* root_raw, const float* root_trans
                            cudaStream_t s) {
   if (n <= 0) return GLAMR_OK;
   const size_t total = (size_t)n * kV * 3;
-  const int blocks = (int)((total + 255) / 256 < 148 * 16 ? (total + 255) / 256 : 148 * 16);
+  const int blocks = (int)((total + 255) / 256 < 132 * 16 ? (total + 255) / 256 : 132 * 16);
   reroot_vertices_kernel<<<blocks, 256, 0, s>>>(n, root_raw, root_trans, root_scale, vertices);
   GLAMR_LAUNCH_CHECK();
   return GLAMR_OK;
@@ -1008,7 +958,7 @@ extern "C" int glamr_smpl_create(glamr_smpl_t** out, const float* v_template, co
       }
     if ((rc = upload(h, t, &d.pd_tiles))) goto fail;
   }
-  {  // blend basis [20736 cols][224 k] = posedirs^T | shapedirs | v_template, tf32 hi / lo, UMMA K-major core-matrix image per
+  {  // blend basis [20736 cols][224 k] = posedirs^T | shapedirs | v_template, tf32 hi / lo, wgmma K-major core-matrix image per
      // (256-column tile, 8-wide K chunk): [hi | lo][k group (4 wide)][256 cols][4]
     auto tf32_rna = [](float x) {            // cvt.rna.tf32.f32: round to nearest, ties away from zero, 10-bit mantissa
       uint32_t u;

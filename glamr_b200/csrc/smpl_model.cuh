@@ -10,10 +10,10 @@ struct SmplDev {
   const float* pd_tiles;     // [54][207][384]  posedirs, vertex-tile major: one contiguous 13,824 B block per
                              //                 (tile, 9-row chunk) so a CTA streams its slab with 1-D bulk TMA
   const float* tcB;          // [81 col tiles][28 K chunks][hi | lo][2 K groups][256 cols][4]  the blend basis (posedirs | shapedirs |
-                             //                 v_template) pre-split into tf32 hi / lo and pre-tiled as the UMMA K-major core-matrix image:
+                             //                 v_template) pre-split into tf32 hi / lo and pre-tiled as the wgmma K-major core-matrix image:
                              //                 one contiguous 16 KB block per (tile, chunk) = one bulk copy per pipeline stage
   const float* skW;          // [54 vertex tiles][hi | lo][6 joint groups][128 vertices][4]  dense skinning weights W[v][24], tf32 hi / lo,
-                             //                 UMMA K-major image: one contiguous 24 KB block per vertex tile (lbs_skin_tc_kernel)
+                             //                 wgmma K-major image: one contiguous 24 KB block per vertex tile (lbs_skin_tc_kernel)
   const float* v_template;   // [6912][3]  (padded with zeros)
   const float* shapedirs;    // [6912][30] ([v][c][l] as in the model file)
   const float* j_template;   // [24][3]    J_regressor @ v_template
@@ -42,7 +42,7 @@ struct SmplWorkspace {
   float* jposed;    // [n][24][3]   posed LBS joints
   float* vcompact;  // [n][S][3]    skinned support vertices
   float* root_raw;  // [n][3]       un-rooted joint 0 (for vertex re-rooting)
-  float* tcA;       // [n/128][28][hi | lo][2][128][4]  blend features (pose feature | betas | 1 | 0-pad), tf32 hi / lo, UMMA image per
+  float* tcA;       // [n/128][28][hi | lo][2][128][4]  blend features (pose feature | betas | 1 | 0-pad), tf32 hi / lo, wgmma image per
                     //              (128-frame tile, K chunk): 8 KB contiguous = one bulk copy per stage
   float* vpT;       // [20736][mpad]  blended vertices v_posed, TRANSPOSED (column-major over frames) so that the skinning kernel's
                     //              lanes = frames read 128 contiguous bytes per vertex coordinate

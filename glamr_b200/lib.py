@@ -1,6 +1,6 @@
 """ctypes binding of the CUDA library (include/glamr_b200.h).
 
-The library is built in-tree by ``__graft_entry__.build()`` (nvcc, sm_100a) as ``glamr_b200/libglamr_b200.so``.
+The library is built in-tree by ``__graft_entry__.build()`` (nvcc, sm_90a) as ``glamr_b200/libglamr_b200.so``.
 There is no CPU fallback: ``load()`` raises if the shared object is missing, and every call raises on a non-zero
 return code.
 """
@@ -71,7 +71,7 @@ _lib = None
 
 def nvcc_command(out_path=None, experiment=False):
     srcs = [os.path.join(CSRC, s) for s in SOURCES if os.path.exists(os.path.join(CSRC, s))]
-    return ['nvcc', '-gencode', 'arch=compute_100a,code=sm_100a', '-lineinfo', '-O3', '-std=c++17',
+    return ['nvcc', '-gencode', 'arch=compute_90a,code=sm_90a', '-lineinfo', '-O3', '-std=c++17',
             '-Xcompiler', '-fPIC', '-shared'] + (['-DGLAMR_EXPERIMENT'] if experiment else []) + \
            ['-o', out_path or (EXP_SO_PATH if experiment else REL_SO_PATH)] + srcs
 
@@ -85,7 +85,7 @@ def build_experiment():
 
 
 def build(force=False, verbose=False):
-    """Compile the CUDA library for sm_100a (cross-compiles without a GPU)."""
+    """Compile the CUDA library for sm_90a (cross-compiles without a GPU)."""
     srcs = [os.path.join(CSRC, f) for f in os.listdir(CSRC)] + [os.path.join(HERE, '..', 'include', 'glamr_b200.h')]
     newest = max(os.path.getmtime(p) for p in srcs)
     if not force and os.path.exists(REL_SO_PATH) and os.path.getmtime(REL_SO_PATH) >= newest:

@@ -46,7 +46,7 @@ class _GraphCache:
     capture is refused the key stays on the eager path."""
 
     def __init__(self, enabled=None, max_entries=8):
-        if enabled is None:          # GLAMR_PRIOR_GRAPH=1|0; the default flips to on once verified on a B200
+        if enabled is None:          # GLAMR_PRIOR_GRAPH=1|0
             enabled = os.environ.get('GLAMR_PRIOR_GRAPH', PRIOR_GRAPH_DEFAULT) == '1'
         self.enabled, self.max_entries, self.entries = enabled, max_entries, {}
 

@@ -520,9 +520,8 @@ class GlobalReconOptimizer:
     def _setup_peers(self):
         """Exchange CUDA-IPC handles of one small buffer per rank so that the per-iteration gradient reduction runs over
         NVLink peer memory inside the Adam kernel (include/glamr_b200.h, glamr_opt_set_peers).  Collective: every rank
-        calls it at the same point.  Opt-in (GLAMR_ALLREDUCE=peer): measured on B200s it is slower than the NCCL
-        all-reduce captured in the iteration graph (2 GPUs 0.167 vs 0.162 ms, 4 GPUs 0.207 vs 0.173 ms per iteration),
-        so NCCL stays the default; any rank failing to map a peer also falls back to NCCL."""
+        calls it at the same point.  Opt-in (GLAMR_ALLREDUCE=peer): the NCCL all-reduce captured in the iteration graph
+        is the default; any rank failing to map a peer also falls back to NCCL."""
         import os
         self._peer_ok, self._peer_own, self._peer_opened = False, None, []
         if self.world <= 1:

@@ -1,4 +1,4 @@
-/* glamr_b200 -- C ABI of the B200 (sm_100a) CUDA library behind GLAMR's global-reconstruction path.
+/* glamr_b200 -- C ABI of the H100 (sm_90a) CUDA library behind GLAMR's global-reconstruction path.
  *
  * GLAMR (NVlabs/GLAMR) is pure Python/PyTorch: it has no FFI layer, the seams a replacement binds to are Python
  * call sites.  Each entry point below names the reference interface it stands behind (paths relative to the

@@ -1,5 +1,6 @@
 """CPU-only checks: the C-ABI library exports every symbol include/glamr_b200.h declares (no compute calls), struct
-layouts agree with the ctypes mirror, the built-in stage tables equal the reference YAML, the product refuses CPU."""
+layouts agree with the ctypes mirror, the built-in stage tables equal the reference YAML (stored verbatim under
+tests/golden/reference_cfg), the product refuses CPU."""
 import ctypes
 import numpy as np
 import os
@@ -9,7 +10,7 @@ import torch
 import yaml
 
 import __graft_entry__ as ge
-from conftest import REFERENCE_ROOT
+from conftest import GOLDEN
 from glamr_b200 import lib as L
 from glamr_b200.config import BUILTIN_IDS, Config, builtin_config_dict
 
@@ -47,10 +48,9 @@ def test_product_requires_cuda_device():
         L.require_cuda('cpu')
 
 
-@pytest.mark.reference
 @pytest.mark.parametrize('cfg_id', BUILTIN_IDS)
 def test_builtin_configs_equal_reference_yaml(cfg_id):
-    ref = yaml.safe_load(open(os.path.join(REFERENCE_ROOT, 'global_recon', 'cfg', cfg_id + '.yml')))
+    ref = yaml.safe_load(open(os.path.join(GOLDEN, 'reference_cfg', cfg_id + '.yml')))
     mine = builtin_config_dict(cfg_id)
     assert mine['grecon_model_specs'] == ref['grecon_model_specs']
     assert mine['opt_stage_specs'] == ref['opt_stage_specs']

@@ -1,5 +1,5 @@
 """Parity of the CUDA path (through the C-ABI library) against the oracle and the reference-generated golden
-fixtures.  Runs on the B200 box:  python -m pytest tests -m gpu"""
+fixtures.  Runs on an H100:  python -m pytest tests -m gpu"""
 import copy
 import ctypes
 
@@ -75,7 +75,7 @@ LBS_PATHS = {'tensor_core': 2, 'tensor_core_blend_simt_skin': 1, 'simt': 0}
 
 @pytest.fixture(params=list(LBS_PATHS))
 def lbs_path(request):
-    """the implementations of the blend + skinning: tcgen05 3xTF32 blend GEMM + tcgen05 skinning, the same blend with the SIMT
+    """the implementations of the blend + skinning: wgmma 3xTF32 blend GEMM + wgmma skinning, the same blend with the SIMT
     skinning kernel, and the single FP32 SIMT kernel"""
     from glamr_b200 import lib as L
     L.check(L.load().glamr_smpl_set_lbs_path(LBS_PATHS[request.param]), 'set_lbs_path')
@@ -413,7 +413,7 @@ def test_product_fails_loudly_on_cpu_device(smpl_assets):
                                         (7, 5, 3, 1), (200, 512, 384, 1), (256, 256, 512, 0), (257, 256, 256, 0), (1500, 512, 384, 1),
                                         (3200, 768, 256, 0)])
 def test_linear_layer_kernels_match_float64(M, N, K, relu):
-    """Y = act(X W^T + b) of the prior networks: the skinny FP32 kernel (M <= 256), the tcgen05 3xTF32 tile kernel and the
+    """Y = act(X W^T + b) of the prior networks: the skinny FP32 kernel (M <= 256), the wgmma 3xTF32 tile kernel and the
     FP32 tile kernel (mode 0) against a float64 product; ragged M / N / K, unaligned K (69) included"""
     import ctypes
     from glamr_b200 import lib as L

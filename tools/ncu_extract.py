@@ -1,6 +1,6 @@
 """Per-kernel table of the ncu metrics the profile notes quote, from an `ncu -i x.ncu-rep --page raw --csv` dump.
 
-    python tools/ncu_extract.py profiles/iter_kernels_r02c_raw.csv
+    python tools/ncu_extract.py raw.csv
 """
 import csv
 import sys

@@ -21,4 +21,4 @@ for mode in (1, 0):
     for _ in range(10): out = m.inference(batch)
     torch.cuda.synchronize(); res[mode] = ((time.perf_counter() - t0) / 10 * 1e3, out)
 d = (res[1][1]['infer_out_body_pose'] - res[0][1]['infer_out_body_pose']).abs().max().item()
-print(f'B={B} T={T}: tcgen05 3xTF32 {res[1][0]:.2f} ms/batch, FP32 SIMT {res[0][0]:.2f} ms/batch, max |pose diff| {d:.2e}')
+print(f'B={B} T={T}: wgmma 3xTF32 {res[1][0]:.2f} ms/batch, FP32 SIMT {res[0][0]:.2f} ms/batch, max |pose diff| {d:.2e}')

@@ -1,4 +1,4 @@
-"""ncu launch list (CSV of `--metrics gpu__time_duration.sum`) -> per-kernel table (markdown) for profiles/.
+"""ncu launch list (CSV of `--metrics gpu__time_duration.sum`) -> per-kernel table (markdown).
 
     python tools/summarize_launches.py gpurun_out/launches.csv [skip_first_n_launches_per_kernel]
 """

@@ -1,4 +1,4 @@
-"""Latency experiments on the tcgen05 GEMM (GLAMR_TC_DEBUG bits: 1 no MMA, 2 no split/store, 4 no epilogue, 8 no loads)."""
+"""Latency experiments on the wgmma GEMM (GLAMR_TC_DEBUG bits: 1 no MMA, 2 no split/store, 4 no epilogue, 8 no loads)."""
 import ctypes, os, sys, torch
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 from glamr_b200 import lib as L

@@ -1,4 +1,4 @@
-"""tcgen05 3xTF32 GEMM vs fp64 torch and vs the FP32 SIMT kernel."""
+"""wgmma 3xTF32 GEMM vs fp64 torch and vs the FP32 SIMT kernel."""
 import ctypes, os, sys, torch
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 from glamr_b200 import lib as L
@@ -15,7 +15,7 @@ for (M, N, K, relu) in [(50, 256, 69, 0), (128, 128, 32, 0), (3200, 768, 256, 0)
         rc = lib.glamr_linear_forward(M, N, K, X.data_ptr(), W.data_ptr(), b.data_ptr(), relu, Y.data_ptr(), mode, torch.cuda.current_stream().cuda_stream)
         torch.cuda.synchronize()
         out[mode] = (rc, float((Y.double() - ref).abs().max()))
-    print(f'M={M} N={N} K={K} relu={relu}: tcgen05 rc/err {out[1]}  simt rc/err {out[0]}  ref scale {float(ref.abs().max()):.2f}', flush=True)
+    print(f'M={M} N={N} K={K} relu={relu}: wgmma rc/err {out[1]}  simt rc/err {out[0]}  ref scale {float(ref.abs().max()):.2f}', flush=True)
 
 # latency of the shapes the prior networks launch at B = 1 (one 120-frame window): back-to-back launches on one stream
 for (M, N, K) in [(120, 256, 256), (120, 512, 256), (120, 256, 512), (300, 512, 256), (7680, 256, 256), (7680, 512, 256)]:
@@ -30,5 +30,5 @@ for (M, N, K) in [(120, 256, 256), (120, 512, 256), (120, 256, 512), (300, 512, 
         for _ in range(200): lib.glamr_linear_forward(M, N, K, X.data_ptr(), W.data_ptr(), b.data_ptr(), 0, Y.data_ptr(), mode, st)
         e1.record(); torch.cuda.synchronize()
         us = e0.elapsed_time(e1) * 1e3 / 200
-        line += f"  {'tcgen05' if mode else 'simt'} {us:.2f} us ({2.0 * M * N * K / us * 1e-6:.2f} TFLOP/s)"
+        line += f"  {'wgmma' if mode else 'simt'} {us:.2f} us ({2.0 * M * N * K / us * 1e-6:.2f} TFLOP/s)"
     print(line, flush=True)
