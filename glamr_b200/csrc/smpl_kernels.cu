@@ -336,25 +336,33 @@ __global__ void __launch_bounds__(128) blend_features_kernel(int n, const float*
 // GEMM.  lbs_blend_tc_kernel runs it on the Hopper tensor cores (wgmma) with FP32 accuracy (3xTF32: hi*hi + lo*hi + hi*lo,
 // |error| ~ 2e-7 on the blended vertex): both operands are PRE-SPLIT into tf32 hi / lo and pre-tiled in global memory as the
 // K-major core-matrix image wgmma reads from shared memory (basis once at glamr_smpl_create, features by pose_prep_frame), so a
-// pipeline stage is two 1-D bulk TMA copies (8 KB of A, 16 KB of B) with no SIMT work on the operand path.  CTA tile = 128 frames x
+// pipeline stage is two 1-D bulk TMA copies (8 KB of A, 16 KB of B) with no SIMT work on the operand path.  Tile = 128 frames x
 // 256 basis columns, K in 28 steps of 8; warp 8 = TMA producer, warpgroups 0 and 1 = consumers (64 frames each, m64n256k8, the
 // accumulator in 128 registers per thread), which release a stage once the wgmma group that read it has retired and finally store
 // the accumulator TRANSPOSED ([column][frame]) so that lbs_skin_kernel (lanes = frames) reads contiguous bytes per vertex
-// coordinate.  4 stages x 24 KB = 96 KB of shared memory per CTA.
-constexpr int kTcStages = 4;
+// coordinate.  8 stages x 24 KB = 192 KB of shared memory per CTA: with 4 stages the blend alone runs as fast, but the iteration of
+// 4 x 300 frame-persons, where the blend shares the GPU with the residual and backward kernels, is ~5 % slower.
+// Persistent: the grid has one CTA per SM (the register file holds one), and CTA b runs tiles b, b + grid, ...  The stage ring runs on
+// across tiles, so the producer fetches the next tile's first stages while the consumers store the current accumulator.  Tiles are
+// numbered column-tile major (frame tile fastest): the CTAs that read one 448 KB basis column tile run at the same time, and the
+// 36 MB basis leaves HBM about once per launch instead of once per frame tile.  A last frame tile with at most 64 frames is a half
+// tile: both warpgroups take its 64 rows, each for 128 of the 256 columns (m64n128k8) -- same products, same K order.
+constexpr int kTcStages = 8;
 constexpr int kTcThreads = 288;           // warpgroups 0-1 consume, warp 8 produces
 constexpr uint32_t kTcABytes = kTcAStageFloats * sizeof(float);      // 8,192
 constexpr uint32_t kTcBBytes = kTcBStageFloats * sizeof(float);      // 16,384
 constexpr size_t kTcSmemBytes = (size_t)kTcStages * (kTcABytes + kTcBBytes) + 128;
 
-__global__ void __launch_bounds__(kTcThreads, 1) lbs_blend_tc_kernel(SmplDev m, SmplWorkspace w, int mtile0) {
+// mtile0 / mtiles: the 128-frame tiles of this launch (the optimiser may split the blend in two launches); half_last: the last of them
+// holds at most 64 frames
+__global__ void __launch_bounds__(kTcThreads, 1) lbs_blend_tc_kernel(SmplDev m, SmplWorkspace w, int mtile0, int mtiles, int half_last) {
   extern __shared__ __align__(128) unsigned char tc_raw[];
   float* As = reinterpret_cast<float*>(tc_raw);                                   // [stages][hi | lo][2][128][4]
   float* Bs = As + kTcStages * kTcAStageFloats;                                   // [stages][hi | lo][2][256][4]
   uint64_t* full = reinterpret_cast<uint64_t*>(Bs + kTcStages * kTcBStageFloats); // [stages]
   uint64_t* empty = full + kTcStages;                                             // [stages]
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-  const int ntile = blockIdx.x, mtile = blockIdx.y + mtile0;     // mtile0: first 128-frame tile of this launch (the optimiser splits the blend in two launches)
+  const int ntiles = kTcNTiles * mtiles;
   pdl_launch_dependents();
   if (tid == 0) {
 #pragma unroll
@@ -365,65 +373,90 @@ __global__ void __launch_bounds__(kTcThreads, 1) lbs_blend_tc_kernel(SmplDev m, 
 
   if (warp == 8) {
     if (lane == 0) {
-      const float* gA = w.tcA + (size_t)mtile * kTcChunks * kTcAStageFloats;
-      const float* gB = m.tcB + (size_t)ntile * kTcChunks * kTcBStageFloats;
-      // the basis is a model constant: its first stages are requested before this grid waits for the kernel that writes the features
-      for (int c = 0; c < kTcStages; ++c) {
-        mbar_expect_tx_only(&full[c], kTcBBytes);
-        tma_bulk_g2s(Bs + c * kTcBStageFloats, gB + (size_t)c * kTcBStageFloats, kTcBBytes, &full[c]);
+      // the basis is a model constant: the first stages of the first tile are requested before this grid waits for the kernel that
+      // writes the features
+      {
+        const float* gB = m.tcB + (size_t)(blockIdx.x / mtiles) * kTcChunks * kTcBStageFloats;
+        for (int c = 0; c < kTcStages; ++c) {
+          mbar_expect_tx_only(&full[c], kTcBBytes);
+          tma_bulk_g2s(Bs + c * kTcBStageFloats, gB + (size_t)c * kTcBStageFloats, kTcBBytes, &full[c]);
+        }
       }
       pdl_wait();
-      for (int c = 0; c < kTcChunks; ++c) {
-        const int s = c % kTcStages;
-        if (c >= kTcStages) {
-          mbar_wait(&empty[s], ((c / kTcStages) - 1) & 1);                       // the wgmma groups that read this stage have retired
-          mbar_expect_tx(&full[s], kTcABytes + kTcBBytes);
-          tma_bulk_g2s(Bs + s * kTcBStageFloats, gB + (size_t)c * kTcBStageFloats, kTcBBytes, &full[s]);
-        } else {
-          mbar_expect_tx(&full[s], kTcABytes);
+      int q = 0;                                                                  // stage uses so far (all tiles)
+      for (int t = blockIdx.x; t < ntiles; t += gridDim.x) {
+        const float* gA = w.tcA + (size_t)(mtile0 + t % mtiles) * kTcChunks * kTcAStageFloats;
+        const float* gB = m.tcB + (size_t)(t / mtiles) * kTcChunks * kTcBStageFloats;
+        for (int c = 0; c < kTcChunks; ++c, ++q) {
+          const int s = q % kTcStages;
+          if (q >= kTcStages) {
+            mbar_wait(&empty[s], ((q / kTcStages) - 1) & 1);                     // the wgmma groups that read this stage have retired
+            mbar_expect_tx(&full[s], kTcABytes + kTcBBytes);
+            tma_bulk_g2s(Bs + s * kTcBStageFloats, gB + (size_t)c * kTcBStageFloats, kTcBBytes, &full[s]);
+          } else {
+            mbar_expect_tx(&full[s], kTcABytes);
+          }
+          tma_bulk_g2s(As + s * kTcAStageFloats, gA + (size_t)c * kTcAStageFloats, kTcABytes, &full[s]);
         }
-        tma_bulk_g2s(As + s * kTcAStageFloats, gA + (size_t)c * kTcAStageFloats, kTcABytes, &full[s]);
       }
     }
     return;
   }
-  // ---- consumers: warpgroup g owns frames 64 g .. 64 g + 63 of the tile
+  // ---- consumers: warpgroup g owns frames 64 g .. 64 g + 63 of a full tile, columns 128 g .. 128 g + 127 of a half tile
   const int g = warp >> 2;
   float acc[kTcN / 2];
-#pragma unroll
-  for (int i = 0; i < kTcN / 2; ++i) acc[i] = 0.0f;
-#pragma unroll 1
-  for (int c = 0; c < kTcChunks; ++c) {
-    const int s = c % kTcStages;
-    mbar_wait(&full[s], (c / kTcStages) & 1);
-    const float* a = As + s * kTcAStageFloats + g * 64 * 4;
-    const float* b = Bs + s * kTcBStageFloats;
-    const uint64_t dah = wgmma_desc_kmajor_noswizzle(a, kTcM), dal = wgmma_desc_kmajor_noswizzle(a + kTcAStageFloats / 2, kTcM);
-    const uint64_t dbh = wgmma_desc_kmajor_noswizzle(b, kTcN), dbl = wgmma_desc_kmajor_noswizzle(b + kTcBStageFloats / 2, kTcN);
-    wgmma_fence();
-    wgmma_m64n256k8_tf32(acc, dah, dbh, c > 0 ? 1u : 0u);
-    wgmma_m64n256k8_tf32(acc, dal, dbh, 1u);
-    wgmma_m64n256k8_tf32(acc, dah, dbl, 1u);
-    wgmma_commit();
-    wgmma_wait<1>();                                                              // the group of chunk c - 1 has retired
-    if (c > 0 && lane == 0) mbar_arrive(&empty[(c - 1) % kTcStages]);
-  }
-  wgmma_wait<0>();
-  wgmma_fence_acc(acc);
-  // ---- epilogue: d[4 i + 2 h + e] = D[16 (warp % 4) + lane / 4 + 8 h][8 i + 2 (lane % 4) + e]
-  // v_posed^T [column][frame], or frame-tiled [frame / 20][column][frame % 20] for the tensor-core skinning; a store instruction
-  // writes 8 consecutive frames (32 bytes) of 4 columns
+  float (&acc_half)[kTcN / 4] = *reinterpret_cast<float (*)[kTcN / 4]>(acc);
   float* const vpb = vp_buffer(w);
   const size_t cstride = w.vp_tiled ? (size_t)kSkF : (size_t)w.mpad;
+  int q = 0;
+#pragma unroll 1
+  for (int t = blockIdx.x; t < ntiles; t += gridDim.x) {
+    const int ntile = t / mtiles, mt = t % mtiles, mtile = mtile0 + mt;
+    const bool half = half_last && mt == mtiles - 1;
+    // full tile: A rows 64 g.., all 256 columns of B; half tile: A rows 0..63, B columns 128 g..
+    const int aoff = half ? 0 : g * 64 * 4, boff = half ? g * 128 * 4 : 0;
+    auto mainloop = [&](auto& d, auto mma) {
+#pragma unroll 1
+      for (int c = 0; c < kTcChunks; ++c, ++q) {
+        const int s = q % kTcStages;
+        mbar_wait(&full[s], (q / kTcStages) & 1);
+        const float* a = As + s * kTcAStageFloats + aoff;
+        const float* b = Bs + s * kTcBStageFloats + boff;
+        const uint64_t dah = wgmma_desc_kmajor_noswizzle(a, kTcM), dal = wgmma_desc_kmajor_noswizzle(a + kTcAStageFloats / 2, kTcM);
+        const uint64_t dbh = wgmma_desc_kmajor_noswizzle(b, kTcN), dbl = wgmma_desc_kmajor_noswizzle(b + kTcBStageFloats / 2, kTcN);
+        wgmma_fence();
+        mma(d, dah, dbh, c > 0 ? 1u : 0u);
+        mma(d, dal, dbh, 1u);
+        mma(d, dah, dbl, 1u);
+        wgmma_commit();
+        wgmma_wait<1>();                                                          // the group of the previous stage use has retired
+        if (c > 0 && lane == 0) mbar_arrive(&empty[(q - 1) % kTcStages]);
+      }
+      wgmma_wait<0>();
+      wgmma_fence_acc(d);
+    };
+    if (half) mainloop(acc_half, [](float (&d)[kTcN / 4], uint64_t da, uint64_t db, uint32_t acc_in) { wgmma_m64n128k8_tf32(d, da, db, acc_in); });
+    else mainloop(acc, [](float (&d)[kTcN / 2], uint64_t da, uint64_t db, uint32_t acc_in) { wgmma_m64n256k8_tf32(d, da, db, acc_in); });
+    __syncwarp();
+    if (lane == 0) mbar_arrive(&empty[(q - 1) % kTcStages]);                     // the tile's last stage: the producer moves on
+    // ---- epilogue: d[4 i + 2 h + e] = D[16 (warp % 4) + lane / 4 + 8 h][8 i + 2 (lane % 4) + e]
+    // v_posed^T [column][frame], or frame-tiled [frame / 20][column][frame % 20] for the tensor-core skinning; a store instruction
+    // writes 8 consecutive frames (32 bytes) of 4 columns
+    const int row0 = mtile * kTcM + (half ? 0 : g * 64) + (warp & 3) * 16 + (lane >> 2);
+    const int col0 = ntile * kTcN + (half ? g * 128 : 0);
+    const int ncols = half ? kTcN / 2 : kTcN;
 #pragma unroll
-  for (int h = 0; h < 2; ++h) {
-    const int frame = mtile * kTcM + g * 64 + (warp & 3) * 16 + (lane >> 2) + 8 * h;   // < w.mpad by construction
-    float* out = (w.vp_tiled ? vpb + ((size_t)(frame / kSkF) * kTcCols + (size_t)ntile * kTcN) * kSkF + frame % kSkF
-                             : vpb + (size_t)ntile * kTcN * w.mpad + frame) + (size_t)(2 * (lane & 3)) * cstride;
+    for (int h = 0; h < 2; ++h) {
+      const int frame = row0 + 8 * h;                                             // < w.mpad by construction
+      float* out = (w.vp_tiled ? vpb + ((size_t)(frame / kSkF) * kTcCols + (size_t)col0) * kSkF + frame % kSkF
+                               : vpb + (size_t)col0 * w.mpad + frame) + (size_t)(2 * (lane & 3)) * cstride;
 #pragma unroll
-    for (int i = 0; i < kTcN / 8; ++i) {
-      out[(size_t)(8 * i) * cstride] = acc[4 * i + 2 * h];
-      out[(size_t)(8 * i + 1) * cstride] = acc[4 * i + 2 * h + 1];
+      for (int i = 0; i < kTcN / 8; ++i) {
+        if (8 * i < ncols) {
+          out[(size_t)(8 * i) * cstride] = acc[4 * i + 2 * h];
+          out[(size_t)(8 * i + 1) * cstride] = acc[4 * i + 2 * h + 1];
+        }
+      }
     }
   }
 }
@@ -540,36 +573,43 @@ __global__ void __launch_bounds__(kLbsThreads) lbs_skin_kernel(SmplDev m, int n_
 // blend stores v_posed frame-tiled for this).  Epilogue straight from the accumulator fragment: the quad of lanes that holds a
 // vertex row owns all 24 columns of a frame pair; each lane dots its column pairs with (x, y) or (z, 1) of v_posed and one
 // shuffle with the neighbouring lane completes an output coordinate -- no shared-memory traffic for the joint transforms, which
-// bounded the SIMT skinning (12 LDS.128 per vertex-frame).  warp 8 = producer; 99 KB of shared memory per CTA.
+// bounded the SIMT skinning (12 LDS.128 per vertex-frame).  warp 8 = producer.
+// Persistent: a work item is one (vertex tile, frame tile) pair, numbered vertex-tile major, and CTA b of a grid of at most one CTA per
+// SM (the register file holds one) runs the contiguous item range [b items / grid, (b + 1) items / grid).  Every CTA gets within one
+// item of the average, which a fixed number of frame tiles per CTA could not give for every n, and its range spans at most two vertex
+// tiles (fewer items than frame tiles per CTA), so the W image is fetched at most twice.  The A image and the v_posed block are
+// double-buffered: both operands of the next item land while the current one runs, so per item the CTA waits for neither; one buffered
+// item alone would leave each item's copy latency exposed, which bounded the kernel.  174 KB of shared memory per CTA.
 constexpr uint32_t kSkWBytes = kSkWImageFloats * sizeof(float);       // 24,576
 constexpr uint32_t kSkBBytes = kSkBImageFloats * sizeof(float);       // 46,080
 constexpr uint32_t kSkVBytes = kSkVpTileFloats * sizeof(float);       // 30,720
-constexpr size_t kSkinTcSmemBytes = (size_t)kSkWBytes + kSkBBytes + kSkVBytes + 128;
+constexpr size_t kSkinTcSmemBytes = (size_t)kSkWBytes + 2 * kSkBBytes + 2 * kSkVBytes + 128;
 
 constexpr int kSkinTcThreads = 288;     // warpgroups 0-1 consume (64 vertices each), warp 8 produces
-constexpr int kSkTilesPerCta = 3;       // frame tiles one CTA sweeps (W stays in shared memory)
 
 __global__ void __launch_bounds__(kSkinTcThreads, 1) lbs_skin_tc_kernel(SmplDev m, int n, SmplWorkspace w, float* __restrict__ vertices) {
   extern __shared__ __align__(128) unsigned char sk_raw[];
   float* Ws = reinterpret_cast<float*>(sk_raw);                       // [hi | lo][6][128][4]
-  float* Bs = Ws + kSkWImageFloats;                                   // [hi | lo][6][240][4]
-  float* Vs = Bs + kSkBImageFloats;                                   // [384 rows = vertex * 3 + coordinate][20 frames]
-  uint64_t* full_w = reinterpret_cast<uint64_t*>(Vs + kSkVpTileFloats);
-  uint64_t* full_b = full_w + 1;          // A image of the current frame tile has landed
-  uint64_t* full_v = full_w + 2;          // v_posed block has landed
-  uint64_t* b_empty = full_w + 3;         // the 8 consumer warps' wgmmas no longer read Bs: the next A image may be fetched
-  uint64_t* v_empty = full_w + 4;         // the 8 consumer warps are done with Vs
+  float* Bs = Ws + kSkWImageFloats;                                   // [2][hi | lo][6][240][4]
+  float* Vs = Bs + 2 * kSkBImageFloats;                               // [2][384 rows = vertex * 3 + coordinate][20 frames]
+  uint64_t* full_w = reinterpret_cast<uint64_t*>(Vs + 2 * kSkVpTileFloats);
+  uint64_t* full_b = full_w + 1;          // [2] A image (and, when the vertex tile changes, the W image) of the item has landed
+  uint64_t* b_empty = full_w + 3;         // [2] the 8 consumer warps' wgmmas no longer read this A image (nor Ws)
+  uint64_t* full_v = full_w + 5;          // [2] v_posed block has landed
+  uint64_t* v_empty = full_w + 7;         // [2] the 8 consumer warps are done with the v_posed block
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-  const int vtile = blockIdx.x;
-  const int ftile0 = blockIdx.y * kSkTilesPerCta;
-  const int ntiles = min(kSkTilesPerCta, (n + kSkF - 1) / kSkF - ftile0);
+  const int nft = (n + kSkF - 1) / kSkF;
+  const int items = kNVTiles * nft;
+  const int i0 = (int)((long long)blockIdx.x * items / gridDim.x), i1 = (int)((long long)(blockIdx.x + 1) * items / gridDim.x);
   pdl_launch_dependents();
   if (tid == 0) {
     mbar_init(full_w, 1);
-    mbar_init(full_b, 1);
-    mbar_init(full_v, 1);
-    mbar_init(b_empty, 8);
-    mbar_init(v_empty, 8);
+    for (int b = 0; b < 2; ++b) {
+      mbar_init(&full_b[b], 1);
+      mbar_init(&b_empty[b], 8);
+      mbar_init(&full_v[b], 1);
+      mbar_init(&v_empty[b], 8);
+    }
     mbar_fence_init();
   }
   __syncthreads();
@@ -577,32 +617,26 @@ __global__ void __launch_bounds__(kSkinTcThreads, 1) lbs_skin_tc_kernel(SmplDev 
   if (warp == 8) {
     if (lane == 0) {
       mbar_expect_tx(full_w, kSkWBytes);
-      tma_bulk_g2s(Ws, m.skW + (size_t)vtile * kSkWImageFloats, kSkWBytes, full_w);          // model constant: before the dependency wait
+      tma_bulk_g2s(Ws, m.skW + (size_t)(i0 / nft) * kSkWImageFloats, kSkWBytes, full_w);     // model constant: before the dependency wait
       pdl_wait();                                                                           // skB (pose prep) and v_posed (blend) below
       const float* const vpb = vp_buffer(w);
-      for (int it = 0; it < ntiles; ++it) {
-        const int ftile = ftile0 + it;
-        if (it > 0) mbar_wait(b_empty, (it - 1) & 1);
-        mbar_expect_tx(full_b, kSkBBytes);
-        tma_bulk_g2s(Bs, w.skB + (size_t)ftile * kSkBImageFloats, kSkBBytes, full_b);
-        if (it > 0) mbar_wait(v_empty, (it - 1) & 1);
-        mbar_expect_tx(full_v, kSkVBytes);
-        tma_bulk_g2s(Vs, vpb + ((size_t)ftile * kTcCols + (size_t)vtile * kTileCols) * kSkF, kSkVBytes, full_v);
+      for (int i = i0, it = 0; i < i1; ++i, ++it) {
+        const int vtile = i / nft, ftile = i - vtile * nft, vb = it & 1;
+        const bool new_w = it > 0 && ftile == 0;                                            // the range crossed into the next vertex tile
+        if (it >= 2) mbar_wait(&b_empty[vb], ((it - 2) >> 1) & 1);
+        if (new_w) mbar_wait(&b_empty[vb ^ 1], ((it - 1) >> 1) & 1);                       // Ws is read until the previous item's wgmmas retire
+        mbar_expect_tx(&full_b[vb], kSkBBytes + (new_w ? kSkWBytes : 0u));
+        tma_bulk_g2s(Bs + vb * kSkBImageFloats, w.skB + (size_t)ftile * kSkBImageFloats, kSkBBytes, &full_b[vb]);
+        if (new_w) tma_bulk_g2s(Ws, m.skW + (size_t)vtile * kSkWImageFloats, kSkWBytes, &full_b[vb]);
+        if (it >= 2) mbar_wait(&v_empty[vb], ((it - 2) >> 1) & 1);
+        mbar_expect_tx(&full_v[vb], kSkVBytes);
+        tma_bulk_g2s(Vs + vb * kSkVpTileFloats, vpb + ((size_t)ftile * kTcCols + (size_t)vtile * kTileCols) * kSkF, kSkVBytes, &full_v[vb]);
       }
     }
     return;
   }
   // ---- consumers: warpgroup g owns vertices 64 g .. 64 g + 63 of the tile
   const int g = warp >> 2, q = lane & 3;
-  int gv[2], ci[2];
-  const float* vrow[2];
-#pragma unroll
-  for (int h = 0; h < 2; ++h) {
-    const int vl = g * 64 + (warp & 3) * 16 + (lane >> 2) + 8 * h;   // accumulator rows of this thread
-    gv[h] = vtile * kVTile + vl;
-    ci[h] = m.compact_of_vertex[min(gv[h], kVPad - 1)];
-    vrow[h] = Vs + (size_t)vl * 3 * kSkF;
-  }
   // column pair j of a frame pair (24 columns) this lane holds: 8 j + 2 q = 12 fr + 4 row + (0: x, y | 2: z, 1)
   int jf[3], jrow[3];
   bool jxy[3];
@@ -614,17 +648,26 @@ __global__ void __launch_bounds__(kSkinTcThreads, 1) lbs_skin_tc_kernel(SmplDev 
     jxy[j] = (c0 & 3) == 0;
   }
   mbar_wait(full_w, 0);
-  for (int it = 0; it < ntiles; ++it) {
-    const int ftile = ftile0 + it;
-    mbar_wait(full_b, it & 1);
+  for (int i = i0, it = 0; i < i1; ++i, ++it) {
+    const int vtile = i / nft, ftile = i - vtile * nft, vb = it & 1;
+    int gv[2], ci[2];
+    const float* vrow[2];
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const int vl = g * 64 + (warp & 3) * 16 + (lane >> 2) + 8 * h;   // accumulator rows of this thread
+      gv[h] = vtile * kVTile + vl;
+      ci[h] = m.compact_of_vertex[min(gv[h], kVPad - 1)];
+      vrow[h] = Vs + vb * kSkVpTileFloats + (size_t)vl * 3 * kSkF;
+    }
+    mbar_wait(&full_b[vb], (it >> 1) & 1);
     float acc[kSkN / 2];
 #pragma unroll
-    for (int i = 0; i < kSkN / 2; ++i) acc[i] = 0.0f;
+    for (int k = 0; k < kSkN / 2; ++k) acc[k] = 0.0f;
     wgmma_fence();
 #pragma unroll
     for (int c = 0; c < kNJ / 8; ++c) {
       const float* a = Ws + c * 2 * kVTile * 4 + g * 64 * 4;
-      const float* b = Bs + c * 2 * kSkN * 4;
+      const float* b = Bs + vb * kSkBImageFloats + c * 2 * kSkN * 4;
       const uint64_t dah = wgmma_desc_kmajor_noswizzle(a, kVTile), dal = wgmma_desc_kmajor_noswizzle(a + kSkWHalf, kVTile);
       const uint64_t dbh = wgmma_desc_kmajor_noswizzle(b, kSkN), dbl = wgmma_desc_kmajor_noswizzle(b + kSkBHalf, kSkN);
       wgmma_m64n240k8_tf32(acc, dah, dbh, c > 0 ? 1u : 0u);
@@ -635,8 +678,8 @@ __global__ void __launch_bounds__(kSkinTcThreads, 1) lbs_skin_tc_kernel(SmplDev 
     wgmma_wait<0>();
     wgmma_fence_acc(acc);
     __syncwarp();
-    if (lane == 0) mbar_arrive(b_empty);
-    mbar_wait(full_v, it & 1);
+    if (lane == 0) mbar_arrive(&b_empty[vb]);
+    mbar_wait(&full_v[vb], (it >> 1) & 1);
 #pragma unroll
     for (int h = 0; h < 2; ++h) {
       const bool v_ok = gv[h] < kV;
@@ -662,7 +705,7 @@ __global__ void __launch_bounds__(kSkinTcThreads, 1) lbs_skin_tc_kernel(SmplDev 
       }
     }
     __syncwarp();
-    if (lane == 0) mbar_arrive(v_empty);
+    if (lane == 0) mbar_arrive(&v_empty[vb]);
   }
 }
 
@@ -771,6 +814,38 @@ static int lbs_set_attrs() {
   }
   return GLAMR_OK;
 }
+// SMs of the device: the persistent LBS GEMM kernels launch at most one CTA per SM
+static int device_sms() {
+  static int sms = 0;
+  if (sms <= 0) {
+    int dev = 0;
+    if (cudaGetDevice(&dev) != cudaSuccess || cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || sms <= 0) sms = 132;
+  }
+  return sms;
+}
+// the blend GEMM over the 128-frame tiles [mt_begin, mt_end) of n frame-persons
+static int launch_blend_gemm(const SmplDev& m, int n, const SmplWorkspace& w, cudaStream_t s, int mt_begin, int mt_end, bool pdl) {
+  const int mtiles = mt_end - mt_begin;
+  const int half_last = (mt_end == (n + kTcM - 1) / kTcM && n - (mt_end - 1) * kTcM <= kTcM / 2) ? 1 : 0;
+  const dim3 grid(min(device_sms(), kTcNTiles * mtiles));
+  if (pdl) {
+    GLAMR_CUDA_TRY(launch_pdl(4, lbs_blend_tc_kernel, grid, dim3(kTcThreads), kTcSmemBytes, s, m, w, mt_begin, mtiles, half_last));
+    return GLAMR_OK;
+  }
+  lbs_blend_tc_kernel<<<grid, kTcThreads, kTcSmemBytes, s>>>(m, w, mt_begin, mtiles, half_last);
+  GLAMR_LAUNCH_CHECK();
+  return GLAMR_OK;
+}
+static int launch_skin_tc(const SmplDev& m, int n, const SmplWorkspace& w, float* vertices, cudaStream_t s, bool pdl) {
+  const dim3 grid(min(device_sms(), kNVTiles * ((n + kSkF - 1) / kSkF)));
+  if (pdl) {
+    GLAMR_CUDA_TRY(launch_pdl(4, lbs_skin_tc_kernel, grid, dim3(kSkinTcThreads), kSkinTcSmemBytes, s, m, n, w, vertices));
+    return GLAMR_OK;
+  }
+  lbs_skin_tc_kernel<<<grid, kSkinTcThreads, kSkinTcSmemBytes, s>>>(m, n, w, vertices);
+  GLAMR_LAUNCH_CHECK();
+  return GLAMR_OK;
+}
 // blend features + blend GEMM for local frame-persons [0, n): v_posed (transposed) of the workspace
 // mt_begin / mt_end: the range of 128-frame tiles of the GEMM this call launches (mt_end < 0: all); features: also (re)build the A operand
 int launch_blend(const SmplDev& m, int n, const float* body_pose, const float* betas, const SmplWorkspace& w, cudaStream_t s, int mt_begin,
@@ -784,10 +859,7 @@ int launch_blend(const SmplDev& m, int n, const float* body_pose, const float* b
     blend_features_kernel<<<(n + 3) / 4, 128, 0, s>>>(n, body_pose, betas, w);
     GLAMR_LAUNCH_CHECK();
   }
-  if (mt_end > mt_begin) {
-    lbs_blend_tc_kernel<<<dim3(kTcNTiles, mt_end - mt_begin), kTcThreads, kTcSmemBytes, s>>>(m, w, mt_begin);
-    GLAMR_LAUNCH_CHECK();
-  }
+  if (mt_end > mt_begin) return launch_blend_gemm(m, n, w, s, mt_begin, mt_end, false);
   return GLAMR_OK;
 }
 // skinning of local frame-persons [0, n) from the workspace's v_posed and A
@@ -795,11 +867,7 @@ int launch_skin(const SmplDev& m, int n, const SmplWorkspace& w, float* vertices
   if (n <= 0) return GLAMR_OK;
   int rc;
   if ((rc = lbs_set_attrs())) return rc;
-  if (w.vp_tiled) {
-    lbs_skin_tc_kernel<<<dim3(kNVTiles, ((n + kSkF - 1) / kSkF + kSkTilesPerCta - 1) / kSkTilesPerCta), kSkinTcThreads, kSkinTcSmemBytes, s>>>(m, n, w, vertices);
-    GLAMR_LAUNCH_CHECK();
-    return GLAMR_OK;
-  }
+  if (w.vp_tiled) return launch_skin_tc(m, n, w, vertices, s, false);
   dim3 grid(kNVTiles, (n + kFramesPerCta - 1) / kFramesPerCta);
   if (m.K == 4) lbs_skin_kernel<4><<<grid, kLbsThreads, kSkinSmemBytes, s>>>(m, 0, n, w, vertices);
   else lbs_skin_kernel<0><<<grid, kLbsThreads, kSkinSmemBytes, s>>>(m, 0, n, w, vertices);
@@ -829,26 +897,13 @@ int launch_lbs(const SmplDev& m, int n_begin, int n_end, const float* betas, con
   }
   if (path >= 1 && m.tcB && w.tcA && n_begin == 0) {
     const int mtiles = (n_end + kTcM - 1) / kTcM;
-    if (w.vp_tiled) {
-      const dim3 sgrid(kNVTiles, ((n_end + kSkF - 1) / kSkF + kSkTilesPerCta - 1) / kSkTilesPerCta);
-      if (pdl) {
-        GLAMR_CUDA_TRY(launch_pdl(4, lbs_blend_tc_kernel, dim3(kTcNTiles, mtiles), dim3(kTcThreads), kTcSmemBytes, s, m, w, 0));
-        GLAMR_CUDA_TRY(launch_pdl(4, lbs_skin_tc_kernel, sgrid, dim3(kSkinTcThreads), kSkinTcSmemBytes, s, m, n_end, w, vertices));
-      } else {
-        lbs_blend_tc_kernel<<<dim3(kTcNTiles, mtiles), kTcThreads, kTcSmemBytes, s>>>(m, w, 0);
-        GLAMR_LAUNCH_CHECK();
-        lbs_skin_tc_kernel<<<sgrid, kSkinTcThreads, kSkinTcSmemBytes, s>>>(m, n_end, w, vertices);
-        GLAMR_LAUNCH_CHECK();
-      }
-      return GLAMR_OK;
-    }
+    int rc;
+    if ((rc = launch_blend_gemm(m, n_end, w, s, 0, mtiles, pdl))) return rc;
+    if (w.vp_tiled) return launch_skin_tc(m, n_end, w, vertices, s, pdl);
     if (pdl) {
-      GLAMR_CUDA_TRY(launch_pdl(4, lbs_blend_tc_kernel, dim3(kTcNTiles, mtiles), dim3(kTcThreads), kTcSmemBytes, s, m, w, 0));
       if (m.K == 4) GLAMR_CUDA_TRY(launch_pdl(4, lbs_skin_kernel<4>, grid, dim3(kLbsThreads), kSkinSmemBytes, s, m, n_begin, n_end, w, vertices));
       else GLAMR_CUDA_TRY(launch_pdl(4, lbs_skin_kernel<0>, grid, dim3(kLbsThreads), kSkinSmemBytes, s, m, n_begin, n_end, w, vertices));
     } else {
-      lbs_blend_tc_kernel<<<dim3(kTcNTiles, mtiles), kTcThreads, kTcSmemBytes, s>>>(m, w, 0);
-      GLAMR_LAUNCH_CHECK();
       if (m.K == 4) lbs_skin_kernel<4><<<grid, kLbsThreads, kSkinSmemBytes, s>>>(m, n_begin, n_end, w, vertices);
       else lbs_skin_kernel<0><<<grid, kLbsThreads, kSkinSmemBytes, s>>>(m, n_begin, n_end, w, vertices);
       GLAMR_LAUNCH_CHECK();
