@@ -573,7 +573,9 @@ __global__ void __launch_bounds__(kLbsThreads) lbs_skin_kernel(SmplDev m, int n_
 // blend stores v_posed frame-tiled for this).  Epilogue straight from the accumulator fragment: the quad of lanes that holds a
 // vertex row owns all 24 columns of a frame pair; each lane dots its column pairs with (x, y) or (z, 1) of v_posed and one
 // shuffle with the neighbouring lane completes an output coordinate -- no shared-memory traffic for the joint transforms, which
-// bounded the SIMT skinning (12 LDS.128 per vertex-frame).  warp 8 = producer.
+// bounded the SIMT skinning (12 LDS.128 per vertex-frame).  The epilogue has no branch before a row's stores: written with a
+// lane-dependent branch and a shuffle and store check per output, every output waited on the one before and the epilogue took
+// ~70 % of an item (tools/skin_phases_exp.py).  warp 8 = producer.
 // Persistent: a work item is one (vertex tile, frame tile) pair, numbered vertex-tile major, and CTA b of a grid of at most one CTA per
 // SM (the register file holds one) runs the contiguous item range [b items / grid, (b + 1) items / grid).  Every CTA gets within one
 // item of the average, which a fixed number of frame tiles per CTA could not give for every n, and its range spans at most two vertex
@@ -586,6 +588,31 @@ constexpr uint32_t kSkVBytes = kSkVpTileFloats * sizeof(float);       // 30,720
 constexpr size_t kSkinTcSmemBytes = (size_t)kSkWBytes + 2 * kSkBBytes + 2 * kSkVBytes + 128;
 
 constexpr int kSkinTcThreads = 288;     // warpgroups 0-1 consume (64 vertices each), warp 8 produces
+
+// Phase clock of the consumer warpgroups (tools/skin_phases_exp.py), experiment build only: each consumer thread adds the clock64
+// cycles since its previous stamp to a phase; lane 0 of the first warp of each warpgroup stores the sums of its CTA at the end.
+#ifdef GLAMR_EXPERIMENT
+constexpr int kSkinPhaseCtas = 1024;
+constexpr int kSkinPhases = 6;          // wait full_b | wgmma issue + retire wait | wait full_v | epilogue | other | items
+__device__ long long g_skin_phases[kSkinPhaseCtas][2][kSkinPhases];
+#define SKIN_CLOCK_INIT() long long sk_ph[kSkinPhases] = {}; long long sk_t = clock64()
+#define SKIN_CLOCK(k) do { const long long sk_now = clock64(); sk_ph[k] += sk_now - sk_t; sk_t = sk_now; } while (0)
+#define SKIN_CLOCK_STORE(items) do { sk_ph[kSkinPhases - 1] = (items);                                                              \
+    if ((warp & 3) == 0 && lane == 0 && blockIdx.x < kSkinPhaseCtas)                                                               \
+      for (int k = 0; k < kSkinPhases; ++k) g_skin_phases[blockIdx.x][g][k] = sk_ph[k]; } while (0)
+extern "C" int glamr_exp_skin_phases(long long* out) {     // the per-CTA sums of the skinning launches since the last call, then zeroed
+  void* p = nullptr;
+  GLAMR_CUDA_TRY(cudaDeviceSynchronize());
+  GLAMR_CUDA_TRY(cudaMemcpyFromSymbol(out, g_skin_phases, sizeof(g_skin_phases)));
+  GLAMR_CUDA_TRY(cudaGetSymbolAddress(&p, g_skin_phases));
+  GLAMR_CUDA_TRY(cudaMemset(p, 0, sizeof(g_skin_phases)));
+  return GLAMR_OK;
+}
+#else
+#define SKIN_CLOCK_INIT() do { } while (0)
+#define SKIN_CLOCK(k) do { } while (0)
+#define SKIN_CLOCK_STORE(items) do { } while (0)
+#endif
 
 __global__ void __launch_bounds__(kSkinTcThreads, 1) lbs_skin_tc_kernel(SmplDev m, int n, SmplWorkspace w, float* __restrict__ vertices) {
   extern __shared__ __align__(128) unsigned char sk_raw[];
@@ -647,6 +674,10 @@ __global__ void __launch_bounds__(kSkinTcThreads, 1) lbs_skin_tc_kernel(SmplDev 
     jrow[j] = (c0 - 12 * jf[j]) >> 2;
     jxy[j] = (c0 & 3) == 0;
   }
+  // the outputs this lane stores after the shuffles: even lanes j = 0 and 1, odd lanes j = 2 (frame offset sf, transform row srow)
+  const bool odd = (q & 1) == 1;
+  const int sf[2] = {odd ? jf[2] : jf[0], jf[1]}, srow[2] = {odd ? jrow[2] : jrow[0], jrow[1]};
+  SKIN_CLOCK_INIT();
   mbar_wait(full_w, 0);
   for (int i = i0, it = 0; i < i1; ++i, ++it) {
     const int vtile = i / nft, ftile = i - vtile * nft, vb = it & 1;
@@ -659,7 +690,9 @@ __global__ void __launch_bounds__(kSkinTcThreads, 1) lbs_skin_tc_kernel(SmplDev 
       ci[h] = m.compact_of_vertex[min(gv[h], kVPad - 1)];
       vrow[h] = Vs + vb * kSkVpTileFloats + (size_t)vl * 3 * kSkF;
     }
+    SKIN_CLOCK(4);
     mbar_wait(&full_b[vb], (it >> 1) & 1);
+    SKIN_CLOCK(0);
     float acc[kSkN / 2];
 #pragma unroll
     for (int k = 0; k < kSkN / 2; ++k) acc[k] = 0.0f;
@@ -677,36 +710,55 @@ __global__ void __launch_bounds__(kSkinTcThreads, 1) lbs_skin_tc_kernel(SmplDev 
     wgmma_commit();
     wgmma_wait<0>();
     wgmma_fence_acc(acc);
+    SKIN_CLOCK(1);
     __syncwarp();
     if (lane == 0) mbar_arrive(&b_empty[vb]);
+    SKIN_CLOCK(4);
     mbar_wait(&full_v[vb], (it >> 1) & 1);
+    SKIN_CLOCK(2);
+    // Epilogue, straight-line: per frame pair x, y, z of frames 2 p and 2 p + 1 are loaded once and lane-dependent selects stand in for
+    // branches, and a row is stored after all its outputs are computed, so the compiler can overlap the frame pairs; per output the same
+    // arithmetic as fmaf(t0, x, t1 * y) + fmaf(t0, z, t1) (t1 * 1.0f is exact).  Most rows store nothing: the optimiser keeps only
+    // the support vertices.
 #pragma unroll
     for (int h = 0; h < 2; ++h) {
-      const bool v_ok = gv[h] < kV;
+      const float2* const vr = reinterpret_cast<const float2*>(vrow[h]);   // [coordinate][10 frame pairs]
+      float o0[kSkF / 2], o1[kSkF / 2];                                     // the outputs this lane stores: j = 0 | 2 and j = 1
 #pragma unroll
       for (int p = 0; p < kSkF / 2; ++p) {
+        const float2 x = vr[p], y = vr[kSkF / 2 + p], z = vr[kSkF + p];
         float part[3];
 #pragma unroll
         for (int j = 0; j < 3; ++j) {
           const float t0 = acc[4 * (3 * p + j) + 2 * h], t1 = acc[4 * (3 * p + j) + 2 * h + 1];
-          const int f = 2 * p + jf[j];
-          part[j] = jxy[j] ? fmaf(t0, vrow[h][f], t1 * vrow[h][kSkF + f]) : fmaf(t0, vrow[h][2 * kSkF + f], t1);
-          part[j] += __shfl_xor_sync(0xffffffffu, part[j], 1);      // the neighbouring lane holds the other half of the row
+          const float xf = jf[j] ? x.y : x.x, yf = jf[j] ? y.y : y.x, zf = jf[j] ? z.y : z.x;
+          part[j] = fmaf(t0, jxy[j] ? xf : zf, t1 * (jxy[j] ? yf : 1.0f));
         }
 #pragma unroll
-        for (int j = 0; j < 3; ++j) {
-          if ((j == 2) != ((q & 1) == 1)) continue;                  // even lanes store j = 0, 1; odd lanes j = 2
-          const int fl = ftile * kSkF + 2 * p + jf[j];               // local frame-person index
-          if (fl < n && v_ok) {
-            if (vertices) vertices[((size_t)fl * kV + gv[h]) * 3 + jrow[j]] = part[j];
-            if (ci[h] >= 0) w.vcompact[((size_t)fl * m.S + ci[h]) * 3 + jrow[j]] = part[j];
+        for (int j = 0; j < 3; ++j) part[j] += __shfl_xor_sync(0xffffffffu, part[j], 1);   // the neighbouring lane holds the other half of the row
+        o0[p] = odd ? part[2] : part[0];
+        o1[p] = part[1];
+      }
+      const bool v_ok = gv[h] < kV;
+      if (v_ok && (vertices || ci[h] >= 0)) {
+#pragma unroll
+        for (int p = 0; p < kSkF / 2; ++p)
+#pragma unroll
+          for (int k = 0; k < 2; ++k) {
+            if (k == 1 && odd) continue;                               // even lanes store j = 0, 1; odd lanes j = 2
+            const int fl = ftile * kSkF + 2 * p + sf[k];               // local frame-person index
+            if (fl < n) {
+              if (vertices) vertices[((size_t)fl * kV + gv[h]) * 3 + srow[k]] = k ? o1[p] : o0[p];
+              if (ci[h] >= 0) w.vcompact[((size_t)fl * m.S + ci[h]) * 3 + srow[k]] = k ? o1[p] : o0[p];
+            }
           }
-        }
       }
     }
+    SKIN_CLOCK(3);
     __syncwarp();
     if (lane == 0) mbar_arrive(&v_empty[vb]);
   }
+  SKIN_CLOCK_STORE(i1 - i0);
 }
 
 // ------------------------------------------------------------------------------------------------ joints_finalize
