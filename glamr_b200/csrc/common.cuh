@@ -1,5 +1,6 @@
 // Shared device/host helpers for the glamr_b200 CUDA library (sm_90a only).
 #pragma once
+#include <cuda_fp16.h>
 #include <cuda_runtime.h>
 #include <stdint.h>
 #include <stdio.h>
@@ -53,14 +54,14 @@ constexpr int kNChunks = kPF / kChunkK;      // 23
 // k = 0..206 pose feature x posedirs, 207..216 betas x shapedirs, 217 = 1 x v_template, zero padded to 224
 constexpr int kTcFeat = kPF + kNB + 1;       // 218
 constexpr int kTcK = 224;                    // K padded to a multiple of the per-stage chunk
-constexpr int kTcChunkK = 8;                 // one wgmma tf32 step (k8) per pipeline stage
-constexpr int kTcChunks = kTcK / kTcChunkK;  // 28
+constexpr int kTcChunkK = 16;                // one wgmma f16 step (k16) per pipeline stage
+constexpr int kTcChunks = kTcK / kTcChunkK;  // 14
 constexpr int kTcM = 128;                    // frames per CTA tile (two consumer warpgroups of 64 rows)
 constexpr int kTcN = 256;                    // basis columns per CTA tile (wgmma N)
 constexpr int kTcNTiles = (kV * 3 + kTcN - 1) / kTcN;   // 81
 constexpr int kTcCols = kTcNTiles * kTcN;    // 20736
-constexpr int kTcAStageFloats = 2 * (kTcChunkK / 4) * kTcM * 4;   // hi | lo images of a [128 x 8] K-major core-matrix tile: 2048 floats
-constexpr int kTcBStageFloats = 2 * (kTcChunkK / 4) * kTcN * 4;   // 4096 floats
+constexpr int kTcAStageHalves = 2 * (kTcChunkK / 8) * kTcM * 8;   // hi | lo images of a [128 x 16] K-major core-matrix tile: 4096 halves
+constexpr int kTcBStageHalves = 2 * (kTcChunkK / 8) * kTcN * 8;   // 8192 halves
 // tensor-core skinning (lbs_skin_tc_kernel): T[vertex][frame x 12] = W[vertex][24 joints] . A[24 joints][frame x 12]
 constexpr int kSkF = 20;                     // frames per CTA tile
 constexpr int kSkN = kSkF * 12;              // 240 accumulator columns (wgmma N): the 3x4 blended transform of each frame
@@ -114,8 +115,9 @@ __device__ __forceinline__ void tma_bulk_g2s(void* smem_dst, const void* gsrc, u
 __device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
 __device__ __forceinline__ void pdl_launch_dependents() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
 
-// ---- wgmma helpers: shared-memory descriptor of a K-major, un-swizzled operand tile and one m64nNk8 tf32 MMA --------
-// The operand tile is stored as 8-row x 16-byte core matrices: element (r, k) at ((k / 4) * rows + r) * 16 + (k % 4) * 4 bytes.
+// ---- wgmma helpers: shared-memory descriptor of a K-major, un-swizzled operand tile and the m64nNk8 tf32 / m64nNk16 f16 MMAs --
+// The operand tile is stored as 8-row x 16-byte core matrices: element (r, k) at ((k / 4) * rows + r) * 16 + (k % 4) * 4 bytes
+// (tf32), ((k / 8) * rows + r) * 16 + (k % 8) * 2 bytes (f16).
 // rows = rows of the whole stored tile (it fixes the leading byte offset between 16-byte K groups); a warpgroup's 64-row slice
 // starts 64 * 16 bytes further in.
 __device__ __forceinline__ uint64_t wgmma_desc_kmajor_noswizzle(const void* smem_ptr, int rows) {
@@ -185,11 +187,28 @@ __device__ __forceinline__ void wgmma_m64n240k8_tf32(float (&d)[120], uint64_t d
         "+f"(d[112]), "+f"(d[113]), "+f"(d[114]), "+f"(d[115]), "+f"(d[116]), "+f"(d[117]), "+f"(d[118]), "+f"(d[119])
       : "l"(da), "l"(db), "r"(accumulate));
 }
-__device__ __forceinline__ void wgmma_m64n256k8_tf32(float (&d)[128], uint64_t da, uint64_t db, uint32_t accumulate) {
+// D[64 x N] (+)= A[64 x 16] B[N x 16]^T, both operands f16 in shared memory (K-major, the core-matrix layout above with 8 halves
+// per 16-byte row), FP32 accumulator with the fragment of the tf32 forms
+__device__ __forceinline__ void wgmma_m64n128k16_f16(float (&d)[64], uint64_t da, uint64_t db, uint32_t accumulate) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %66, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n128k16.f32.f16.f16 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, %64, %65, p, 1, 1, 0, 0;\n\t}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+        "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+        "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+        "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]),
+        "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]),
+        "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),
+        "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]),
+        "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+      : "l"(da), "l"(db), "r"(accumulate));
+}
+__device__ __forceinline__ void wgmma_m64n256k16_f16(float (&d)[128], uint64_t da, uint64_t db, uint32_t accumulate) {
   asm volatile(
       "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %130, 0;\n\t"
-      "wgmma.mma_async.sync.aligned.m64n256k8.f32.tf32.tf32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63, %64, %65, %66, %67, %68, %69, %70, %71, %72, %73, %74, %75, %76, %77, %78, %79, %80, %81, %82, %83, %84, %85, %86, %87, %88, %89, %90, %91, %92, %93, %94, %95, %96, %97, %98, %99, %100, %101, %102, %103, %104, %105, %106, %107, %108, %109, %110, %111, %112, %113, %114, %115, %116, %117, %118, %119, %120, %121, %122, %123, %124, %125, %126, %127}, %128, %129, p, 1, 1;\n\t}\n"
+      "wgmma.mma_async.sync.aligned.m64n256k16.f32.f16.f16 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63, %64, %65, %66, %67, %68, %69, %70, %71, %72, %73, %74, %75, %76, %77, %78, %79, %80, %81, %82, %83, %84, %85, %86, %87, %88, %89, %90, %91, %92, %93, %94, %95, %96, %97, %98, %99, %100, %101, %102, %103, %104, %105, %106, %107, %108, %109, %110, %111, %112, %113, %114, %115, %116, %117, %118, %119, %120, %121, %122, %123, %124, %125, %126, %127}, %128, %129, p, 1, 1, 0, 0;\n\t}\n"
       : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
         "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
         "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
@@ -217,6 +236,13 @@ __device__ __forceinline__ void split_tf32(float x, float& hi, float& lo) {
   hi = __uint_as_float(h);
   asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(l) : "f"(x - hi));
   lo = __uint_as_float(l);
+}
+// x s = hi + lo with hi = fp16(x s), lo = fp16(x s - hi), s a power of two: the operands of the 3xFP16 tensor-core products of the
+// blend.  While x s stays in FP16's normal range, hi and lo carry 11 significant bits each, the same split as a tf32 hi / lo pair.
+__device__ __forceinline__ void split_f16_scaled(float x, float s, __half& hi, __half& lo) {
+  const float xs = x * s;
+  hi = __float2half_rn(xs);
+  lo = __float2half_rn(xs - __half2float(hi));
 }
 
 __device__ __forceinline__ float warp_sum(float v) {

@@ -3,6 +3,8 @@
 // regression + joint remap + re-rooting (joints_finalize).  Reference arithmetic: smplx.lbs as stated in-tree at
 // HybrIK/hybrik/models/layers/smpl/lbs.py:195-288,402-548 and GLAMR's wrapper lib/models/smpl.py:289-343.
 #include <math.h>
+#include <algorithm>
+#include <cmath>
 #include <stdlib.h>
 #include <string.h>
 
@@ -299,67 +301,78 @@ lbs_kernel(SmplDev m, int n_begin, int n_end, const float* __restrict__ betas, S
 
 // ------------------------------------------------------------------------------------------------ blend features
 // The A operand of the blend GEMM for frame-person f: (R_j - I) of the 23 body joints (lbs.py:256-258), the betas, the constant 1
-// that multiplies v_template and zero padding, as tf32 hi / lo in the wgmma image (see pose_prep_frame).  It depends on the body
+// that multiplies v_template and zero padding, as scaled fp16 hi / lo in the wgmma image (put_blend_features).  It depends on the body
 // pose and the betas only -- NOT on the root orientation -- so the optimiser evaluates it (and the blend GEMM behind it) off the
 // critical path of the iteration.  One warp per frame-person.
 __global__ void __launch_bounds__(128) blend_features_kernel(int n, const float* __restrict__ body_pose, const float* __restrict__ betas, SmplWorkspace w) {
   const int f = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
   if (f >= n) return;
-  float* tile = w.tcA + (size_t)(f >> 7) * kTcChunks * kTcAStageFloats;
-  const int r = f & 127;
-  auto put = [&](int k, float v) {
-    float hi, lo;
-    split_tf32(v, hi, lo);
-    float* q = tile + (size_t)(k >> 3) * kTcAStageFloats + (((k >> 2) & 1) * kTcM + r) * 4 + (k & 3);
-    q[0] = hi;
-    q[kTcAStageFloats / 2] = lo;
-  };
+  float R[9];
   if (lane >= 1 && lane < kNJ) {
     const float* bp = body_pose + (size_t)f * 69 + (lane - 1) * 3;
     const float rv[3] = {bp[0], bp[1], bp[2]};
-    float R[9];
     rodrigues_smplx(rv, R);
-#pragma unroll
-    for (int k = 0; k < 9; ++k) put((lane - 1) * 9 + k, R[k] - ((k % 4 == 0) ? 1.0f : 0.0f));
-  } else if (lane == 0) {
-#pragma unroll
-    for (int l = 0; l < kNB; ++l) put(kPF + l, betas ? betas[(size_t)f * kNB + l] : 0.0f);
-    put(kPF + kNB, 1.0f);
-#pragma unroll
-    for (int k = kTcFeat; k < kTcK; ++k) put(k, 0.0f);
   }
+  put_blend_features(w, f, lane, R, betas ? betas + (size_t)f * kNB : nullptr);
 }
 
 // ------------------------------------------------------------------------------------------------ tensor-core LBS
 // The shape blend + pose blend of SMPL is one contraction  v_posed[frame, col] = sum_k feat[frame, k] basis[col, k]
 // (k: 207 pose features x posedirs | 10 betas x shapedirs | 1 x v_template; lbs.py:240,256-267), i.e. a [n x 218] x [218 x 20670]
-// GEMM.  lbs_blend_tc_kernel runs it on the Hopper tensor cores (wgmma) with FP32 accuracy (3xTF32: hi*hi + lo*hi + hi*lo,
-// |error| ~ 2e-7 on the blended vertex): both operands are PRE-SPLIT into tf32 hi / lo and pre-tiled in global memory as the
-// K-major core-matrix image wgmma reads from shared memory (basis once at glamr_smpl_create, features by pose_prep_frame), so a
-// pipeline stage is two 1-D bulk TMA copies (8 KB of A, 16 KB of B) with no SIMT work on the operand path.  Tile = 128 frames x
-// 256 basis columns, K in 28 steps of 8; warp 8 = TMA producer, warpgroups 0 and 1 = consumers (64 frames each, m64n256k8, the
-// accumulator in 128 registers per thread), which release a stage once the wgmma group that read it has retired and finally store
-// the accumulator TRANSPOSED ([column][frame]) so that lbs_skin_kernel (lanes = frames) reads contiguous bytes per vertex
-// coordinate.  8 stages x 24 KB = 192 KB of shared memory per CTA: with 4 stages the blend alone runs as fast, but the iteration of
+// GEMM.  lbs_blend_tc_kernel runs it on the Hopper tensor cores (wgmma) with FP32 accuracy (3xFP16: hi*hi + lo*hi + hi*lo,
+// |error| ~ 2e-7 on the blended vertex): both operands are scaled by powers of two (the basis by 2^e_B, feature row f by 2^e_f) into
+// FP16's normal range, where an fp16 hi / lo pair carries the 22 significant bits of a tf32 pair at twice the tensor-core rate and
+// half the bytes.  They are PRE-SPLIT and pre-tiled in global memory as the K-major core-matrix image wgmma reads from shared memory
+// (basis once at glamr_smpl_create, features by put_blend_features), so a pipeline stage is two 1-D bulk TMA copies (8 KB of A, 16 KB
+// of B) with no SIMT work on the operand path.  Tile = 128 frames x 256 basis columns, K in 14 steps of 16; warp 8 = TMA producer,
+// warpgroups 0 and 1 = consumers (64 frames each, m64n256k16, the accumulator in 128 registers per thread), which release a stage once
+// the wgmma group that read it has retired and finally multiply each row by its exact unscale factor 2^-(e_f + e_B) and store the
+// accumulator TRANSPOSED ([column][frame]) so that lbs_skin_kernel (lanes = frames) reads contiguous bytes per vertex coordinate.  8 stages x 24 KB = 192 KB of shared memory per CTA: with 4 stages the blend alone runs as fast, but the iteration of
 // 4 x 300 frame-persons, where the blend shares the GPU with the residual and backward kernels, is ~5 % slower.
 // Persistent: the grid has one CTA per SM (the register file holds one), and CTA b runs tiles b, b + grid, ...  The stage ring runs on
 // across tiles, so the producer fetches the next tile's first stages while the consumers store the current accumulator.  Tiles are
 // numbered column-tile major (frame tile fastest): the CTAs that read one 448 KB basis column tile run at the same time, and the
-// 36 MB basis leaves HBM about once per launch instead of once per frame tile.  A last frame tile with at most 64 frames is a half
-// tile: both warpgroups take its 64 rows, each for 128 of the 256 columns (m64n128k8) -- same products, same K order.
+// 18.6 MB basis leaves HBM about once per launch instead of once per frame tile.  A last frame tile with at most 64 frames is a half
+// tile: both warpgroups take its 64 rows, each for 128 of the 256 columns (m64n128k16) -- same products, same K order.
 constexpr int kTcStages = 8;
 constexpr int kTcThreads = 288;           // warpgroups 0-1 consume, warp 8 produces
-constexpr uint32_t kTcABytes = kTcAStageFloats * sizeof(float);      // 8,192
-constexpr uint32_t kTcBBytes = kTcBStageFloats * sizeof(float);      // 16,384
+constexpr uint32_t kTcABytes = kTcAStageHalves * sizeof(__half);     // 8,192
+constexpr uint32_t kTcBBytes = kTcBStageHalves * sizeof(__half);     // 16,384
 constexpr size_t kTcSmemBytes = (size_t)kTcStages * (kTcABytes + kTcBBytes) + 128;
+
+// Phase clock of the consumer warpgroups (tools/blend_phases_exp.py), experiment build only: each consumer thread adds the clock64
+// cycles since its previous stamp to a phase; lane 0 of the first warp of each warpgroup adds the sums of its CTA at the end of a launch.
+#ifdef GLAMR_EXPERIMENT
+constexpr int kBlendPhaseCtas = 1024;
+constexpr int kBlendPhases = 5;         // wait full | wgmma issue + retire wait | epilogue | other | tiles
+__device__ unsigned long long g_blend_phases[kBlendPhaseCtas][2][kBlendPhases];
+#define BLEND_CLOCK_INIT() long long bl_ph[kBlendPhases] = {}; long long bl_t = clock64()
+#define BLEND_CLOCK(k) do { const long long bl_now = clock64(); bl_ph[k] += bl_now - bl_t; bl_t = bl_now; } while (0)
+#define BLEND_CLOCK_TILE() (++bl_ph[kBlendPhases - 1])
+#define BLEND_CLOCK_STORE() do { if ((warp & 3) == 0 && lane == 0 && blockIdx.x < kBlendPhaseCtas)                                     \
+      for (int k = 0; k < kBlendPhases; ++k) atomicAdd(&g_blend_phases[blockIdx.x][g][k], (unsigned long long)bl_ph[k]); } while (0)
+extern "C" int glamr_exp_blend_phases(long long* out) {    // the per-CTA sums of the blend launches since the last call, then zeroed
+  void* p = nullptr;
+  GLAMR_CUDA_TRY(cudaDeviceSynchronize());
+  GLAMR_CUDA_TRY(cudaMemcpyFromSymbol(out, g_blend_phases, sizeof(g_blend_phases)));
+  GLAMR_CUDA_TRY(cudaGetSymbolAddress(&p, g_blend_phases));
+  GLAMR_CUDA_TRY(cudaMemset(p, 0, sizeof(g_blend_phases)));
+  return GLAMR_OK;
+}
+#else
+#define BLEND_CLOCK_INIT() do { } while (0)
+#define BLEND_CLOCK(k) do { } while (0)
+#define BLEND_CLOCK_TILE() do { } while (0)
+#define BLEND_CLOCK_STORE() do { } while (0)
+#endif
 
 // mtile0 / mtiles: the 128-frame tiles of this launch (the optimiser may split the blend in two launches); half_last: the last of them
 // holds at most 64 frames
 __global__ void __launch_bounds__(kTcThreads, 1) lbs_blend_tc_kernel(SmplDev m, SmplWorkspace w, int mtile0, int mtiles, int half_last) {
   extern __shared__ __align__(128) unsigned char tc_raw[];
-  float* As = reinterpret_cast<float*>(tc_raw);                                   // [stages][hi | lo][2][128][4]
-  float* Bs = As + kTcStages * kTcAStageFloats;                                   // [stages][hi | lo][2][256][4]
-  uint64_t* full = reinterpret_cast<uint64_t*>(Bs + kTcStages * kTcBStageFloats); // [stages]
+  __half* As = reinterpret_cast<__half*>(tc_raw);                                 // [stages][hi | lo][2][128][8]
+  __half* Bs = As + kTcStages * kTcAStageHalves;                                  // [stages][hi | lo][2][256][8]
+  uint64_t* full = reinterpret_cast<uint64_t*>(Bs + kTcStages * kTcBStageHalves); // [stages]
   uint64_t* empty = full + kTcStages;                                             // [stages]
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const int ntiles = kTcNTiles * mtiles;
@@ -376,27 +389,27 @@ __global__ void __launch_bounds__(kTcThreads, 1) lbs_blend_tc_kernel(SmplDev m, 
       // the basis is a model constant: the first stages of the first tile are requested before this grid waits for the kernel that
       // writes the features
       {
-        const float* gB = m.tcB + (size_t)(blockIdx.x / mtiles) * kTcChunks * kTcBStageFloats;
+        const __half* gB = m.tcB + (size_t)(blockIdx.x / mtiles) * kTcChunks * kTcBStageHalves;
         for (int c = 0; c < kTcStages; ++c) {
           mbar_expect_tx_only(&full[c], kTcBBytes);
-          tma_bulk_g2s(Bs + c * kTcBStageFloats, gB + (size_t)c * kTcBStageFloats, kTcBBytes, &full[c]);
+          tma_bulk_g2s(Bs + c * kTcBStageHalves, gB + (size_t)c * kTcBStageHalves, kTcBBytes, &full[c]);
         }
       }
       pdl_wait();
       int q = 0;                                                                  // stage uses so far (all tiles)
       for (int t = blockIdx.x; t < ntiles; t += gridDim.x) {
-        const float* gA = w.tcA + (size_t)(mtile0 + t % mtiles) * kTcChunks * kTcAStageFloats;
-        const float* gB = m.tcB + (size_t)(t / mtiles) * kTcChunks * kTcBStageFloats;
+        const __half* gA = w.tcA + (size_t)(mtile0 + t % mtiles) * kTcChunks * kTcAStageHalves;
+        const __half* gB = m.tcB + (size_t)(t / mtiles) * kTcChunks * kTcBStageHalves;
         for (int c = 0; c < kTcChunks; ++c, ++q) {
           const int s = q % kTcStages;
           if (q >= kTcStages) {
             mbar_wait(&empty[s], ((q / kTcStages) - 1) & 1);                     // the wgmma groups that read this stage have retired
             mbar_expect_tx(&full[s], kTcABytes + kTcBBytes);
-            tma_bulk_g2s(Bs + s * kTcBStageFloats, gB + (size_t)c * kTcBStageFloats, kTcBBytes, &full[s]);
+            tma_bulk_g2s(Bs + s * kTcBStageHalves, gB + (size_t)c * kTcBStageHalves, kTcBBytes, &full[s]);
           } else {
             mbar_expect_tx(&full[s], kTcABytes);
           }
-          tma_bulk_g2s(As + s * kTcAStageFloats, gA + (size_t)c * kTcAStageFloats, kTcABytes, &full[s]);
+          tma_bulk_g2s(As + s * kTcAStageHalves, gA + (size_t)c * kTcAStageHalves, kTcABytes, &full[s]);
         }
       }
     }
@@ -409,21 +422,24 @@ __global__ void __launch_bounds__(kTcThreads, 1) lbs_blend_tc_kernel(SmplDev m, 
   float* const vpb = vp_buffer(w);
   const size_t cstride = w.vp_tiled ? (size_t)kSkF : (size_t)w.mpad;
   int q = 0;
+  BLEND_CLOCK_INIT();
 #pragma unroll 1
   for (int t = blockIdx.x; t < ntiles; t += gridDim.x) {
     const int ntile = t / mtiles, mt = t % mtiles, mtile = mtile0 + mt;
     const bool half = half_last && mt == mtiles - 1;
     // full tile: A rows 64 g.., all 256 columns of B; half tile: A rows 0..63, B columns 128 g..
-    const int aoff = half ? 0 : g * 64 * 4, boff = half ? g * 128 * 4 : 0;
+    const int aoff = half ? 0 : g * 64 * 8, boff = half ? g * 128 * 8 : 0;
     auto mainloop = [&](auto& d, auto mma) {
 #pragma unroll 1
       for (int c = 0; c < kTcChunks; ++c, ++q) {
         const int s = q % kTcStages;
+        BLEND_CLOCK(3);
         mbar_wait(&full[s], (q / kTcStages) & 1);
-        const float* a = As + s * kTcAStageFloats + aoff;
-        const float* b = Bs + s * kTcBStageFloats + boff;
-        const uint64_t dah = wgmma_desc_kmajor_noswizzle(a, kTcM), dal = wgmma_desc_kmajor_noswizzle(a + kTcAStageFloats / 2, kTcM);
-        const uint64_t dbh = wgmma_desc_kmajor_noswizzle(b, kTcN), dbl = wgmma_desc_kmajor_noswizzle(b + kTcBStageFloats / 2, kTcN);
+        BLEND_CLOCK(0);
+        const __half* a = As + s * kTcAStageHalves + aoff;
+        const __half* b = Bs + s * kTcBStageHalves + boff;
+        const uint64_t dah = wgmma_desc_kmajor_noswizzle(a, kTcM), dal = wgmma_desc_kmajor_noswizzle(a + kTcAStageHalves / 2, kTcM);
+        const uint64_t dbh = wgmma_desc_kmajor_noswizzle(b, kTcN), dbl = wgmma_desc_kmajor_noswizzle(b + kTcBStageHalves / 2, kTcN);
         wgmma_fence();
         mma(d, dah, dbh, c > 0 ? 1u : 0u);
         mma(d, dal, dbh, 1u);
@@ -431,12 +447,14 @@ __global__ void __launch_bounds__(kTcThreads, 1) lbs_blend_tc_kernel(SmplDev m, 
         wgmma_commit();
         wgmma_wait<1>();                                                          // the group of the previous stage use has retired
         if (c > 0 && lane == 0) mbar_arrive(&empty[(q - 1) % kTcStages]);
+        BLEND_CLOCK(1);
       }
       wgmma_wait<0>();
       wgmma_fence_acc(d);
+      BLEND_CLOCK(1);
     };
-    if (half) mainloop(acc_half, [](float (&d)[kTcN / 4], uint64_t da, uint64_t db, uint32_t acc_in) { wgmma_m64n128k8_tf32(d, da, db, acc_in); });
-    else mainloop(acc, [](float (&d)[kTcN / 2], uint64_t da, uint64_t db, uint32_t acc_in) { wgmma_m64n256k8_tf32(d, da, db, acc_in); });
+    if (half) mainloop(acc_half, [](float (&d)[kTcN / 4], uint64_t da, uint64_t db, uint32_t acc_in) { wgmma_m64n128k16_f16(d, da, db, acc_in); });
+    else mainloop(acc, [](float (&d)[kTcN / 2], uint64_t da, uint64_t db, uint32_t acc_in) { wgmma_m64n256k16_f16(d, da, db, acc_in); });
     __syncwarp();
     if (lane == 0) mbar_arrive(&empty[(q - 1) % kTcStages]);                     // the tile's last stage: the producer moves on
     // ---- epilogue: d[4 i + 2 h + e] = D[16 (warp % 4) + lane / 4 + 8 h][8 i + 2 (lane % 4) + e]
@@ -448,17 +466,21 @@ __global__ void __launch_bounds__(kTcThreads, 1) lbs_blend_tc_kernel(SmplDev m, 
 #pragma unroll
     for (int h = 0; h < 2; ++h) {
       const int frame = row0 + 8 * h;                                             // < w.mpad by construction
+      const float unscale = w.tcUnscale[frame] * m.tcB_unscale;                   // 2^-(e_f + e_B): exact
       float* out = (w.vp_tiled ? vpb + ((size_t)(frame / kSkF) * kTcCols + (size_t)col0) * kSkF + frame % kSkF
                                : vpb + (size_t)col0 * w.mpad + frame) + (size_t)(2 * (lane & 3)) * cstride;
 #pragma unroll
       for (int i = 0; i < kTcN / 8; ++i) {
         if (8 * i < ncols) {
-          out[(size_t)(8 * i) * cstride] = acc[4 * i + 2 * h];
-          out[(size_t)(8 * i + 1) * cstride] = acc[4 * i + 2 * h + 1];
+          out[(size_t)(8 * i) * cstride] = acc[4 * i + 2 * h] * unscale;
+          out[(size_t)(8 * i + 1) * cstride] = acc[4 * i + 2 * h + 1] * unscale;
         }
       }
     }
+    BLEND_CLOCK(2);
+    BLEND_CLOCK_TILE();
   }
+  BLEND_CLOCK_STORE();
 }
 
 // Skinning of the blended vertices (lbs.py:273-284): CTA = 128 vertices x 32 frames, warp = 32 vertices, lane = frame.
@@ -567,8 +589,8 @@ __global__ void __launch_bounds__(kLbsThreads) lbs_skin_kernel(SmplDev m, int n_
 // ------------------------------------------------------------------------------------------------ tensor-core skinning
 // lbs.py:273-284 as a GEMM with a fused epilogue.  The blended transform of vertex v in frame f is T[v][f] = sum_j W[v][j] A_j[f]
 // (12 numbers), i.e. [128 vertices x 24 joints] x [24 joints x (20 frames x 12)] per CTA: two consumer warpgroups of 64 vertices,
-// each m64n240k8 with the accumulator in 120 registers per thread, K = 24 in three steps, 3xTF32 (hi*hi + lo*hi + hi*lo) like the
-// blend.  Both operands are pre-tiled wgmma images (W: model constant built at glamr_smpl_create; A: written by pose_prep_frame), so
+// each m64n240k8 with the accumulator in 120 registers per thread, K = 24 in three steps, 3xTF32 (hi*hi + lo*hi + hi*lo; the
+// blend's split, but in tf32).  Both operands are pre-tiled wgmma images (W: model constant built at glamr_smpl_create; A: written by pose_prep_frame), so
 // the whole operand traffic of a CTA is three bulk copies: W image 24 KB, A image 45 KB, and the 128 x 20 v_posed block 30 KB (the
 // blend stores v_posed frame-tiled for this).  Epilogue straight from the accumulator fragment: the quad of lanes that holds a
 // vertex row owns all 24 columns of a frame pair; each lane dots its column pairs with (x, y) or (z, 1) of v_posed and one
@@ -1065,8 +1087,9 @@ extern "C" int glamr_smpl_create(glamr_smpl_t** out, const float* v_template, co
       }
     if ((rc = upload(h, t, &d.pd_tiles))) goto fail;
   }
-  {  // blend basis [20736 cols][224 k] = posedirs^T | shapedirs | v_template, tf32 hi / lo, wgmma K-major core-matrix image per
-     // (256-column tile, 8-wide K chunk): [hi | lo][k group (4 wide)][256 cols][4]
+  {  // blend basis [20736 cols][224 k] = posedirs^T | shapedirs | v_template scaled by 2^e_B, fp16 hi / lo, wgmma K-major core-matrix
+     // image per (256-column tile, 16-wide K chunk): [hi | lo][k group (8 wide)][256 cols][8].  e_B brings max |basis| into
+     // [2^14, 2^15), so every entry above 2^-18 max |basis| keeps the 22 significant bits of its hi / lo pair in FP16's normal range.
     auto tf32_rna = [](float x) {            // cvt.rna.tf32.f32: round to nearest, ties away from zero, 10-bit mantissa
       uint32_t u;
       memcpy(&u, &x, 4);
@@ -1075,18 +1098,27 @@ extern "C" int glamr_smpl_create(glamr_smpl_t** out, const float* v_template, co
       memcpy(&r, &u, 4);
       return r;
     };
-    std::vector<float> img((size_t)kTcNTiles * kTcChunks * kTcBStageFloats, 0.0f);
+    auto basis = [&](int col, int k) {
+      if (k < kPF) return posedirs[(size_t)k * kV * 3 + col];
+      if (k < kPF + kNB) return shapedirs[(size_t)col * kNB + (k - kPF)];       // shapedirs [v][c][l] = [col][l]
+      return v_template[col];
+    };
+    float amax = 0.0f;
+    for (int col = 0; col < kV * 3; ++col)
+      for (int k = 0; k < kTcFeat; ++k) amax = std::max(amax, std::fabs(basis(col, k)));
+    int ex = 0;
+    if (amax > 0.0f && std::isfinite(amax)) std::frexp(amax, &ex);            // amax in [2^(ex-1), 2^ex)
+    const int e_B = amax > 0.0f && std::isfinite(amax) ? 15 - ex : 0;
+    d.tcB_unscale = std::ldexp(1.0f, -e_B);
+    std::vector<__half> img((size_t)kTcNTiles * kTcChunks * kTcBStageHalves, __float2half_rn(0.0f));
     for (int col = 0; col < kV * 3; ++col) {
       const int tile = col / kTcN, r = col % kTcN;
       for (int k = 0; k < kTcFeat; ++k) {
-        float v;
-        if (k < kPF) v = posedirs[(size_t)k * kV * 3 + col];
-        else if (k < kPF + kNB) v = shapedirs[(size_t)col * kNB + (k - kPF)];      // shapedirs [v][c][l] = [col][l]
-        else v = v_template[col];
-        const float hi = tf32_rna(v), lo = tf32_rna(v - hi);
-        float* q = &img[((size_t)tile * kTcChunks + (k >> 3)) * kTcBStageFloats + ((((k >> 2) & 1) * kTcN + r) * 4) + (k & 3)];
+        const float v = std::ldexp(basis(col, k), e_B);
+        const __half hi = __float2half_rn(v), lo = __float2half_rn(v - __half2float(hi));
+        __half* q = &img[((size_t)tile * kTcChunks + (k >> 4)) * kTcBStageHalves + ((((k >> 3) & 1) * kTcN + r) * 8) + (k & 7)];
         q[0] = hi;
-        q[kTcBStageFloats / 2] = lo;
+        q[kTcBStageHalves / 2] = lo;
       }
     }
     if ((rc = upload(h, img, &d.tcB))) goto fail;

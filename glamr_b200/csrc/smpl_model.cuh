@@ -9,9 +9,10 @@ struct SmplDev {
   // dense constants
   const float* pd_tiles;     // [54][207][384]  posedirs, vertex-tile major: one contiguous 13,824 B block per
                              //                 (tile, 9-row chunk) so a CTA streams its slab with 1-D bulk TMA
-  const float* tcB;          // [81 col tiles][28 K chunks][hi | lo][2 K groups][256 cols][4]  the blend basis (posedirs | shapedirs |
-                             //                 v_template) pre-split into tf32 hi / lo and pre-tiled as the wgmma K-major core-matrix image:
-                             //                 one contiguous 16 KB block per (tile, chunk) = one bulk copy per pipeline stage
+  const __half* tcB;         // [81 col tiles][14 K chunks][hi | lo][2 K groups][256 cols][8]  the blend basis (posedirs | shapedirs |
+                             //                 v_template) scaled by 2^e_B, pre-split into fp16 hi / lo and pre-tiled as the wgmma K-major
+                             //                 core-matrix image: one contiguous 16 KB block per (tile, chunk) = one bulk copy per stage
+  float tcB_unscale;         // 2^-e_B
   const float* skW;          // [54 vertex tiles][hi | lo][6 joint groups][128 vertices][4]  dense skinning weights W[v][24], tf32 hi / lo,
                              //                 wgmma K-major image: one contiguous 24 KB block per vertex tile (lbs_skin_tc_kernel)
   const float* v_template;   // [6912][3]  (padded with zeros)
@@ -42,8 +43,9 @@ struct SmplWorkspace {
   float* jposed;    // [n][24][3]   posed LBS joints
   float* vcompact;  // [n][S][3]    skinned support vertices
   float* root_raw;  // [n][3]       un-rooted joint 0 (for vertex re-rooting)
-  float* tcA;       // [n/128][28][hi | lo][2][128][4]  blend features (pose feature | betas | 1 | 0-pad), tf32 hi / lo, wgmma image per
-                    //              (128-frame tile, K chunk): 8 KB contiguous = one bulk copy per stage
+  __half* tcA;      // [n/128][14][hi | lo][2][128][8]  blend features (pose feature | betas | 1 | 0-pad), row f scaled by 2^e_f, fp16
+                    //              hi / lo, wgmma image per (128-frame tile, K chunk): 8 KB contiguous = one bulk copy per stage
+  float* tcUnscale; // [mpad]  2^-e_f of each feature row
   float* vpT;       // [20736][mpad]  blended vertices v_posed, TRANSPOSED (column-major over frames) so that the skinning kernel's
                     //              lanes = frames read 128 contiguous bytes per vertex coordinate
   int mpad;         // frames padded to a multiple of 128
@@ -67,7 +69,7 @@ inline size_t smpl_workspace_floats(int n, int S) {
   const size_t n32 = ((size_t)n + 31) / 32 * 32;   // the pose feature is tile-major over whole 32-frame tiles
   const size_t n128 = ((size_t)n + kTcM - 1) / kTcM * kTcM;
   return (size_t)n * (kNJ * 3 + (size_t)S * 3 + 3) + n32 * (kPFPad + kNJ * 12) + 64 + 64 +
-         (n128 / kTcM) * kTcChunks * kTcAStageFloats + (size_t)kTcCols * ((n128 + kSkF - 1) / kSkF * kSkF) +
+         (n128 / kTcM) * kTcChunks * kTcAStageHalves / 2 + n128 + (size_t)kTcCols * ((n128 + kSkF - 1) / kSkF * kSkF) +
          ((n128 + kSkF - 1) / kSkF) * kSkBImageFloats + 64;
 }
 int lbs_path();                              // 2 tensor-core blend + tensor-core skinning, 1 tensor-core blend + SIMT skinning, 0 one-kernel FP32 SIMT path
@@ -81,7 +83,8 @@ inline SmplWorkspace smpl_carve_workspace(void* base, int n, int S) {
   w.root_raw = p; p += (size_t)n * 3;
   p = (float*)(((uintptr_t)p + 255) & ~(uintptr_t)255);          // bulk-copy sources: 16-byte aligned (256 for good measure)
   w.mpad = (int)(((size_t)n + kTcM - 1) / kTcM * kTcM);
-  w.tcA = p; p += (size_t)(w.mpad / kTcM) * kTcChunks * kTcAStageFloats;
+  w.tcA = reinterpret_cast<__half*>(p); p += (size_t)(w.mpad / kTcM) * kTcChunks * kTcAStageHalves / 2;
+  w.tcUnscale = p; p += w.mpad;
   w.skB = p; p += (size_t)((w.mpad + kSkF - 1) / kSkF) * kSkBImageFloats;
   w.vpT = p;                                   // [20736][mpad] or, frame-tiled, [ceil(mpad/20)][20736][20]
   w.vp_tiled = lbs_path() == 2 ? 1 : 0;
@@ -95,6 +98,42 @@ __device__ __forceinline__ float* vp_buffer(const SmplWorkspace& w) {
   if (!w.vpT2) return w.vpT;
   return ((((int)*w.flip_src) + w.flip_add) & 1) ? w.vpT2 : w.vpT;
 }
+// The blend features of frame-person f (smpl_kernels.cu, lbs_blend_tc_kernel): lane 1..23 writes (R - I) of joint `lane` (R: its
+// rotation), lane 0 the betas (beta: 10 floats or nullptr = zeros), the constant 1 that multiplies v_template and the zero padding,
+// and the row's unscale factor.  The row is scaled by the power of two 2^e_f that brings m = max(2, max_l |beta_l|) into
+// [2^14, 2^15): |R - I| <= 2 and 1 <= m bound every other feature, so each scaled feature lies below 2^15 and its hi / lo pair misses
+// it by at most about 2^-22 of its value or 2^-39 m (the FP16 subnormal spacing), whichever is larger.  Every lane derives e_f from the
+// betas itself.
+__device__ __forceinline__ void put_blend_features(const SmplWorkspace& w, int f, int lane, const float* R, const float* __restrict__ beta) {
+  float m = 2.0f;
+  if (beta) {
+#pragma unroll
+    for (int l = 0; l < kNB; ++l) m = fmaxf(m, fabsf(beta[l]));
+  }
+  const int e = 14 - ((int)((__float_as_uint(m) >> 23) & 0xFF) - 127);
+  const float scale = ldexpf(1.0f, e);
+  __half* tile = w.tcA + (size_t)(f >> 7) * kTcChunks * kTcAStageHalves;
+  const int r = f & 127;
+  auto put = [&](int k, float v) {
+    __half hi, lo;
+    split_f16_scaled(v, scale, hi, lo);
+    __half* q = tile + (size_t)(k >> 4) * kTcAStageHalves + (((k >> 3) & 1) * kTcM + r) * 8 + (k & 7);
+    q[0] = hi;
+    q[kTcAStageHalves / 2] = lo;
+  };
+  if (lane >= 1 && lane < kNJ) {
+#pragma unroll
+    for (int k = 0; k < 9; ++k) put((lane - 1) * 9 + k, R[k] - ((k % 4 == 0) ? 1.0f : 0.0f));
+  } else if (lane == 0) {
+#pragma unroll
+    for (int l = 0; l < kNB; ++l) put(kPF + l, beta ? beta[l] : 0.0f);
+    put(kPF + kNB, 1.0f);
+#pragma unroll
+    for (int k = kTcFeat; k < kTcK; ++k) put(k, 0.0f);
+    w.tcUnscale[f] = ldexpf(1.0f, -e);
+  }
+}
+
 // un-rooted joint `idx` of [24 LBS | picks | extra regressed] for local frame-person f  (lib/models/smpl.py:299-301)
 __device__ __forceinline__ void raw_joint(const SmplDev& m, const SmplWorkspace& w, int f, int idx, float* o) {
   if (idx < kNJ) {
@@ -152,29 +191,7 @@ __device__ __forceinline__ void pose_prep_frame(const SmplDev& m, int f, const f
 #pragma unroll
     for (int k = 0; k < 9; ++k) pf[k * 32] = R[k] - ((k % 4 == 0) ? 1.0f : 0.0f);
   }
-  if (w.tcA) {
-    // the same features (+ betas, + the constant 1 that multiplies v_template, + zero padding) as the A operand of the
-    // tensor-core blend GEMM: tf32 hi / lo, K-major core-matrix image of this frame's 128-frame tile
-    float* tile = w.tcA + (size_t)(f >> 7) * kTcChunks * kTcAStageFloats;
-    const int r = f & 127;
-    auto put = [&](int k, float v) {
-      float hi, lo;
-      split_tf32(v, hi, lo);
-      float* q = tile + (size_t)(k >> 3) * kTcAStageFloats + (((k >> 2) & 1) * kTcM + r) * 4 + (k & 3);
-      q[0] = hi;
-      q[kTcAStageFloats / 2] = lo;
-    };
-    if (lane >= 1 && lane < kNJ) {
-#pragma unroll
-      for (int k = 0; k < 9; ++k) put((lane - 1) * 9 + k, R[k] - ((k % 4 == 0) ? 1.0f : 0.0f));
-    } else if (lane == 0) {
-#pragma unroll
-      for (int l = 0; l < kNB; ++l) put(kPF + l, beta ? beta[l] : 0.0f);
-      put(kPF + kNB, 1.0f);
-#pragma unroll
-      for (int k = kTcFeat; k < kTcK; ++k) put(k, 0.0f);
-    }
-  }
+  if (w.tcA) put_blend_features(w, f, lane, R, beta);   // the same features as the A operand of the tensor-core blend GEMM
 
   float GR[9], Gt[3];
 #pragma unroll
