@@ -123,15 +123,20 @@ GLAMR_HD void local_quat(const float* d6, float heading, float* q_hl, float* loc
   aa_to_quat(ha, hq);
   quat_mul(hq, local_q, q_hl);
 }
-// world pose of absolute frame t from its traj_local row `tl`, scanned heading and scanned xy (ignored outside the exist range);
-// writes orient/trans base + world of frame-person n, returns nothing else
+// Does local frame i of person ps come out of the trajectory codec?  With GLAMR_TRAJ_BASE no frame does: the base pose is the
+// constant one init left (global_recon_model.py:448-449 not taken).
+GLAMR_HD bool traj_codec_frame(const OptCtx& c, const glamr_person_t& ps, int i) {
+  return c.pb.traj_source == GLAMR_TRAJ_PREDICTED && i >= 0 && i < ps.len;
+}
+// world pose of absolute frame t from its traj_local row `tl`, scanned heading and scanned xy (ignored for frames the codec does not
+// produce); writes orient/trans base + world of frame-person n, returns nothing else
 GLAMR_HD void traj_post_vals(const OptCtx& c, int p, int t, const float* tl, float heading, float x, float y, float* ow_out) {
   const glamr_person_t& ps = c.pb.persons[p];
   const int T = c.pb.T;
   const int n = p * T + t;
   const int i = t - ps.start;
   float ob[3], tb[3];
-  if (i >= 0 && i < ps.len) {
+  if (traj_codec_frame(c, ps, i)) {
     float q_hl[4], lq[4], hq[4], q[4];
     local_quat(tl + 3, heading, q_hl, lq, hq);
     const float base[4] = {0.5f, 0.5f, 0.5f, 0.5f};
@@ -176,7 +181,7 @@ GLAMR_HD void traj_post(const OptCtx& c, int p, int t) {
   const int n = p * c.pb.T + t;
   const int i = t - ps.start;
   float* tl = c.sc.traj_local + (size_t)n * 11;
-  if (i >= 0 && i < ps.len) {
+  if (traj_codec_frame(c, ps, i)) {
     traj_post_vals(c, p, t, tl, c.sc.heading[n], c.sc.xy[2 * (size_t)n], c.sc.xy[2 * (size_t)n + 1], nullptr);
   } else {
     for (int k = 0; k < 11; ++k) tl[k] = 0.0f;
@@ -891,7 +896,26 @@ GLAMR_HD void traj_back_pre(const OptCtx& c, int p, int t, TermAcc& acc) {
     aa_to_quat_vjp(ob, gbq, g_ob);
   }
   float g_heading = 0.0f, g_x = 0.0f, g_y = 0.0f;
-  if (i >= 0 && i < ps.len) {
+  if (!traj_codec_frame(c, ps, i) && i >= 0 && i < ps.len) {
+    // GLAMR_TRAJ_BASE: no codec reads traj_local_rot / traj_local_z, only their regularisers do (loss_func.py:233-237)
+    float ssr = 0.0f;
+#pragma unroll
+    for (int k = 0; k < 6; ++k) {
+      const float x = c.theta[ps.off_rot + 6 * i + k];
+      float g = 0.0f;
+      if (pb.owner) { ssr += x * x; g = 2.0f * kFps2 * c.gs[GLAMR_T_ROT_REG] * x; }
+      c.sc.grad[ps.off_rot + 6 * i + k] = g;
+    }
+    const float x = c.theta[ps.off_z + i];
+    float g = 0.0f;
+    if (pb.owner) {
+      g = 2.0f * kFps2 * c.gs[GLAMR_T_Z_REG] * x;
+      if (pb.term_enabled[GLAMR_T_Z_REG]) acc.v[GLAMR_T_Z_REG] += (double)(kFps2 * x * x);
+      if (pb.term_enabled[GLAMR_T_ROT_REG]) acc.v[GLAMR_T_ROT_REG] += (double)(kFps2 * ssr);
+    }
+    c.sc.grad[ps.off_z + i] = g;
+  }
+  if (traj_codec_frame(c, ps, i)) {
     const float* tl = c.sc.traj_local + n * 11;
     float q_hl[4], lq[4], hq[4], q[4], gq[4], gq_hl[4], ghq[4], glq[4];
     local_quat(tl + 3, c.sc.heading[n], q_hl, lq, hq);
@@ -934,19 +958,25 @@ GLAMR_HD void traj_back_pre(const OptCtx& c, int p, int t, TermAcc& acc) {
   c.sc.g_xy[2 * n + 1] = g_y;
   c.sc.g_head[n] = g_heading;
 }
-// after the reverse inclusive scan of g_xy over the local frames: rot_2d backward (traj_utils.py:7-11,:76)
+// after the reverse inclusive scan of g_xy over the local frames: rot_2d backward (traj_utils.py:7-11,:76).
+// GLAMR_TRAJ_BASE (no scans ran): the xy / dxy variables get their regulariser gradient only.
 GLAMR_HD void traj_back_mid(const OptCtx& c, int p, int i, TermAcc& acc) {
   const glamr_problem_t& pb = c.pb;
   const glamr_person_t& ps = pb.persons[p];
   const size_t n = (size_t)p * pb.T + ps.start + i;
-  const float Gx = c.sc.g_xy[2 * n], Gy = c.sc.g_xy[2 * n + 1];
+  const bool codec = pb.traj_source == GLAMR_TRAJ_PREDICTED;
+  const float Gx = codec ? c.sc.g_xy[2 * n] : 0.0f, Gy = codec ? c.sc.g_xy[2 * n + 1] : 0.0f;
   if (i == 0) {
     c.sc.grad[ps.off_xy] = Gx;
     c.sc.grad[ps.off_xy + 1] = Gy;
   } else {
-    const float t = c.sc.heading[n - 1];
-    const float ct = cosf(t), st = sinf(t);
-    float gx = Gx * ct + Gy * st, gy = -Gx * st + Gy * ct;
+    float gx = 0.0f, gy = 0.0f;
+    if (codec) {
+      const float t = c.sc.heading[n - 1];
+      const float ct = cosf(t), st = sinf(t);
+      gx = Gx * ct + Gy * st;
+      gy = -Gx * st + Gy * ct;
+    }
     const float x = c.theta[ps.off_dxy + 2 * (i - 1)], y = c.theta[ps.off_dxy + 2 * (i - 1) + 1];
     if (pb.owner) {
       gx += 2.0f * kFps2 * c.gs[GLAMR_T_DXY_REG] * x;
@@ -957,7 +987,7 @@ GLAMR_HD void traj_back_mid(const OptCtx& c, int p, int i, TermAcc& acc) {
     c.sc.grad[ps.off_dxy + 2 * (i - 1) + 1] = gy;
   }
   // heading[i] rotates d_xy of frame i+1: add that dependence to this frame's own heading gradient
-  if (i + 1 < ps.len) {
+  if (codec && i + 1 < ps.len) {
     const float* tl = c.sc.traj_local + (n + 1) * 11;
     const float Gx1 = c.sc.g_xy[2 * (n + 1)], Gy1 = c.sc.g_xy[2 * (n + 1) + 1];
     const float t = c.sc.heading[n];
@@ -966,11 +996,12 @@ GLAMR_HD void traj_back_mid(const OptCtx& c, int p, int i, TermAcc& acc) {
   }
 }
 // after the reverse inclusive scan of g_head: heading variables + dheading regularisers (loss_func.py:216-230)
+// GLAMR_TRAJ_BASE (no scan ran): the regularisers only
 GLAMR_HD void traj_back_post(const OptCtx& c, int p, int i, TermAcc& acc) {
   const glamr_problem_t& pb = c.pb;
   const glamr_person_t& ps = pb.persons[p];
   const size_t n = (size_t)p * pb.T + ps.start + i;
-  const float G = c.sc.g_head[n];
+  const float G = pb.traj_source == GLAMR_TRAJ_PREDICTED ? c.sc.g_head[n] : 0.0f;
   if (i == 0) {
     c.sc.grad[ps.off_heading] = G;
   } else {

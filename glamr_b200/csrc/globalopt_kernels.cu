@@ -66,15 +66,17 @@ __global__ void __launch_bounds__(kScanThreads) traj_cam_forward_kernel(OptCtx c
   const glamr_person_t& ps = c.pb.persons[p];
   const int len = ps.len, T = c.pb.T;
   const size_t n0 = (size_t)p * T + ps.start;
-  for (int i = threadIdx.x; i < len; i += kScanThreads) traj_pre(c, p, i);
-  __syncthreads();
-  block_scan_inplace(c.sc.heading + n0, len, 1, false, sm);
-  __syncthreads();
-  for (int i = threadIdx.x; i < len; i += kScanThreads) traj_mid(c, p, i);
-  __syncthreads();
-  block_scan_inplace(c.sc.xy + 2 * n0, len, 2, false, sm);
-  block_scan_inplace(c.sc.xy + 2 * n0 + 1, len, 2, false, sm);
-  __syncthreads();
+  if (c.pb.traj_source == GLAMR_TRAJ_PREDICTED) {          // uniform over the grid: the barriers below stay CTA-wide
+    for (int i = threadIdx.x; i < len; i += kScanThreads) traj_pre(c, p, i);
+    __syncthreads();
+    block_scan_inplace(c.sc.heading + n0, len, 1, false, sm);
+    __syncthreads();
+    for (int i = threadIdx.x; i < len; i += kScanThreads) traj_mid(c, p, i);
+    __syncthreads();
+    block_scan_inplace(c.sc.xy + 2 * n0, len, 2, false, sm);
+    block_scan_inplace(c.sc.xy + 2 * n0 + 1, len, 2, false, sm);
+    __syncthreads();
+  }
   for (int t = threadIdx.x; t < T; t += kScanThreads) traj_post(c, p, t);
 }
 
@@ -262,15 +264,20 @@ __global__ void __launch_bounds__(kScanThreads) traj_cam_backward_kernel(OptCtx 
     const glamr_person_t& ps = c.pb.persons[p];
     const int len = ps.len, T = c.pb.T;
     const size_t n0 = (size_t)p * T + ps.start;
+    const bool codec = c.pb.traj_source == GLAMR_TRAJ_PREDICTED;     // GLAMR_TRAJ_BASE: no reverse scans
     for (int t = threadIdx.x; t < T; t += kScanThreads) traj_back_pre(c, p, t, acc);
     __syncthreads();
-    block_scan_inplace(c.sc.g_xy + 2 * n0, len, 2, true, sm);
-    block_scan_inplace(c.sc.g_xy + 2 * n0 + 1, len, 2, true, sm);
-    __syncthreads();
+    if (codec) {
+      block_scan_inplace(c.sc.g_xy + 2 * n0, len, 2, true, sm);
+      block_scan_inplace(c.sc.g_xy + 2 * n0 + 1, len, 2, true, sm);
+      __syncthreads();
+    }
     for (int i = threadIdx.x; i < len; i += kScanThreads) traj_back_mid(c, p, i, acc);
     __syncthreads();
-    block_scan_inplace(c.sc.g_head + n0, len, 1, true, sm);
-    __syncthreads();
+    if (codec) {
+      block_scan_inplace(c.sc.g_head + n0, len, 1, true, sm);
+      __syncthreads();
+    }
     for (int i = threadIdx.x; i < len; i += kScanThreads) traj_back_post(c, p, i, acc);
   }
   block_reduce_terms(acc, partial_traj + (size_t)blockIdx.x * GLAMR_NUM_TERMS, smd);
@@ -410,7 +417,8 @@ __global__ void __launch_bounds__(kScanThreads) forward_pose_kernel(OptCtx c, Sm
   const int t0 = j * kFwdFrames, t1 = min(t0 + kFwdFrames, T);
   const glamr_person_t& ps = c.pb.persons[p];
   const int len = ps.len, start = ps.start;
-  const int cnt = min(len, t1 - start);               // local frames [0, cnt) feed this chunk's prefix sums (<= 0: chunk precedes the track)
+  // local frames [0, cnt) feed this chunk's prefix sums (<= 0: chunk precedes the track, or GLAMR_TRAJ_BASE: no codec at all)
+  const int cnt = c.pb.traj_source == GLAMR_TRAJ_PREDICTED ? min(len, t1 - start) : 0;
   float* s_head = fwd_dyn;
   float* s_x = fwd_dyn + lpad;
   float* s_y = fwd_dyn + 2 * lpad;
@@ -442,7 +450,7 @@ __global__ void __launch_bounds__(kScanThreads) forward_pose_kernel(OptCtx c, Sm
     const int t = t0 + tid, i = t - start;
     const size_t n = (size_t)p * T + t;
     float tl[11], head = 0.0f, x = 0.0f, y = 0.0f;
-    if (i >= 0 && i < len) {
+    if (traj_codec_frame(c, ps, i)) {
       traj_pre_vals(c, p, i, tl);
       head = s_head[i]; x = s_x[i]; y = s_y[i];
       c.sc.heading[n] = head;
@@ -584,15 +592,20 @@ __global__ void __launch_bounds__(kScanThreads) residuals_backward_kernel(OptCtx
     }
     __syncthreads();
     // ---- phase B2: reverse trajectory codec
+    const bool codec = c.pb.traj_source == GLAMR_TRAJ_PREDICTED;     // GLAMR_TRAJ_BASE: no reverse scans
     for (int t = tid; t < T; t += kScanThreads) traj_back_pre(c, p, t, acc);
     __syncthreads();
-    block_scan_inplace(c.sc.g_xy + 2 * nb, len, 2, true, sm);
-    block_scan_inplace(c.sc.g_xy + 2 * nb + 1, len, 2, true, sm);
-    __syncthreads();
+    if (codec) {
+      block_scan_inplace(c.sc.g_xy + 2 * nb, len, 2, true, sm);
+      block_scan_inplace(c.sc.g_xy + 2 * nb + 1, len, 2, true, sm);
+      __syncthreads();
+    }
     for (int i = tid; i < len; i += kScanThreads) traj_back_mid(c, p, i, acc);
     __syncthreads();
-    block_scan_inplace(c.sc.g_head + nb, len, 1, true, sm);
-    __syncthreads();
+    if (codec) {
+      block_scan_inplace(c.sc.g_head + nb, len, 1, true, sm);
+      __syncthreads();
+    }
     for (int i = tid; i < len; i += kScanThreads) traj_back_post(c, p, i, acc);
     block_reduce_terms(acc, a.partial + (size_t)p * GLAMR_NUM_TERMS, smd);
     __syncthreads();                            // this CTA's gradient stores are visible to all of its threads
@@ -695,6 +708,7 @@ static OptCtx make_ctx(const glamr_opt* st, const float* theta, float* grad) {
 extern "C" int glamr_opt_create(glamr_opt_t** out, const glamr_smpl_t* smpl, const glamr_problem_t* pb) {
   if (!out || !smpl || !pb || pb->P <= 0 || pb->T <= 0 || pb->J <= 0 || pb->n_params <= 0) return GLAMR_EINVAL;
   if (pb->J != smpl->dev.n_map) return GLAMR_EINVAL;
+  if (pb->traj_source != GLAMR_TRAJ_PREDICTED && pb->traj_source != GLAMR_TRAJ_BASE) return GLAMR_EINVAL;
   glamr_opt* st = (glamr_opt*)calloc(1, sizeof(glamr_opt));
   if (!st) return GLAMR_EINVAL;
   st->smpl = smpl->dev;
@@ -866,6 +880,7 @@ static int join_pending(glamr_opt_t* st, cudaStream_t s);
 extern "C" int glamr_opt_set_problem(glamr_opt_t* st, const glamr_problem_t* pb, int reset_adam, void* stream) {
   if (!st || !pb) return GLAMR_EINVAL;
   if (pb->P != st->pb.P || pb->T != st->pb.T || pb->J != st->pb.J || pb->n_params != st->pb.n_params) return GLAMR_EINVAL;
+  if (pb->traj_source != GLAMR_TRAJ_PREDICTED && pb->traj_source != GLAMR_TRAJ_BASE) return GLAMR_EINVAL;
   {
     const int rc = join_pending(st, (cudaStream_t)stream);
     if (rc) return rc;

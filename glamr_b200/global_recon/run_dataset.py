@@ -82,7 +82,8 @@ def run(args, make_model=None, make_in_dict=None):
             from glamr_b200.synthetic import make_smpl_assets
             from glamr_b200.synthetic_nets import make_prior_states
             smpl = SMPL(make_smpl_assets(0), device=device)
-            mt = MotionTrajJointModel(None, device, None, smpl=smpl, states=make_prior_states(1234))
+            if cfg.grecon_model_specs.get('flag_infer_motion_traj', False):      # no learned prior without it
+                mt = MotionTrajJointModel(None, device, None, smpl=smpl, states=make_prior_states(1234))
         model = model_dict[cfg.grecon_model_name](cfg, device, None, smpl=smpl, mt_model=mt)
     else:
         model = make_model(cfg, local)

@@ -28,6 +28,7 @@ TERM_INDEX = {
     'cam_up_reg': 17, 'cam_rot_smoothness': 18, 'cam_trans_smoothness': 19, 'cam_depth_smoothness': 20,
 }
 CAM_CONST, CAM_PER_FRAME, CAM_FIXED, CAM_FROM_PERSONS = 0, 1, 2, 3
+TRAJ_PREDICTED, TRAJ_BASE = 0, 1          # enum glamr_traj_source
 (R_ORIENT_WORLD, R_TRANS_WORLD, R_ORIENT_BASE, R_TRANS_BASE, R_KP_PRED, R_ORIENT_CIW, R_TRANS_CIW, R_CAM_POSE,
  R_CAM_POSE_INV, R_JOINTS_WORLD, R_TRAJ_LOCAL) = range(11)
 
@@ -53,7 +54,8 @@ class Person(ctypes.Structure):
 class Problem(ctypes.Structure):
     _fields_ = [(n, ctypes.c_int32) for n in
                 ['P', 'T', 'J', 'cam_mode', 'off_cam_rot', 'off_cam_trans', 'use_world_res', 'has_world_dheading',
-                 'trans_res_all', 'cam_up_first_only', 'n_params', 'n_begin', 'n_end', 'owner', 'cam_traj_rot_quat', 'traj_rot_smooth_quat']] + \
+                 'trans_res_all', 'cam_up_first_only', 'n_params', 'n_begin', 'n_end', 'owner', 'cam_traj_rot_quat', 'traj_rot_smooth_quat',
+                 'traj_source']] + \
                [('cam_up_first_weight', ctypes.c_float), ('rel_trans_weight', ctypes.c_float),
                 ('term_weight', ctypes.c_float * NUM_TERMS), ('term_norm', ctypes.c_float * NUM_TERMS),
                 ('term_enabled', ctypes.c_int32 * NUM_TERMS), ('term_monitor', ctypes.c_int32 * NUM_TERMS)] + \

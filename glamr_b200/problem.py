@@ -64,11 +64,17 @@ class StageCompiler:
 
     def __init__(self, data, layout, flags, device, aa_to_rot6d, num_joints=26, aa_to_quat=None):
         """flags: dict with flag_fixed_cam, flag_opt_cam, flag_opt_cam_from_person_pose, flag_cam_inv_trans_res_all,
-        flag_opt_vis_local_rot, cam_fix_frames.  aa_to_rot6d: callable (device math lives in the CUDA library)."""
+        flag_opt_vis_local_rot, cam_fix_frames and optionally flag_opt_traj / traj_source (when absent they are read off
+        `data`: a predicted trajectory leaves traj_local_pred, flag_opt_traj leaves the world_res variables).
+        aa_to_rot6d: callable (device math lives in the CUDA library)."""
         self.data, self.layout, self.flags, self.device, self.J = data, layout, flags, device, num_joints
         self.pids = list(data['person_data'].keys())
         self.P, self.T = len(self.pids), data['seq_len']
         T, dev = self.T, device
+        persons = [data['person_data'][pid] for pid in self.pids]
+        self.traj_source = flags.get('traj_source', L.TRAJ_PREDICTED if all('traj_local_pred' in d for d in persons) else L.TRAJ_BASE)
+        self.opt_traj = flags.get('flag_opt_traj', all('smpl_orient_world_res' in d for d in persons))
+        self.has_local = all('traj_local_xy' in d for d in persons)        # created with flag_opt_traj and flag_pred_traj (:185-199)
         self.keep = []                               # tensors whose storage the structs point into
         self.const = []
         pose_all, beta_all, scale_all = [], [], []
@@ -80,7 +86,8 @@ class StageCompiler:
                 mask[s:e] = 0.0
             c = {
                 'start': start, 'len': Ln,
-                'traj_local_pred': _f32(d['traj_local_pred'], dev),
+                # without a predicted trajectory no kernel reads it; zeros keep the pointer valid
+                'traj_local_pred': _f32(d['traj_local_pred'] if 'traj_local_pred' in d else torch.zeros(Ln, 11), dev),
                 'orient_base_init': _f32(d['smpl_orient_world_base'], dev).clone(),
                 'trans_base_init': _f32(d['root_trans_world_base'], dev).clone(),
                 'cam_K': _f32(d['cam_K'], dev).reshape(T, 9),
@@ -207,8 +214,24 @@ class StageCompiler:
         keep.append(cam_const)
         pb.cam_pose_const = cam_const.data_ptr()
         pb.trans_res_all = int(fl['flag_cam_inv_trans_res_all'])
-        pb.use_world_res = int('world_res' in opt_variables)
-        pb.has_world_dheading = int(any('world_dheading' in data['person_data'][pid] for pid in self.pids))
+        # ---- trajectory source; the world variables enter the forward only with flag_opt_traj (:451-468)
+        pb.traj_source = self.traj_source
+        pb.use_world_res = int(self.opt_traj and 'world_res' in opt_variables)
+        pb.has_world_dheading = int(self.opt_traj and any('world_dheading' in data['person_data'][pid] for pid in self.pids))
+        # combinations the reference fails on (KeyError / None.items() in get_parameter or loss_func.py): fail clearly here
+        if not self.has_local:
+            for key in opt_variables:
+                if 'local' in key and self.opt_traj:
+                    raise ValueError(f"optimisation variable '{key}' needs the local trajectory variables, which exist only with "
+                                     "flag_pred_traj and flag_opt_traj")
+            for name in loss_cfg:
+                if name.startswith('local_traj_'):
+                    raise ValueError(f"residual '{name}' needs the local trajectory variables, which exist only with "
+                                     "flag_pred_traj and flag_opt_traj")
+        if not self.opt_traj:
+            for name in ('traj_rot_res', 'traj_trans_res', 'rel_transform'):
+                if name in loss_cfg:
+                    raise ValueError(f"residual '{name}' needs flag_opt_traj (world_res / rel_transform_cam are not created without it)")
         pb.empty_index, pb.fill_src, pb.inv_num_persons = self.empty_index.data_ptr(), self.fill_src.data_ptr(), self.inv_num.data_ptr()
         pb.smpl_pose_all, pb.smpl_beta_all = self.pose_all.data_ptr(), self.beta_all.data_ptr()
         pb.scale_all = None if self.scale_all is None else self.scale_all.data_ptr()
@@ -312,10 +335,10 @@ class StageCompiler:
         for p in range(P):
             o, sz = lay.persons[p], sizes(lens[p])
             for key in opt_variables:
-                if key == 'world_res':
+                if key == 'world_res' and self.opt_traj:
                     on(o['orient_res'], 3 * T)
                     on(o['trans_res'], 3 * T)
-                if 'local' in key:
+                if 'local' in key and self.opt_traj:
                     name = key[len('local_'):]
                     if name not in sz:
                         raise KeyError(f'unknown optimisation variable {key}')

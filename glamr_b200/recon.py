@@ -188,15 +188,24 @@ class GlobalReconOptimizer:
         self.flag_opt_cam_from_person_pose = g('flag_opt_cam_from_person_pose', False)
         self.flag_init_cam_all_frames = g('flag_init_cam_all_frames', False)
         self.cam_fix_frames = g('cam_fix_frames', [[0, None]])
+        self.flag_traj_from_cam = g('flag_traj_from_cam', False)
+        self.traj_interp_method = g('traj_interp_method', 'linear_interp')
         self.opt_stage_specs = self.cfg.opt_stage_specs
-        for flag in ['flag_opt_motion_latent', 'flag_opt_traj_latent', 'flag_use_pen_loss', 'flag_traj_from_cam', 'absolute_heading',
+        for flag in ['flag_opt_motion_latent', 'flag_opt_traj_latent', 'flag_use_pen_loss', 'absolute_heading',
                      'flag_opt_person2cam_rot', 'flag_opt_person2cam_trans']:
             if g(flag, False):
                 raise NotImplementedError(f'{flag} is not implemented in the CUDA path (SURVEY.md §8(f)-4); no CPU fallback')
         if g('heading_type', 'scalar') != 'scalar':
             raise NotImplementedError("heading_type 'vec' is not implemented in the CUDA path")
-        if not self.flag_opt_traj:
-            raise NotImplementedError('flag_opt_traj=false is not implemented in the CUDA path')
+        if self.flag_traj_from_cam and self.traj_interp_method not in ('linear_interp', 'last_pose'):
+            raise ValueError(f'unknown traj interp method: {self.traj_interp_method}!')          # :347-348
+        # the learned trajectory (predictor + codec) is optimised only through the local variables, which the reference
+        # creates only with flag_opt_traj (:171-199); its forward then fails on the missing traj_local_xy (:397)
+        if not self.flag_opt_traj and self.flag_infer_motion_traj and self.flag_pred_traj:
+            raise ValueError('flag_opt_traj=false needs flag_infer_motion_traj=false or flag_pred_traj=false: the predicted '
+                             'trajectory is composed with the local trajectory variables, which exist only with flag_opt_traj')
+        # which trajectory the kernels evaluate (include/glamr_b200.h, enum glamr_traj_source)
+        self.traj_source = L.TRAJ_PREDICTED if (self.flag_infer_motion_traj and self.flag_pred_traj) else L.TRAJ_BASE
         self.rank, self.world = dist if dist is not None else (0, 1)
         self.log_interval = g('log_interval', 1)
         self.use_cuda_graph = g('use_cuda_graph', True)
@@ -216,7 +225,8 @@ class GlobalReconOptimizer:
     @property
     def _flags(self):
         return {k: getattr(self, k) for k in ['flag_fixed_cam', 'flag_opt_cam', 'flag_opt_cam_from_person_pose',
-                                              'flag_cam_inv_trans_res_all', 'flag_opt_vis_local_rot', 'cam_fix_frames']}
+                                              'flag_cam_inv_trans_res_all', 'flag_opt_vis_local_rot', 'cam_fix_frames',
+                                              'flag_opt_traj', 'traj_source']}
 
     # ------------------------------------------------------------------------------------------------ init_data
     def _person_from_estimate(self, est, gt_entry):
@@ -338,6 +348,33 @@ class GlobalReconOptimizer:
         d['root_trans_world'] = d['root_trans_world_base']
         d['smpl_orient_world'] = d['smpl_orient_world_base']
 
+    def get_traj_from_cam(self, data):
+        """:325-351 -- the world trajectory seen through the initial camera: translation as observed (the estimate is
+        already interpolated over gaps), orientation interpolated with separate heading ('linear_interp') or both held at
+        the last visible frame over the exist range ('last_pose', which also holds the body pose unless the prior infilled it)."""
+        for d in data['person_data'].values():
+            d['person_transform_world'] = torch.matmul(data['cam_pose_inv'], d['person_transform_cam'])
+            trans = d['person_transform_world'][:, :3, 3]
+            orient_q = G.rotation_matrix_to_quaternion(d['person_transform_world'][:, :3, :3].contiguous())
+            vis = d['vis_frames']
+            if self.traj_interp_method == 'linear_interp':
+                orient_q = self._interp_orient_q_sep_heading(orient_q[vis], vis)
+            else:
+                # forward fill from the last visible frame, over the exist range only (its first frame is visible); the
+                # source frames are visible, so one gather reproduces the reference's frame-by-frame loop
+                vis_h, ex_h = vis.cpu().numpy(), d['exist_frames'].cpu().numpy()
+                idx = np.arange(len(vis_h))
+                src = np.maximum.accumulate(np.where(vis_h, idx, 0))
+                fill = np.where(ex_h & ~vis_h)[0]
+                if fill.size:
+                    dst_t, src_t = torch.as_tensor(fill, device=self.device), torch.as_tensor(src[fill], device=self.device)
+                    trans[dst_t] = trans[src_t]
+                    orient_q[dst_t] = orient_q[src_t]
+                    if not (self.flag_infer_motion_traj and self.flag_infill_motion):
+                        d['smpl_pose'][dst_t] = d['smpl_pose'][src_t]
+            d['root_trans_world'] = d['root_trans_world_base'] = trans
+            d['smpl_orient_world'] = d['smpl_orient_world_base'] = G.quaternion_to_angle_axis(orient_q)
+
     def init_cam_pose(self, data, all_frames=False):
         """:294-317"""
         cands = [torch.matmul(d['person_transform_world'], d['person2cam']) * d['vis_frames'][:, None, None]
@@ -449,29 +486,37 @@ class GlobalReconOptimizer:
         if self.flag_infer_motion_traj:
             self.infer_motion_traj_all(persons)
         if not (self.flag_infer_motion_traj and self.flag_pred_traj):
-            raise NotImplementedError('flag_pred_traj=false (default trajectory) is not implemented in the CUDA path')
+            for d in persons.values():
+                self.init_default_traj(d)
         for d in persons.values():
             d['person_transform_world'] = G.make_transform(d['smpl_orient_world'], d['root_trans_world'], 'axis_angle')
             d['person_transform_cam'] = G.make_transform(d['smpl_orient_cam'].float(), d['root_trans_cam'].float(), 'axis_angle')
             d['person2cam'] = G.inverse_transform(d['person_transform_cam'])
-        last = d
-        for d in persons.values():
-            d['smpl_orient_world_res'] = torch.zeros_like(last['smpl_orient_world'])
-            d['root_trans_world_res'] = torch.zeros_like(last['root_trans_world'])
-        rel = {}
-        ids = list(persons.keys())
-        for i in range(len(ids)):
-            for j in range(len(ids)):
-                if i != j:
-                    rel[(i, j)] = torch.matmul(G.inverse_transform(persons[ids[i]]['person_transform_cam']), persons[ids[j]]['person_transform_cam'])
-        for d in persons.values():
-            Ln = int(d['exist_len'].sum())
-            d['traj_local_xy'] = torch.zeros(2, device=dev)
-            d['traj_local_dxy'] = torch.zeros(Ln - 1, 2, device=dev)
-            d['traj_local_heading'] = torch.zeros(1, device=dev)
-            d['traj_local_dheading'] = torch.zeros(Ln - 1, device=dev)
-            d['traj_local_z'] = torch.zeros(Ln, device=dev)
-            d['traj_local_rot'] = torch.zeros(Ln, 6, device=dev)
+        rel = None
+        if self.flag_opt_traj:                                     # :171-205
+            last = d
+            for d in persons.values():
+                d['smpl_orient_world_res'] = torch.zeros_like(last['smpl_orient_world'])
+                d['root_trans_world_res'] = torch.zeros_like(last['root_trans_world'])
+            rel = {}
+            ids = list(persons.keys())
+            for i in range(len(ids)):
+                for j in range(len(ids)):
+                    if i != j:
+                        rel[(i, j)] = torch.matmul(G.inverse_transform(persons[ids[i]]['person_transform_cam']), persons[ids[j]]['person_transform_cam'])
+            if self.flag_pred_traj:
+                for d in persons.values():
+                    Ln = int(d['exist_len'].sum())
+                    d['traj_local_xy'] = torch.zeros(2, device=dev)
+                    d['traj_local_dxy'] = torch.zeros(Ln - 1, 2, device=dev)
+                    d['traj_local_heading'] = torch.zeros(1, device=dev)
+                    d['traj_local_dheading'] = torch.zeros(Ln - 1, device=dev)
+                    d['traj_local_z'] = torch.zeros(Ln, device=dev)
+                    d['traj_local_rot'] = torch.zeros(Ln, 6, device=dev)
+            else:
+                for d in persons.values():
+                    d['root_trans_world_base'][:] = d['root_trans_world_base'][0].clone()
+                    d['smpl_orient_world_base'][:] = d['smpl_orient_world_base'][0].clone()
         fr_num_persons = sum(d['vis_frames'] for d in persons.values())
         n_empty = int((fr_num_persons == 0).sum())
         data = {
@@ -483,7 +528,10 @@ class GlobalReconOptimizer:
             'meta': {'algo': 'global_recon', 'mt_cfg': getattr(self.mt_cfg, 'yml_dict', None), 'num_fr': num_fr},
         }
         self.init_cam_pose(data)
-        self.init_traj_heading_from_cam(data)
+        if self.flag_traj_from_cam:
+            self.get_traj_from_cam(data)
+        if self.flag_infer_motion_traj and self.flag_pred_traj:
+            self.init_traj_heading_from_cam(data)
         if self.flag_init_cam_all_frames:
             self.init_cam_pose(data, all_frames=True)
         self._attach(data)
@@ -627,7 +675,7 @@ class GlobalReconOptimizer:
         ob, tb = self._read(L.R_ORIENT_BASE, P, T, 3), self._read(L.R_TRANS_BASE, P, T, 3)
         kp = self._read(L.R_KP_PRED, P, T, J, 2)
         ociw, tciw = self._read(L.R_ORIENT_CIW, P, T, 3), self._read(L.R_TRANS_CIW, P, T, 3)
-        tl = self._read(L.R_TRAJ_LOCAL, P, T, 11)
+        tl = self._read(L.R_TRAJ_LOCAL, P, T, 11) if self.traj_source == L.TRAJ_PREDICTED else None
         jw = self._read(L.R_JOINTS_WORLD, P, T, J, 3)
         if self.world > 1:
             # per-frame-person outputs exist only on the rank that evaluated that frame-person: keep the own shard, sum over ranks
@@ -650,7 +698,8 @@ class GlobalReconOptimizer:
             d['smpl_orient_world_base'], d['root_trans_world_base'] = ob[p], tb[p]
             d['kp_2d_pred'] = kp[p]
             d['smpl_orient_cam_in_world'], d['root_trans_cam_in_world'] = ociw[p], tciw[p]
-            d['traj_local'] = tl[p][d['exist_frames']]
+            if self.traj_source == L.TRAJ_PREDICTED:           # without the codec the reference has no traj_local
+                d['traj_local'] = tl[p][d['exist_frames']]
             d['joints_world'] = jw[p]
             d['person_transform_world'] = G.make_transform(ow[p], tw[p], 'axis_angle')
 

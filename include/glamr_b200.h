@@ -152,6 +152,13 @@ enum glamr_cam_mode {
   GLAMR_CAM_FROM_PERSONS = 3  /* mean of person_transform_world @ person2cam + residuals   (:481-508)            */
 };
 
+enum glamr_traj_source {
+  GLAMR_TRAJ_PREDICTED = 0,   /* traj_local_pred + local variables through the trajectory codec on the exist range   (:448-449) */
+  GLAMR_TRAJ_BASE = 1         /* every frame: orient/trans_base_init, then world_res / world_dheading (flag_infer_motion_traj or
+                               * flag_pred_traj false: no codec, no prefix scans; the traj_local_* variables only see their
+                               * regularisers).  flag_opt_traj false: the same with neither world variable active       */
+};
+
 typedef struct glamr_person {
   int32_t start, len;              /* exist range [start, start+len) of this person (exist_frames)              */
   int32_t off_xy, off_heading, off_dxy, off_dheading, off_z, off_rot;     /* offsets into theta (floats)        */
@@ -189,6 +196,7 @@ typedef struct glamr_problem {
   int32_t owner;                   /* != 0: this rank also evaluates the replicated terms (camera, regs, rel)    */
   int32_t cam_traj_rot_quat;       /* cam_traj_rot: rot_type 'quat' (loss_func.py:158-161) instead of '6d'          */
   int32_t traj_rot_smooth_quat;    /* traj_rot_smoothness: rot_type 'quat' (loss_func.py:126-128)                  */
+  int32_t traj_source;             /* enum glamr_traj_source; 0 (zero-initialised) = the predicted trajectory      */
   float cam_up_first_weight;
   float rel_trans_weight;
   float term_weight[GLAMR_NUM_TERMS];   /* YAML weight, 0 if the term is absent                                  */
