@@ -73,6 +73,22 @@ GLAMR_HD float traj_pre_vals(const OptCtx& c, int p, int i, float* tl) {
   const glamr_person_t& ps = c.pb.persons[p];
   const float* pr = ps.traj_local_pred + (size_t)i * 11;
   const float* th = c.theta;
+  if (c.pb.heading_vec) {
+    // heading_type 'vec' (:403-405): the variables move the predicted heading vector; the row keeps the un-normalised vector and
+    // its angle (vec_to_heading, traj_utils.py:69) enters the scan
+    const float m = (i == 0) ? 1.0f : ps.dheading_mask[i - 1];
+    const int o = (i == 0) ? ps.off_heading : ps.off_dheading + 2 * (i - 1);
+    const int od = (i == 0) ? ps.off_xy : ps.off_dxy + 2 * (i - 1);
+    tl[0] = pr[0] + th[od];
+    tl[1] = pr[1] + th[od + 1];
+    tl[2] = pr[2] + th[ps.off_z + i];
+    const float rm = ps.rot_mask ? ps.rot_mask[i] : 1.0f;
+#pragma unroll
+    for (int k = 0; k < 6; ++k) tl[3 + k] = pr[3 + k] + th[ps.off_rot + 6 * i + k] * rm;
+    tl[9] = (i == 0) ? pr[9] + th[o] : pr[9] + th[o] * m;
+    tl[10] = (i == 0) ? pr[10] + th[o + 1] : pr[10] + th[o + 1] * m;
+    return safe_atan2(tl[10], tl[9]);
+  }
   float h = safe_atan2(pr[10], pr[9]);
   if (i == 0) {
     h += th[ps.off_heading];
@@ -146,6 +162,7 @@ GLAMR_HD void traj_post_vals(const OptCtx& c, int p, int t, const float* tl, flo
   } else {
 #pragma unroll
     for (int k = 0; k < 3; ++k) { ob[k] = ps.orient_base_init[t * 3 + k]; tb[k] = ps.trans_base_init[t * 3 + k]; }
+    if (ps.world_dxy_base) { tb[0] = ps.world_dxy_base[2 * t]; tb[1] = ps.world_dxy_base[2 * t + 1]; }
   }
   float ow[3], tw[3];
 #pragma unroll
@@ -166,6 +183,17 @@ GLAMR_HD void traj_post_vals(const OptCtx& c, int p, int t, const float* tl, flo
     quat_to_aa(q, ow);
 #pragma unroll
     for (int k = 0; k < 3; ++k) tw[k] = tb[k];
+  }
+  if (c.pb.has_world_dxy) {
+    // root_trans_world[:, :2] += world_dxy (:467-468), in place: when root_trans_world IS the base (world_dxy_alias), the base
+    // takes the add too, and outside the codec's frames it keeps it for the next evaluation
+    tw[0] += c.theta[ps.off_world_dxy + 2 * t];
+    tw[1] += c.theta[ps.off_world_dxy + 2 * t + 1];
+    if (c.pb.world_dxy_alias) {
+      tb[0] = tw[0];
+      tb[1] = tw[1];
+      if (ps.world_dxy_base && !traj_codec_frame(c, ps, i)) { ps.world_dxy_base[2 * t] = tw[0]; ps.world_dxy_base[2 * t + 1] = tw[1]; }
+    }
   }
 #pragma unroll
   for (int k = 0; k < 3; ++k) {
@@ -857,6 +885,10 @@ GLAMR_HD void traj_back_pre(const OptCtx& c, int p, int t, TermAcc& acc) {
   for (int k = 0; k < 3; ++k) { g_ow[k] = c.sc.g_orient[n * 3 + k]; g_tw[k] = c.sc.g_trans[n * 3 + k]; }
   const float* ob = c.sc.orient_base + n * 3;
   float g_ob[3] = {g_ow[0], g_ow[1], g_ow[2]}, g_tb[3] = {g_tw[0], g_tw[1], g_tw[2]};
+  if (pb.has_world_dxy) {     // trans_world x / y = (...) + world_dxy, aliased or not
+    c.sc.grad[ps.off_world_dxy + 2 * t] = g_tw[0];
+    c.sc.grad[ps.off_world_dxy + 2 * t + 1] = g_tw[1];
+  }
   if (pb.use_world_res) {
     // traj_rot_res / traj_trans_res regularisers (loss_func.py:204-209) on the owner rank
     float go[3] = {g_ow[0], g_ow[1], g_ow[2]}, gt[3] = {g_tw[0], g_tw[1], g_tw[2]};
@@ -996,24 +1028,44 @@ GLAMR_HD void traj_back_mid(const OptCtx& c, int p, int i, TermAcc& acc) {
   }
 }
 // after the reverse inclusive scan of g_head: heading variables + dheading regularisers (loss_func.py:216-230)
-// GLAMR_TRAJ_BASE (no scan ran): the regularisers only
+// GLAMR_TRAJ_BASE (no scan ran): the regularisers only.
+// heading_type 'vec': the scanned angle is safe_atan2 of the row's vector, so G reaches its two components (each masked as in the
+// forward), and the regularisers act on both components of traj_local_dheading [len-1,2] (heading_to_vec elementwise for _reg_new).
+// Both heading types share one loop and one update of the term sums, which keeps traj_cam_backward_kernel free of spills.
 GLAMR_HD void traj_back_post(const OptCtx& c, int p, int i, TermAcc& acc) {
   const glamr_problem_t& pb = c.pb;
   const glamr_person_t& ps = pb.persons[p];
   const size_t n = (size_t)p * pb.T + ps.start + i;
   const float G = pb.traj_source == GLAMR_TRAJ_PREDICTED ? c.sc.g_head[n] : 0.0f;
+  const int nc = pb.heading_vec ? 2 : 1;
+  float gx = G, gy = 0.0f;
+  if (pb.heading_vec) {
+    const float* tl = c.sc.traj_local + n * 11;
+    gx = 0.0f;
+    if (pb.traj_source == GLAMR_TRAJ_PREDICTED) safe_atan2_vjp(tl[10], tl[9], G, gy, gx);
+  }
   if (i == 0) {
-    c.sc.grad[ps.off_heading] = G;
-  } else {
-    const float x = c.theta[ps.off_dheading + i - 1];
-    float g = G * ps.dheading_mask[i - 1];
+    c.sc.grad[ps.off_heading] = gx;
+    if (nc == 2) c.sc.grad[ps.off_heading + 1] = gy;
+    return;
+  }
+  const float m = ps.dheading_mask[i - 1];
+  double s_reg = 0.0, s_reg_new = 0.0;
+  for (int k = 0; k < nc; ++k) {
+    const int o = ps.off_dheading + nc * (i - 1) + k;
+    const float x = c.theta[o];
+    float g = (k == 0 ? gx : gy) * m;
     if (pb.owner) {
       const float sx = sinf(x), cx = cosf(x);
       g += 2.0f * kFps2 * c.gs[GLAMR_T_DHEADING_REG] * x + 2.0f * kFps2 * c.gs[GLAMR_T_DHEADING_REG_NEW] * sx;
-      if (pb.term_enabled[GLAMR_T_DHEADING_REG]) acc.v[GLAMR_T_DHEADING_REG] += (double)(kFps2 * x * x);
-      if (pb.term_enabled[GLAMR_T_DHEADING_REG_NEW]) acc.v[GLAMR_T_DHEADING_REG_NEW] += (double)(kFps2 * ((cx - 1.0f) * (cx - 1.0f) + sx * sx));
+      s_reg += (double)(kFps2 * x * x);
+      s_reg_new += (double)(kFps2 * ((cx - 1.0f) * (cx - 1.0f) + sx * sx));
     }
-    c.sc.grad[ps.off_dheading + i - 1] = g;
+    c.sc.grad[o] = g;
+  }
+  if (pb.owner) {
+    if (pb.term_enabled[GLAMR_T_DHEADING_REG]) acc.v[GLAMR_T_DHEADING_REG] += s_reg;
+    if (pb.term_enabled[GLAMR_T_DHEADING_REG_NEW]) acc.v[GLAMR_T_DHEADING_REG_NEW] += s_reg_new;
   }
 }
 

@@ -248,7 +248,7 @@ __device__ void reduce_tail(const OptCtx& c, const double* partial, int n_slots,
 
 // blocks [0,P): reverse trajectory codec of one person; blocks [P, P+cam_blocks): camera backward of 256 frames (modes
 // 0-2; mode 3 runs camera_backward/scatter kernels first).  The last CTA to finish folds all partial sums.
-__global__ void __launch_bounds__(kScanThreads) traj_cam_backward_kernel(OptCtx c, int with_cam, double* partial_traj, const double* partial_all,
+__global__ void __launch_bounds__(kScanThreads, 1) traj_cam_backward_kernel(OptCtx c, int with_cam, double* partial_traj, const double* partial_all,
                                                                          int n_slots, float* reduce_buf, unsigned int* ticket, PeerCtx pc) {
   __shared__ float sm[kScanThreads / 32 + 1];
   __shared__ double smd[(kScanThreads / 32) * GLAMR_NUM_TERMS];

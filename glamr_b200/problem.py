@@ -19,8 +19,12 @@ from . import lib as L
 
 
 class VariableLayout:
-    def __init__(self, T, n_empty, trans_res_rows, lens):
+    def __init__(self, T, n_empty, trans_res_rows, lens, heading_dim=1, world_dxy=False):
+        """heading_dim 2: heading_type 'vec' (traj_local_heading [2], traj_local_dheading [L-1,2]); world_dxy: every person also
+        gets a world_dxy [T,2] block (only when a stage can create it, so other problems keep their layout)"""
         self.T, self.n_empty, self.trans_res_rows, self.lens = T, n_empty, trans_res_rows, list(lens)
+        self.heading_dim, self.world_dxy = heading_dim, bool(world_dxy)
+        hd = heading_dim
         off = 0
 
         def take(n):
@@ -33,8 +37,9 @@ class VariableLayout:
         self.cam_inv_rot_res, self.cam_inv_trans_res = take(6 * n_empty), take(3 * trans_res_rows)
         self.persons = []
         for Ln in self.lens:
-            self.persons.append(dict(xy=take(2), heading=take(1), dxy=take(2 * (Ln - 1)), dheading=take(Ln - 1), z=take(Ln),
-                                     rot=take(6 * Ln), world_dheading=take(T), orient_res=take(3 * T), trans_res=take(3 * T)))
+            self.persons.append(dict(xy=take(2), heading=take(hd), dxy=take(2 * (Ln - 1)), dheading=take(hd * (Ln - 1)), z=take(Ln),
+                                     rot=take(6 * Ln), world_dheading=take(T), orient_res=take(3 * T), trans_res=take(3 * T),
+                                     world_dxy=take(2 * T if self.world_dxy else 0)))
         self.n_params = off
 
     def views(self, theta, p=None):
@@ -46,13 +51,17 @@ class VariableLayout:
                     'cam_rot_6d_fix': v(self.cam_rot_fix, 6, 1, 6), 'cam_trans_fix': v(self.cam_trans_fix, 3, 1, 3),
                     'cam_inv_rot_residual': v(self.cam_inv_rot_res, 6 * self.n_empty, self.n_empty, 6),
                     'cam_inv_trans_residual': v(self.cam_inv_trans_res, 3 * self.trans_res_rows, self.trans_res_rows, 3)}
-        o, Ln = self.persons[p], self.lens[p]
+        o, Ln, hd = self.persons[p], self.lens[p], self.heading_dim
         v = lambda k, n, *shape: theta[o[k]:o[k] + n].view(*shape)
-        return {'traj_local_xy': v('xy', 2, 2), 'traj_local_heading': v('heading', 1, 1),
-                'traj_local_dxy': v('dxy', 2 * (Ln - 1), Ln - 1, 2), 'traj_local_dheading': v('dheading', Ln - 1, Ln - 1),
-                'traj_local_z': v('z', Ln, Ln), 'traj_local_rot': v('rot', 6 * Ln, Ln, 6),
-                'world_dheading': v('world_dheading', T, T, 1), 'smpl_orient_world_res': v('orient_res', 3 * T, T, 3),
-                'root_trans_world_res': v('trans_res', 3 * T, T, 3)}
+        out = {'traj_local_xy': v('xy', 2, 2), 'traj_local_heading': v('heading', hd, hd),
+               'traj_local_dxy': v('dxy', 2 * (Ln - 1), Ln - 1, 2),
+               'traj_local_dheading': v('dheading', Ln - 1, Ln - 1) if hd == 1 else v('dheading', 2 * (Ln - 1), Ln - 1, 2),
+               'traj_local_z': v('z', Ln, Ln), 'traj_local_rot': v('rot', 6 * Ln, Ln, 6),
+               'world_dheading': v('world_dheading', T, T, 1), 'smpl_orient_world_res': v('orient_res', 3 * T, T, 3),
+               'root_trans_world_res': v('trans_res', 3 * T, T, 3)}
+        if self.world_dxy:
+            out['world_dxy'] = v('world_dxy', 2 * T, T, 2)
+        return out
 
 
 def _f32(x, device):
@@ -65,7 +74,8 @@ class StageCompiler:
     def __init__(self, data, layout, flags, device, aa_to_rot6d, num_joints=26, aa_to_quat=None):
         """flags: dict with flag_fixed_cam, flag_opt_cam, flag_opt_cam_from_person_pose, flag_cam_inv_trans_res_all,
         flag_opt_vis_local_rot, cam_fix_frames and optionally flag_opt_traj / traj_source (when absent they are read off
-        `data`: a predicted trajectory leaves traj_local_pred, flag_opt_traj leaves the world_res variables).
+        `data`: a predicted trajectory leaves traj_local_pred, flag_opt_traj leaves the world_res variables) and heading_vec
+        (heading_type 'vec'; default: the layout's heading size).
         aa_to_rot6d: callable (device math lives in the CUDA library)."""
         self.data, self.layout, self.flags, self.device, self.J = data, layout, flags, device, num_joints
         self.pids = list(data['person_data'].keys())
@@ -75,6 +85,7 @@ class StageCompiler:
         self.traj_source = flags.get('traj_source', L.TRAJ_PREDICTED if all('traj_local_pred' in d for d in persons) else L.TRAJ_BASE)
         self.opt_traj = flags.get('flag_opt_traj', all('smpl_orient_world_res' in d for d in persons))
         self.has_local = all('traj_local_xy' in d for d in persons)        # created with flag_opt_traj and flag_pred_traj (:185-199)
+        self.heading_vec = bool(flags.get('heading_vec', layout.heading_dim == 2))
         self.keep = []                               # tensors whose storage the structs point into
         self.const = []
         pose_all, beta_all, scale_all = [], [], []
@@ -99,6 +110,8 @@ class StageCompiler:
                 'dheading_mask': _f32(mask, dev),
                 'rot_mask': _f32(d['vis_frames'][start:start + Ln], dev) if flags.get('flag_opt_vis_local_rot', False) else None,
                 'vis': _f32(d['vis_frames'], dev),
+                # x / y of the base that world_dxy's in-place add advances (include/glamr_b200.h, world_dxy_base)
+                'world_dxy_base': _f32(d['root_trans_world_base'], dev)[:, :2].contiguous().clone() if layout.world_dxy else None,
             }
             self.const.append(c)
             pose_all.append(_f32(d['smpl_pose'], dev))
@@ -218,6 +231,16 @@ class StageCompiler:
         pb.traj_source = self.traj_source
         pb.use_world_res = int(self.opt_traj and 'world_res' in opt_variables)
         pb.has_world_dheading = int(self.opt_traj and any('world_dheading' in data['person_data'][pid] for pid in self.pids))
+        pb.heading_vec = int(self.heading_vec)
+        # world_dxy, once created, is added in place to root_trans_world (:467-468); that tensor IS the base unless world_res
+        # alone composes the pose, and then the add lands in the base too
+        has_dxy = self.opt_traj and any('world_dxy' in data['person_data'][pid] for pid in self.pids)
+        alias = has_dxy and (pb.has_world_dheading or not pb.use_world_res)
+        if alias and self.traj_source == L.TRAJ_BASE:
+            raise ValueError("world_dxy with a trajectory that does not come from the predictor needs world_res in opt_variables and "
+                             "no world_dheading: otherwise the reference adds world_dxy in place to a base it never re-creates, and "
+                             "its second backward fails (autograd graph already freed)")
+        pb.has_world_dxy, pb.world_dxy_alias = int(has_dxy), int(alias)
         # combinations the reference fails on (KeyError / None.items() in get_parameter or loss_func.py): fail clearly here
         if not self.has_local:
             for key in opt_variables:
@@ -252,9 +275,9 @@ class StageCompiler:
             ps.start, ps.len = c['start'], c['len']
             ps.off_xy, ps.off_heading, ps.off_dxy, ps.off_dheading = o['xy'], o['heading'], o['dxy'], o['dheading']
             ps.off_z, ps.off_rot, ps.off_world_dheading = o['z'], o['rot'], o['world_dheading']
-            ps.off_orient_res, ps.off_trans_res = o['orient_res'], o['trans_res']
+            ps.off_orient_res, ps.off_trans_res, ps.off_world_dxy = o['orient_res'], o['trans_res'], o['world_dxy']
             for name in ['traj_local_pred', 'orient_base_init', 'trans_base_init', 'cam_K', 'kp_target', 'orient_cam_6d',
-                         'orient_cam_q', 'trans_cam', 'person2cam', 'dheading_mask', 'rot_mask', 'vis']:
+                         'orient_cam_q', 'trans_cam', 'person2cam', 'dheading_mask', 'rot_mask', 'vis', 'world_dxy_base']:
                 setattr(ps, name, None if c[name] is None else c[name].data_ptr())
             base = dev_w.data_ptr() + p * dev_w.shape[1] * 4
             ps.kp_w, ps.kp_dist_mask = base, base + T * J * 4
@@ -331,7 +354,8 @@ class StageCompiler:
         else:
             on(lay.cam_rot, 6 * T)
             on(lay.cam_trans, 3 * T)
-        sizes = lambda Ln: {'xy': 2, 'heading': 1, 'dxy': 2 * (Ln - 1), 'dheading': Ln - 1, 'z': Ln, 'rot': 6 * Ln}
+        hd = lay.heading_dim
+        sizes = lambda Ln: {'xy': 2, 'heading': hd, 'dxy': 2 * (Ln - 1), 'dheading': hd * (Ln - 1), 'z': Ln, 'rot': 6 * Ln}
         for p in range(P):
             o, sz = lay.persons[p], sizes(lens[p])
             for key in opt_variables:
@@ -345,7 +369,9 @@ class StageCompiler:
                     on(o[name], sz[name])
                 if key == 'world_dheading':
                     on(o['world_dheading'], T)
-                if key in ('world_dxy', 'person2cam_rot', 'person2cam_trans'):
+                if key == 'world_dxy' and self.opt_traj:          # without flag_opt_traj the forward never reads it (:451)
+                    on(o['world_dxy'], 2 * T)
+                if key in ('person2cam_rot', 'person2cam_trans'):
                     raise NotImplementedError(f"optimisation variable '{key}' is not implemented in the CUDA path")
         active = active.to(dev)
         keep.append(active)
@@ -360,7 +386,12 @@ def make_layout(data, flags):
     T = data['seq_len']
     n_empty = int((torch.as_tensor(data['fr_num_persons']) == 0).sum())
     rows = T if flags['flag_cam_inv_trans_res_all'] else n_empty
-    return VariableLayout(T, n_empty, rows, [int(d['exist_len']) for d in persons.values()])
+    world_dxy = flags.get('world_dxy', False) or any('world_dxy' in d for d in persons.values())
+    heading_vec = flags.get('heading_vec')
+    if heading_vec is None:              # read off the variables init_data created (:191-196)
+        heading_vec = any('traj_local_heading' in d and torch.as_tensor(d['traj_local_heading']).numel() == 2 for d in persons.values())
+    return VariableLayout(T, n_empty, rows, [int(d['exist_len']) for d in persons.values()],
+                          heading_dim=2 if heading_vec else 1, world_dxy=world_dxy)
 
 
 def bind_variables(data, layout, theta):
@@ -373,7 +404,7 @@ def bind_variables(data, layout, theta):
     for p, d in enumerate(data['person_data'].values()):
         pv = layout.views(theta, p)
         for name in ['traj_local_xy', 'traj_local_heading', 'traj_local_dxy', 'traj_local_dheading', 'traj_local_z',
-                     'traj_local_rot', 'smpl_orient_world_res', 'root_trans_world_res', 'world_dheading']:
+                     'traj_local_rot', 'smpl_orient_world_res', 'root_trans_world_res', 'world_dheading', 'world_dxy']:
             # world_dheading exists once a stage has requested it (global_recon_model.py:624-627); with continue_opt it
             # arrives already optimised and forward() keeps composing with it (:459-465)
             if name in d:
@@ -383,7 +414,7 @@ def bind_variables(data, layout, theta):
 
 def begin_stage_variables(data, layout, theta, flags, opt_variables):
     """Side effects of GlobalReconOptimizer.get_parameter (global_recon_model.py:596-631): camera variables are
-    re-initialised from the current cam_pose, world_dheading is created (zeros) the first time it is requested."""
+    re-initialised from the current cam_pose, world_dheading / world_dxy are created (zeros) the first time they are requested."""
     gv = layout.views(theta)
     if 'cam' in opt_variables:
         cam = torch.as_tensor(data['cam_pose']).to(theta)
@@ -402,3 +433,10 @@ def begin_stage_variables(data, layout, theta, flags, opt_variables):
         for p, d in enumerate(data['person_data'].values()):
             if 'world_dheading' not in d:
                 d['world_dheading'] = layout.views(theta, p)['world_dheading']
+    if 'world_dxy' in opt_variables:
+        if not layout.world_dxy:
+            raise ValueError("opt_variables lists 'world_dxy' but the variable layout has no world_dxy block "
+                             "(make_layout(..., flags={'world_dxy': True, ...}))")
+        for p, d in enumerate(data['person_data'].values()):
+            if 'world_dxy' not in d:
+                d['world_dxy'] = layout.views(theta, p)['world_dxy']

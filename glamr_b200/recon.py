@@ -191,12 +191,20 @@ class GlobalReconOptimizer:
         self.flag_traj_from_cam = g('flag_traj_from_cam', False)
         self.traj_interp_method = g('traj_interp_method', 'linear_interp')
         self.opt_stage_specs = self.cfg.opt_stage_specs
-        for flag in ['flag_opt_motion_latent', 'flag_opt_traj_latent', 'flag_use_pen_loss', 'absolute_heading',
+        for flag in ['flag_opt_motion_latent', 'flag_opt_traj_latent', 'flag_use_pen_loss',
                      'flag_opt_person2cam_rot', 'flag_opt_person2cam_trans']:
             if g(flag, False):
                 raise NotImplementedError(f'{flag} is not implemented in the CUDA path (SURVEY.md §8(f)-4); no CPU fallback')
-        if g('heading_type', 'scalar') != 'scalar':
-            raise NotImplementedError("heading_type 'vec' is not implemented in the CUDA path")
+        if g('absolute_heading', False):
+            raise NotImplementedError('absolute_heading is not implemented in the CUDA path: without latent optimisation the reference '
+                                      "reads the predictor's per-frame heading increments as absolute headings (:283,:421), which "
+                                      'does not give a usable trajectory')
+        self.heading_type = g('heading_type', 'scalar')
+        if self.heading_type not in ('scalar', 'vec'):
+            raise ValueError(f"unknown heading_type {self.heading_type!r} (expected 'scalar' or 'vec')")
+        self.heading_vec = self.heading_type == 'vec'
+        # world_dxy gets its own block of theta only when a stage can create it, so every other problem keeps its layout
+        self.world_dxy = any('world_dxy' in st.get('opt_variables', []) for st in cfg.opt_stage_specs.values())
         if self.flag_traj_from_cam and self.traj_interp_method not in ('linear_interp', 'last_pose'):
             raise ValueError(f'unknown traj interp method: {self.traj_interp_method}!')          # :347-348
         # the learned trajectory (predictor + codec) is optimised only through the local variables, which the reference
@@ -226,7 +234,7 @@ class GlobalReconOptimizer:
     def _flags(self):
         return {k: getattr(self, k) for k in ['flag_fixed_cam', 'flag_opt_cam', 'flag_opt_cam_from_person_pose',
                                               'flag_cam_inv_trans_res_all', 'flag_opt_vis_local_rot', 'cam_fix_frames',
-                                              'flag_opt_traj', 'traj_source']}
+                                              'flag_opt_traj', 'traj_source', 'heading_vec', 'world_dxy']}
 
     # ------------------------------------------------------------------------------------------------ init_data
     def _person_from_estimate(self, est, gt_entry):
@@ -509,8 +517,9 @@ class GlobalReconOptimizer:
                     Ln = int(d['exist_len'].sum())
                     d['traj_local_xy'] = torch.zeros(2, device=dev)
                     d['traj_local_dxy'] = torch.zeros(Ln - 1, 2, device=dev)
-                    d['traj_local_heading'] = torch.zeros(1, device=dev)
-                    d['traj_local_dheading'] = torch.zeros(Ln - 1, device=dev)
+                    hd = 2 if self.heading_vec else 1                   # heading_type 'vec': heading vectors (:191-196)
+                    d['traj_local_heading'] = torch.zeros(hd, device=dev)
+                    d['traj_local_dheading'] = torch.zeros((Ln - 1, 2) if self.heading_vec else (Ln - 1,), device=dev)
                     d['traj_local_z'] = torch.zeros(Ln, device=dev)
                     d['traj_local_rot'] = torch.zeros(Ln, 6, device=dev)
             else:

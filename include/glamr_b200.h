@@ -163,7 +163,7 @@ typedef struct glamr_person {
   int32_t start, len;              /* exist range [start, start+len) of this person (exist_frames)              */
   int32_t off_xy, off_heading, off_dxy, off_dheading, off_z, off_rot;     /* offsets into theta (floats)        */
   int32_t off_world_dheading, off_orient_res, off_trans_res;              /* [T], [T,3], [T,3]                  */
-  int32_t pad_;
+  int32_t off_world_dxy;           /* [T,2] world_dxy (read only with has_world_dxy)                              */
   const float* traj_local_pred;    /* [len,11]                                                                    */
   const float* orient_base_init;   /* [T,3] smpl_orient_world_base outside the exist range                        */
   const float* trans_base_init;    /* [T,3]                                                                       */
@@ -181,6 +181,12 @@ typedef struct glamr_person {
   const float* kp_dist_mask;       /* [T,J]                                                                       */
   const float* ctr_w;              /* [T]  cam_traj_rot                                                           */
   const float* ctt_w;              /* [T]  cam_traj_trans                                                         */
+  /* [T,2] or NULL (-> trans_base_init): x / y of root_trans_world_base on the frames the codec does not produce.  The
+   * reference adds world_dxy IN PLACE to root_trans_world, which aliases the base unless world_res alone composes the
+   * pose (:451-468); the base then keeps every evaluation's world_dxy.  With world_dxy_alias each trajectory forward adds
+   * the current world_dxy here exactly once.  Caller-owned, initialised to trans_base_init[:, :2], persists across
+   * stages; every rank keeps its own copy (the trajectory forward is replicated).                                  */
+  float* world_dxy_base;
 } glamr_person_t;
 
 typedef struct glamr_problem {
@@ -197,6 +203,10 @@ typedef struct glamr_problem {
   int32_t cam_traj_rot_quat;       /* cam_traj_rot: rot_type 'quat' (loss_func.py:158-161) instead of '6d'          */
   int32_t traj_rot_smooth_quat;    /* traj_rot_smoothness: rot_type 'quat' (loss_func.py:126-128)                  */
   int32_t traj_source;             /* enum glamr_traj_source; 0 (zero-initialised) = the predicted trajectory      */
+  int32_t heading_vec;             /* heading_type 'vec' (:403-405): traj_local_heading [2] / _dheading [len-1,2] are added to
+                                    * the predicted heading VECTOR, whose angle enters the scan; 0 = 'scalar' (angle)   */
+  int32_t has_world_dxy;           /* world_dxy [T,2] is added to root_trans_world x / y (:467-468)                */
+  int32_t world_dxy_alias;         /* that add also lands in the base (see glamr_person_t.world_dxy_base)          */
   float cam_up_first_weight;
   float rel_trans_weight;
   float term_weight[GLAMR_NUM_TERMS];   /* YAML weight, 0 if the term is absent                                  */
