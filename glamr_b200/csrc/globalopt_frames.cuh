@@ -115,18 +115,22 @@ GLAMR_HD void traj_pre(const OptCtx& c, int p, int i) {
 #pragma unroll
   for (int k = 0; k < 11; ++k) c.sc.traj_local[(size_t)n * 11 + k] = tl[k];
 }
-// after the inclusive scan of heading: rotate d_xy of frame i >= 1 by heading[i-1]   (traj_utils.py:76-77)
+// d_xy rotated by heading h (traj_utils.py:76-77).  traj_mid and forward_pose_kernel both call this, with the products and their
+// sums spelled out as fmaf: left to the compiler, the two call sites were contracted differently and root_trans_world.y of the
+// fused head came out one rounding away from the default one
+GLAMR_HD void rotate_dxy(float h, float& x, float& y) {
+  const float ct = cosf(h), st = sinf(h);
+  const float rx = fmaf(x, ct, -(y * st)), ry = fmaf(x, st, y * ct);
+  x = rx;
+  y = ry;
+}
+// after the inclusive scan of heading: rotate d_xy of frame i >= 1 by heading[i-1]
 GLAMR_HD void traj_mid(const OptCtx& c, int p, int i) {
   const glamr_person_t& ps = c.pb.persons[p];
   const int n = p * c.pb.T + ps.start + i;
   const float* tl = c.sc.traj_local + (size_t)n * 11;
   float x = tl[0], y = tl[1];
-  if (i > 0) {
-    const float t = c.sc.heading[n - 1];
-    const float ct = cosf(t), st = sinf(t);
-    const float rx = x * ct - y * st, ry = x * st + y * ct;
-    x = rx; y = ry;
-  }
+  if (i > 0) rotate_dxy(c.sc.heading[n - 1], x, y);
   c.sc.xy[2 * (size_t)n] = x;
   c.sc.xy[2 * (size_t)n + 1] = y;
 }

@@ -432,13 +432,7 @@ __global__ void __launch_bounds__(kScanThreads) forward_pose_kernel(OptCtx c, Sm
   if (cnt > 0) block_scan_inplace(s_head, cnt, 1, false, sm);
   __syncthreads();
   for (int i = tid; i < cnt; i += kScanThreads) {
-    if (i > 0) {                                       // traj_utils.py:76-77: d_xy of frame i rotated by heading[i-1]
-      const float h = s_head[i - 1];
-      const float ct = cosf(h), st = sinf(h);
-      const float x = s_x[i], y = s_y[i];
-      s_x[i] = x * ct - y * st;
-      s_y[i] = x * st + y * ct;
-    }
+    if (i > 0) rotate_dxy(s_head[i - 1], s_x[i], s_y[i]);    // d_xy of frame i rotated by heading[i-1], as in traj_mid
   }
   __syncthreads();
   if (cnt > 0) {
@@ -885,9 +879,15 @@ extern "C" int glamr_opt_set_problem(glamr_opt_t* st, const glamr_problem_t* pb,
     const int rc = join_pending(st, (cudaStream_t)stream);
     if (rc) return rc;
   }
+  // the pipelined blend left v_posed of [n_begin, n_end) in the workspace: another frame-person range must not skin it
+  const bool new_range = pb->n_begin != st->pb.n_begin || pb->n_end != st->pb.n_end;
   st->pb = *pb;
   st->gen++;
   compute_gs(st);
+  if (new_range && !(reset_adam & 2)) {
+    if (st->aux) GLAMR_CUDA_TRY(cudaStreamSynchronize(st->aux));
+    st->vpt_ready = 0;
+  }
   if (reset_adam & 2) {      // handle re-used for a new sequence: scratch (incl. tickets, moments) back to its initial zeros
     if (st->aux) GLAMR_CUDA_TRY(cudaStreamSynchronize(st->aux));
     st->vpt_ready = 0;       // new body poses: the pipelined blend has to be primed again
@@ -1260,6 +1260,8 @@ extern "C" int glamr_opt_read(glamr_opt_t* st, int what, const float** ptr, size
     case GLAMR_R_CAM_POSE_INV: *ptr = st->sc.cam_inv; *count = 12 * T; break;
     case GLAMR_R_JOINTS_WORLD: *ptr = st->sc.joints_world; *count = N * J * 3; break;
     case GLAMR_R_TRAJ_LOCAL: *ptr = st->sc.traj_local; *count = 11 * N; break;
+    case GLAMR_R_ADAM_M: *ptr = st->adam.m; *count = st->pb.n_params; break;
+    case GLAMR_R_ADAM_V: *ptr = st->adam.v; *count = st->pb.n_params; break;
     default: return GLAMR_EINVAL;
   }
   return GLAMR_OK;

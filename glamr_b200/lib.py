@@ -30,7 +30,7 @@ TERM_INDEX = {
 CAM_CONST, CAM_PER_FRAME, CAM_FIXED, CAM_FROM_PERSONS = 0, 1, 2, 3
 TRAJ_PREDICTED, TRAJ_BASE = 0, 1          # enum glamr_traj_source
 (R_ORIENT_WORLD, R_TRANS_WORLD, R_ORIENT_BASE, R_TRANS_BASE, R_KP_PRED, R_ORIENT_CIW, R_TRANS_CIW, R_CAM_POSE,
- R_CAM_POSE_INV, R_JOINTS_WORLD, R_TRAJ_LOCAL) = range(11)
+ R_CAM_POSE_INV, R_JOINTS_WORLD, R_TRAJ_LOCAL, R_ADAM_M, R_ADAM_V) = range(13)
 
 # rowops.cuh
 (ROP_AA_TO_ROTMAT, ROP_RODRIGUES_SMPLX, ROP_ROT6D_TO_ROTMAT, ROP_ROTMAT_TO_QUAT, ROP_QUAT_TO_AA, ROP_AA_TO_QUAT,

@@ -238,7 +238,8 @@ int glamr_opt_create(glamr_opt_t** out, const glamr_smpl_t* smpl, const glamr_pr
 int glamr_opt_destroy(glamr_opt_t* st);
 /* Re-read a modified problem description (new stage: weights, active mask, camera mode; same P, T, J, n_params).
  * reset_adam bit 0 zeroes the Adam moments and step count: the reference builds a fresh torch.optim.Adam per stage
- * (global_recon_model.py:548,:642); bit 1 also zeroes all scratch (handle re-used for a new sequence). */
+ * (global_recon_model.py:548,:642); bit 1 also zeroes all scratch (handle re-used for a new sequence).  A changed
+ * frame-person range [n_begin, n_end) re-primes the pipelined blend: the next evaluation recomputes v_posed for it. */
 int glamr_opt_set_problem(glamr_opt_t* st, const glamr_problem_t* problem, int reset_adam, void* stream);
 /* length (floats) of the caller-owned reduce buffer: [grad (n_params) | un-normalised term sums (GLAMR_NUM_TERMS)] */
 size_t glamr_opt_reduce_count(const glamr_opt_t* st);
@@ -295,7 +296,9 @@ enum glamr_read {
   GLAMR_R_CAM_POSE = 7,        /* [T,12]    world->cam 3x4               */
   GLAMR_R_CAM_POSE_INV = 8,    /* [T,12]                                 */
   GLAMR_R_JOINTS_WORLD = 9,    /* [P,T,J,3]                              */
-  GLAMR_R_TRAJ_LOCAL = 10      /* [P,T,11]  traj_local (rows of the exist range, others 0) */
+  GLAMR_R_TRAJ_LOCAL = 10,     /* [P,T,11]  traj_local (rows of the exist range, others 0) */
+  GLAMR_R_ADAM_M = 11,         /* [n_params] Adam first moment                                */
+  GLAMR_R_ADAM_V = 12          /* [n_params] Adam second moment                               */
 };
 /* ---- multi-GPU without a library collective: gradient reduction over NVLink peer memory --------------------------
  * One process per GPU.  Every rank allocates one buffer (glamr_peer_alloc; size glamr_opt_peer_bytes), ships its
