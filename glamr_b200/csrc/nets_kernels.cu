@@ -78,7 +78,8 @@ __global__ void __launch_bounds__(256) gemm_bias_act_kernel(int M, int N, int K,
 // ------------------------------------------------------------------------------------------------ wgmma GEMM (3xTF32)
 // Y = act(X W^T + b) on the Hopper tensor cores: wgmma.mma_async tf32 with the accumulator in registers.
 // FP32 accuracy is kept with the 3xTF32 split  x = hi + lo (hi = tf32(x), lo = tf32(x - hi)):
-//   X W^T ~= Xhi Whi^T + Xlo Whi^T + Xhi Wlo^T     (error ~2^-21 relative: the 1e-4 parity bar of the infilled pose holds)
+//   X W^T ~= Xhi Whi^T + Xlo Whi^T + Xhi Wlo^T     (error ~2^-21 relative per product; partial sums per K step of 32 are
+//   folded in FP32, see the main loop)
 // CTA = 256 threads = two warpgroups, tile 128 (M) x NT (N), K step 32; warpgroup g computes rows 64 g .. 64 g + 63 (m64nNTk8).
 // Both operands are K-major (X [M,K] and W [N,K] row-major), written by the CTA into shared memory in the canonical no-swizzle
 // layout (8-row x 16-byte core matrices: element (r,k) at ((k/4)*128 + r)*16 + (k%4)*4 bytes => LBO = 2048 B between K groups,
@@ -236,7 +237,11 @@ __global__ void __launch_bounds__(kTcThreads) gemm_tf32x3_wgmma_kernel(int M, in
   asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // generic-proxy smem writes -> visible to the tensor core
   __syncthreads();
 
-  float acc[NT / 2];
+  // Each K step accumulates into `part` on the tensor core, and `part` is folded into `acc` with an FP32 add.  The tensor core's
+  // accumulation does not round to nearest, so a 3xTF32 sum kept in its accumulator over all of K drifts with K (a Linear missed a
+  // float64 product by 4.6x, the infiller's output a float64 oracle by ~20x, what the FP32 kernels miss by); 32-wide partial sums
+  // bound that drift to one K step.
+  float acc[NT / 2], part[NT / 2];
 #pragma unroll
   for (int i = 0; i < NT / 2; ++i) acc[i] = 0.0f;
   for (int it = 0; it < nk; ++it) {
@@ -250,15 +255,14 @@ __global__ void __launch_bounds__(kTcThreads) gemm_tf32x3_wgmma_kernel(int M, in
       const uint64_t dah = wgmma_desc_kmajor_noswizzle(st + koa, TCM), dal = wgmma_desc_kmajor_noswizzle(st + kTcATileFloats + koa, TCM);
       const uint64_t dbh = wgmma_desc_kmajor_noswizzle(st + 2 * kTcATileFloats + kob, NT);
       const uint64_t dbl = wgmma_desc_kmajor_noswizzle(st + 2 * kTcATileFloats + Cfg::kBTileFloats + kob, NT);
-      wgmma_tf32_nt<NT>(acc, dah, dbh, (it > 0 || k8 > 0) ? 1u : 0u);
-      wgmma_tf32_nt<NT>(acc, dal, dbh, 1u);
-      wgmma_tf32_nt<NT>(acc, dah, dbl, 1u);
+      wgmma_tf32_nt<NT>(part, dal, dbh, k8 > 0 ? 1u : 0u);             // the small cross terms first
+      wgmma_tf32_nt<NT>(part, dah, dbl, 1u);
+      wgmma_tf32_nt<NT>(part, dah, dbh, 1u);
     }
     wgmma_commit();
     if (it + 1 < nk) {
-      // stage s^1 was read by both warpgroups' wgmmas of step it-1: retire them, then refill it while step `it` computes
-      wgmma_wait<1>();
-      __syncthreads();
+      // stage s^1 was last read by step it-1, which every warpgroup retired before the barrier that ended that step: refill it
+      // while step `it` computes
       if (WIMG && tid == 0) {                                            // stage s^1 is free: fetch the weight image of step it+1
         mbar_expect_tx(&wbar[s ^ 1], kWBytes);
         tma_bulk_g2s(stage0 + (s ^ 1) * Cfg::kStageFloats + 2 * kTcATileFloats, wimg + (size_t)(it + 1) * (2 * Cfg::kBTileFloats), kWBytes, &wbar[s ^ 1]);
@@ -266,11 +270,13 @@ __global__ void __launch_bounds__(kTcThreads) gemm_tf32x3_wgmma_kernel(int M, in
       if (!(dbg & 2)) tc_store_tiles<NT, WIMG>(stage0 + (s ^ 1) * Cfg::kStageFloats, tid, regs);
       if (it + 2 < nk && !(dbg & 8)) tc_load_tiles<NT, VEC, WIMG>(regs, tid, M, N, K, X, ldx, W, m0, n0, (it + 2) * TCK);
       asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-      __syncthreads();
     }
+    wgmma_wait<0>();
+    wgmma_fence_acc(part);
+#pragma unroll
+    for (int i = 0; i < NT / 2; ++i) acc[i] += part[i];
+    if (it + 1 < nk) __syncthreads();
   }
-  wgmma_wait<0>();                                         // all wgmmas done: the accumulator is final
-  wgmma_fence_acc(acc);
 
   // ---- epilogue: acc[4 i + 2 h + e] = Y[m0 + 64 g + 16 (warp % 4) + lane / 4 + 8 h][n0 + 8 i + 2 (lane % 4) + e]
   if (!(dbg & 4)) {
@@ -310,22 +316,32 @@ struct ScopedFp32Gemm {
   ~ScopedFp32Gemm() { g_gemm_mode = saved; }
 };
 
-// ---- cache of weight operand images, keyed by (device pointer, N, K, tile width); cleared when a network's tensors change
+// ---- weight operand images, keyed by (device pointer, N, K, tile width).  A cache belongs to whoever owns the weights: a
+// glamr_net keeps the images of its own tensors until it replaces one or is destroyed; glamr_linear_forward, whose W is a caller
+// buffer that may be rewritten in place between calls, builds its images for one call only.  g_wimg_cache is the cache of the
+// call in progress (NULL: no images).
 struct WImgKey {
   const float* w; int N, K, NT;
   bool operator<(const WImgKey& o) const { return w != o.w ? w < o.w : (N != o.N ? N < o.N : (K != o.K ? K < o.K : NT < o.NT)); }
 };
-static std::map<WImgKey, float*> g_wimg;
+using WImgCache = std::map<WImgKey, float*>;
+static WImgCache* g_wimg_cache = nullptr;
 static int g_wimg_enabled = -1;     // GLAMR_NET_WIMG=0|1 (default: GLAMR_DEFAULT_NET_WIMG)
-static void wimg_clear() {
-  for (auto& kv : g_wimg) cudaFree(kv.second);
-  g_wimg.clear();
+static void wimg_free(WImgCache& c) {   // the caller has made sure no queued work reads the images
+  for (auto& kv : c) cudaFree(kv.second);
+  c.clear();
 }
+struct ScopedWImgCache {
+  WImgCache* saved;
+  explicit ScopedWImgCache(WImgCache* c) : saved(g_wimg_cache) { g_wimg_cache = c; }
+  ~ScopedWImgCache() { g_wimg_cache = saved; }
+};
 template <int NT>
 static int wimg_get(cudaStream_t s, const float* W, int N, int K, const float** out) {
   const WImgKey key{W, N, K, NT};
-  auto it = g_wimg.find(key);
-  if (it != g_wimg.end()) { *out = it->second; return GLAMR_OK; }
+  WImgCache& cache = *g_wimg_cache;
+  auto it = cache.find(key);
+  if (it != cache.end()) { *out = it->second; return GLAMR_OK; }
   cudaStreamCaptureStatus cap = cudaStreamCaptureStatusNone;
   cudaStreamIsCapturing(s, &cap);
   if (cap != cudaStreamCaptureStatusNone) { *out = nullptr; return GLAMR_OK; }      // never allocate while a graph is being captured
@@ -335,7 +351,7 @@ static int wimg_get(cudaStream_t s, const float* W, int N, int K, const float** 
   const size_t total = (size_t)tiles * ksteps * NT * TCK;
   build_w_image_kernel<NT><<<(unsigned)((total + 255) / 256 < 1056 ? (total + 255) / 256 : 1056), 256, 0, s>>>(W, N, K, ksteps, img);
   GLAMR_LAUNCH_CHECK();
-  g_wimg[key] = img;
+  cache[key] = img;
   *out = img;
   return GLAMR_OK;
 }
@@ -363,7 +379,7 @@ static int gemm_tc_launch(cudaStream_t s, int M, int N, int K, const float* X, i
   dim3 grid((N + NT - 1) / NT, (M + TCM - 1) / TCM);
   const bool vec = (K % 4 == 0) && (ldx % 4 == 0) && (((uintptr_t)X | (uintptr_t)W) % 16 == 0);
   const float* img = nullptr;
-  if (g_wimg_enabled) {
+  if (g_wimg_enabled && g_wimg_cache) {
     const int rc = wimg_get<NT>(s, W, N, K, &img);
     if (rc) return rc;
   }
@@ -720,6 +736,7 @@ using namespace glamr;
 struct glamr_net {
   std::map<std::string, std::pair<float*, size_t>> t;
   std::vector<void*> allocs;
+  mutable WImgCache wimg;           // operand images of this net's weights (GLAMR_NET_WIMG=1), built on first use
 };
 
 namespace {
@@ -834,13 +851,25 @@ int decoder_layer(cudaStream_t s, Arena& A, const DecLayer& L, int B, int S, int
 
 // Y[M,N] = act(X[M,K] W[N,K]^T + bias) -- stand-alone entry for the GEMM used by every Linear of the prior networks
 // (nn.Linear in lib/models/mlp.py:32-41, nn.MultiheadAttention projections, FFN).  mode: 1 wgmma 3xTF32, 0 FP32 SIMT.
+// W is the caller's and may be rewritten between calls, so a weight image (GLAMR_NET_WIMG=1) is built for this call only; the
+// call then waits for its stream before it frees the image.
 extern "C" int glamr_linear_forward(int M, int N, int K, const float* X, const float* W, const float* bias, int relu, float* Y, int mode,
                                     void* stream) {
   if (M <= 0 || N <= 0 || K <= 0 || !X || !W || !Y) return GLAMR_EINVAL;
   const int saved = g_gemm_mode;
   g_gemm_mode = mode;
-  const int rc = gemm((cudaStream_t)stream, M, N, K, X, K, W, bias, nullptr, Y, N, relu ? 1 : 0);
+  WImgCache images;
+  int rc;
+  {
+    ScopedWImgCache scope(&images);
+    rc = gemm((cudaStream_t)stream, M, N, K, X, K, W, bias, nullptr, Y, N, relu ? 1 : 0);
+  }
   g_gemm_mode = saved;
+  if (!images.empty()) {
+    const cudaError_t e = cudaStreamSynchronize((cudaStream_t)stream);
+    wimg_free(images);
+    if (!rc && e != cudaSuccess) rc = (int)e;
+  }
   return rc;
 }
 extern "C" int glamr_net_set_gemm_mode(int mode) {
@@ -857,7 +886,7 @@ extern "C" int glamr_net_create(glamr_net** out) {
 extern "C" int glamr_net_destroy(glamr_net* n) {
   if (!n) return GLAMR_OK;
   cudaDeviceSynchronize();
-  wimg_clear();                              // operand images are keyed by weight pointers that are about to be freed
+  wimg_free(n->wimg);
   for (void* p : n->allocs) cudaFree(p);
   delete n;
   return GLAMR_OK;
@@ -869,7 +898,7 @@ extern "C" int glamr_net_set_tensor(glamr_net* n, const char* name, const float*
   GLAMR_CUDA_TRY(cudaMalloc(&p, numel * sizeof(float)));
   GLAMR_CUDA_TRY(cudaMemcpy(p, host, numel * sizeof(float), cudaMemcpyHostToDevice));
   n->allocs.push_back(p);
-  if (n->t.count(name)) { cudaDeviceSynchronize(); wimg_clear(); }      // a weight was replaced: cached operand images are stale
+  if (n->t.count(name)) { cudaDeviceSynchronize(); wimg_free(n->wimg); }      // a weight was replaced: this net's images are stale
   n->t[name] = {(float*)p, numel};
   return GLAMR_OK;
 }
@@ -900,6 +929,7 @@ extern "C" int glamr_infiller_window_forward(const glamr_net* n, int B, const fl
   const float* pmw = W(n, dd + "p_z_mu_net.weight", 128 * 256, &e), * pmb = W(n, dd + "p_z_mu_net.bias", 128, &e);
   const float* plw = W(n, dd + "p_z_logvar_net.weight", 128 * 256, &e), * plb = W(n, dd + "p_z_logvar_net.bias", 128, &e);
   if (e) return GLAMR_EINVAL;
+  ScopedWImgCache images(&n->wimg);
   Arena A{workspace, workspace_floats, 0};
   const int S = 50, Sc = 30, M = S * B, Mc = Sc * B;
   float* x = A.take((size_t)M * 256);

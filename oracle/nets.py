@@ -45,8 +45,8 @@ class _PosEnc(nn.Module):
         self.fc = nn.Linear(enc_dim + in_dim, enc_dim)
 
     def forward(self, x, pos_offset=0):
-        pos = torch.arange(x.shape[0], device=x.device) + pos_offset
-        mul = torch.exp(torch.arange(0, self.enc_dim, 2, device=x.device) * (-np.log(10000.0) / self.enc_dim))
+        pos = torch.arange(x.shape[0], device=x.device, dtype=x.dtype) + pos_offset
+        mul = torch.exp(torch.arange(0, self.enc_dim, 2, device=x.device, dtype=x.dtype) * (-np.log(10000.0) / self.enc_dim))
         ang = pos.unsqueeze(-1) * mul
         pe = torch.stack([torch.sin(ang), torch.cos(ang)], dim=-1).view(-1, 1, self.enc_dim)
         return self.fc(torch.cat([x, pe.expand(x.shape[:-1] + (self.enc_dim,))], dim=-1))
@@ -61,7 +61,7 @@ class _BiLSTM(nn.Module):
         self.rnn_b = nn.LSTMCell(din, dout // 2)
 
     def _run(self, cell, x, reverse):
-        h = torch.zeros(x.shape[1], cell.hidden_size)
+        h = torch.zeros(x.shape[1], cell.hidden_size, dtype=x.dtype)
         c = torch.zeros_like(h)
         outs = [None] * x.shape[0]
         for t in (reversed(range(x.shape[0])) if reverse else range(x.shape[0])):
@@ -121,7 +121,8 @@ class MotionInfiller(nn.Module):
     def inference(self, batch):
         """multi-step, sample_num 1 (:618-652): in_body_pose [B,T,69], frame_mask [B,T] (1 = visible),
         optional in_motion_latent [n_windows,128] -> infer_out_body_pose [B,1,T,69]"""
-        pose = batch['in_body_pose'].transpose(0, 1).contiguous().float().clone()        # [T,B,69]
+        dt = self.data_decoder.out_fc.weight.dtype                                       # the module's dtype (float32 or float64)
+        pose = batch['in_body_pose'].transpose(0, 1).contiguous().to(dt).clone()         # [T,B,69]
         key_pad_all = ~(batch['frame_mask'] == 1)                                        # True where NOT visible
         T, B = pose.shape[0], pose.shape[1]
         W = PAST + CUR + FUT
@@ -132,11 +133,11 @@ class MotionInfiller(nn.Module):
             win = pose[s:eb]
             kp = key_pad_all[:, s:eb]
             if e > eb:
-                win = torch.cat([win, torch.zeros(e - eb, B, 69)], dim=0)
+                win = torch.cat([win, torch.zeros(e - eb, B, 69, dtype=dt)], dim=0)
                 kp = torch.cat([kp, torch.ones(B, e - eb, dtype=torch.bool)], dim=1)
             kp = kp.clone()
             kp[:, :PAST] = False
-            eps = batch['in_motion_latent'][[i]].float() if 'in_motion_latent' in batch else None
+            eps = batch['in_motion_latent'][[i]].to(dt) if 'in_motion_latent' in batch else None
             out = self.window(win, kp, eps)
             nfr = min(e - FUT, T) - s
             pose[s:s + nfr] = out[:nfr]
@@ -184,7 +185,7 @@ class TrajPredictor(nn.Module):
         out = dd.out_fc(dd.out_mlp(torch.cat([z.repeat(ctx.shape[0], 1, 1), ctx], dim=-1)))
         local = out.clone()
         local[0, :, :2] = 0.0 if init_xy is None else init_xy
-        local[0, :, -2:] = torch.tensor([0.0, 1.0]) if init_heading is None else rt.heading_to_vec(init_heading)
+        local[0, :, -2:] = torch.tensor([0.0, 1.0], dtype=local.dtype) if init_heading is None else rt.heading_to_vec(init_heading)
         trans, q = tc.local_to_global(local)
         return local, trans, rt.quat_to_aa(q)
 
@@ -192,10 +193,11 @@ class TrajPredictor(nn.Module):
 class MotionTrajJoint:
     """motion_traj_joint_model.py:141-145 with multi_step_mfiller=True, multi_step_trajpred=False, sample_num 1"""
 
-    def __init__(self, state_mfiller, state_traj, smpl):
-        self.mfiller, self.traj_predictor, self.smpl = MotionInfiller(), TrajPredictor(), smpl
-        load_state(self.mfiller, state_mfiller)
-        load_state(self.traj_predictor, state_traj)
+    def __init__(self, state_mfiller, state_traj, smpl, dtype=torch.float32):
+        """dtype: of the networks and their inputs; smpl (OracleSMPL) should be built in the same dtype"""
+        self.mfiller, self.traj_predictor, self.smpl, self.dtype = MotionInfiller(), TrajPredictor(), smpl, dtype
+        load_state(self.mfiller, state_mfiller, dtype)
+        load_state(self.traj_predictor, state_traj, dtype)
 
     @torch.no_grad()
     def inference(self, batch, sample_num=1):
@@ -207,7 +209,7 @@ class MotionTrajJoint:
         flat = body.reshape(-1, 69)
         z3 = torch.zeros_like(flat[:, :3])
         joints = self.smpl.get_joints(z3, flat, root_trans=z3)[:, 1:].reshape(B, T, 69).transpose(0, 1).contiguous()
-        eps = batch['in_traj_latent'].float() if 'in_traj_latent' in batch else None
+        eps = batch['in_traj_latent'].to(self.dtype) if 'in_traj_latent' in batch else None
         local, trans, orient = self.traj_predictor.inference(joints, eps)
         data['infer_out_local_traj_tp'] = local.view(T, B, 1, 11)
         data['infer_out_trans'] = trans.transpose(0, 1).unsqueeze(1).contiguous()
@@ -216,9 +218,11 @@ class MotionTrajJoint:
         return data
 
 
-def load_state(module, state):
+def load_state(module, state, dtype=torch.float32):
+    """load a state dict into `module` and convert the module to `dtype`"""
     own = module.state_dict()
     missing = [k for k in own if k not in state]
     if missing:
         raise KeyError(f'missing parameters: {missing[:5]} ...')
-    module.load_state_dict({k: torch.as_tensor(np.asarray(state[k])).float() for k in own}, strict=True)
+    module.to(dtype)
+    module.load_state_dict({k: torch.as_tensor(np.asarray(state[k])).to(dtype) for k in own}, strict=True)

@@ -1,0 +1,768 @@
+"""The learned prior's networks against a float64 restatement: window by window and frame by frame, at the GEMM dispatch edges,
+the window sweep's ragged edges and the trajectory codec's scan-chunk edges.
+
+The reference is oracle.nets in float64 (pure torch, never the library), fed the same float32 inputs and weights.  The float32
+oracle is the yardstick for what float32 arithmetic costs.  Every output element is held to
+
+    |got - o64| <= C * D(b) + R * 2^-24 * |o64|
+
+  D(b)  the largest |o32 - o64| of the float32 oracle in the element's block and sequence: one block per 30-frame window for the
+        infilled pose (frames 0-39 are window 0), one per 32 frames for the trajectory outputs.  D has a floor of FLOOR times the
+        output's peak.  The codec's two prefix sums get the floor 2^-22 sqrt(T) times the scan's largest partial sum instead
+        (torch's float32 cumsum on the CPU accumulates in float64, so the float32 oracle understates a float32 scan); the heading
+        floor reaches the translation through the rotated xy steps, times their summed length.
+  R     the rounding of the float32 output itself.
+Orientations are compared as rotation matrices: axis-angle is ill-conditioned near pi, and quat_to_aa's clamp has a kink near
+the identity.  Linear layers alone are held to C_LIN * 2^-22 * (sum_k |x_k w_k| + |b|), which a 3xTF32 split that drops a cross
+term exceeds by orders of magnitude.
+
+C = 4, R = 8, FLOOR = 2^-24, ORIENT_FLOOR = 2^-20 (rotation-matrix elements) and C_LIN = 16 were set from measurements on an
+H100 80GB HBM3 at a 700 W power limit.  Worst measured |got - o64| / bound over the cases of each test:
+
+    linear layers, every variant       tensor cores 0.13, FP32 kernels 0.078 (a weight rewritten in place: 0.034)
+    one infiller window                0.14 at B <= 5 (FP32 skinny GEMMs), 0.32 at B >= 6 (tensor cores);
+                                       0.32 on the weight-image path with a second net destroyed between calls
+    infiller sweep                     0.15 at B <= 3, 0.39 at 64 x 71
+    trajectory predictor               local 0.36, trans 0.49, orient 0.25
+    codec alone                        trans 0.011 / 7.9e-5, orient 0.33 / 0.0053 (local_heading 0 / 1)
+    end to end, 64 x 120               pose 0.35, local 0.37, trans 0.32, orient 0.019
+    end to end, 2 x 600 with gaps      pose 0.17, local 0.30, trans 0.38, orient 0.0058
+
+C_LIN leaves 8x over the worst linear layer, and a split that drops a cross term costs about 2^-11 sum |x w|, 128x the bound.  The
+block bound has less room on both sides: D is itself one float32 rounding pattern, and another float32 computation of the same
+outputs (the kernels) reaches up to 2 D in a block, while the cheapest modelled bugs below cost 7-10 D.  C = 4 leaves 2x over the
+worst measured case, and the cheapest bugs break it by 1.7x (the trajectory context MLP as 2xTF32), 2.4x (every LayerNorm with
+eps 1e-6) and 2.5x (the encoder's first FFN layer as 2xTF32); the rest break it by 4x to 10^6x.
+
+The CPU tests apply the modelled bugs to the float32 oracle and print the factor by which each breaks the bound.
+"""
+import gc
+import json
+import math
+import os
+import subprocess
+import sys
+
+import numpy as np
+import pytest
+import torch
+import torch.nn.functional as F
+
+REPO = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+if REPO not in sys.path:
+    sys.path.insert(0, REPO)
+
+from glamr_b200.synthetic_nets import make_prior_states  # noqa: E402
+from oracle import nets as on  # noqa: E402
+from oracle import rotations as rt  # noqa: E402
+from oracle import traj_codec as tc  # noqa: E402
+
+DEV = 'cuda:0'
+U = 2.0 ** -24
+C, R, FLOOR = 4.0, 8.0, 2.0 ** -24          # block bound; FLOOR is relative to the output's peak
+ORIENT_FLOOR = 2.0 ** -20                   # floor of the rotation-matrix elements (16 ulp of 1)
+SCAN = 2.0 ** -22                           # prefix-scan floor, times sqrt(T) and the largest partial sum
+C_LIN = 16.0                                # linear layers, times 2^-22 sum |x w|
+TBLOCK = 32                                 # frames per block of the trajectory outputs
+SCAN_CHUNK = 512                            # elements per pass of the library's block scan (glamr_b200/csrc/block_scan.cuh)
+
+
+# ------------------------------------------------------------------------------------------------ the bound
+def window_blocks(T):
+    """block of each frame of the infilled pose: frames 0-39 are window 0, then one block per 30-frame window"""
+    t = torch.arange(T)
+    return torch.where(t < 40, torch.zeros_like(t), (t - 10) // 30)
+
+
+def frame_blocks(T):
+    return torch.arange(T) // TBLOCK
+
+
+def block_bound(o32, o64, bid, floor):
+    """o32, o64 [T,B,F]; bid [T] block per frame; floor: scalar, [B] or [T,B] -> per-element bound [T,B,F]"""
+    o32, o64 = o32.double().cpu(), o64.double().cpu()
+    d = (o32 - o64).abs().amax(-1)                                                     # [T,B]
+    Db = torch.zeros(int(bid.max()) + 1, d.shape[1], dtype=torch.float64).index_reduce_(0, bid, d, 'amax')
+    D = torch.maximum(Db[bid], torch.as_tensor(floor, dtype=torch.float64).expand_as(d))
+    return C * D[..., None] + R * U * o64.abs()
+
+
+def worst(got, o64, bnd):
+    """largest |got - o64| / bound (nan when an element is not finite; an exact element scores 0 against a zero bound)"""
+    err = (got.double().cpu() - o64.double().cpu()).abs()
+    return float(torch.where(err == 0, torch.zeros_like(err), err / bnd).max())
+
+
+def peak_floor(o64):
+    return FLOOR * float(o64.abs().max())
+
+
+def codec_floors(local64, local_heading=True):
+    """[B] floors of the heading scan and of the xy scan (with the heading floor carried through the rotated steps)"""
+    local64 = local64.double().cpu()
+    T = local64.shape[0]
+    dh = rt.vec_to_heading(local64[..., -2:])
+    heading = torch.cumsum(dh, 0) if local_heading else dh
+    trans, _ = tc.local_to_global(local64, local_heading)
+    head = SCAN * math.sqrt(T) * heading.abs().amax(0) if local_heading else torch.zeros(local64.shape[1], dtype=torch.float64)
+    steps = local64[1:, :, :2].norm(dim=-1).sum(0) if T > 1 else torch.zeros_like(head)
+    xy = SCAN * math.sqrt(T) * trans[..., :2].abs().amax(0).amax(-1) + head * steps
+    return head, xy
+
+
+def rodrigues(aa):
+    """exact axis-angle -> rotation matrix in float64 (no small-angle branch) [..., 9]"""
+    aa = aa.double().cpu()
+    th = aa.norm(dim=-1, keepdim=True)
+    k = aa / th.clamp_min(1e-300)
+    K = torch.zeros(aa.shape[:-1] + (3, 3), dtype=torch.float64)
+    K[..., 0, 1], K[..., 0, 2], K[..., 1, 2] = -k[..., 2], k[..., 1], -k[..., 0]
+    K = K - K.transpose(-1, -2)
+    s, c = torch.sin(th)[..., None], torch.cos(th)[..., None]
+    return (torch.eye(3, dtype=torch.float64) + s * K + (1 - c) * K @ K).reshape(aa.shape[:-1] + (9,))
+
+
+def quat_rotmat(q):
+    return rt.quat_to_rotmat(q.double().cpu()).reshape(q.shape[:-1] + (9,))
+
+
+def traj_bounds(local32, local64, trans32, trans64, rot32, rot64, local_heading=True):
+    """bounds of the trajectory outputs [T,B,*]: local element-wise block bound; trans and orientation (rotation matrix) with
+    the scan floors"""
+    T = trans64.shape[0]
+    bid = frame_blocks(T)
+    head, xy = codec_floors(local64, local_heading)
+    out = {}
+    if local32 is not None:
+        out['local'] = block_bound(local32, local64, bid, peak_floor(local64))
+    bt = block_bound(trans32[..., :2], trans64[..., :2], bid, torch.clamp_min(xy, peak_floor(trans64[..., :2])))
+    bz = block_bound(trans32[..., 2:], trans64[..., 2:], bid, peak_floor(trans64[..., 2:]))
+    out['trans'] = torch.cat([bt, bz], -1)
+    out['orient'] = block_bound(rot32, rot64, bid, torch.clamp_min(head, ORIENT_FLOOR))
+    return out
+
+
+# ------------------------------------------------------------------------------------------------ oracle sweeps with bug knobs
+@torch.no_grad()
+def infill_sweep(m, pose, mask, lat, kp_shift=0, commit=0):
+    """MotionInfiller.inference written as the library runs it: the window outputs are committed into the running pose, which is
+    the result.  pose [B,T,69], mask [B,T] (1 = visible), lat [n_windows, 1|B, 128] -> [T,B,69] in the module's dtype.
+    kp_shift: the key-padding mask of the last ragged window shifted by that many frames; commit: frames added to every full
+    window's commit (written as zeros, what a commit past the window's 40 output frames would read)."""
+    dt = m.data_decoder.out_fc.weight.dtype
+    pose = pose.transpose(0, 1).to(dt).clone()
+    kpa = ~(mask == 1)
+    T, B = pose.shape[:2]
+    nwin = int(np.ceil((T - on.PAST) / on.CUR))
+    for i in range(nwin):
+        s, e = i * on.CUR, i * on.CUR + 50
+        eb = min(e, T)
+        win, kp = pose[s:eb], kpa[:, s:eb]
+        if e > eb:
+            win = torch.cat([win, torch.zeros(e - eb, B, 69, dtype=dt, device=pose.device)])
+            kp = torch.cat([kp, torch.ones(B, e - eb, dtype=torch.bool, device=pose.device)], 1)
+        kp = kp.clone()
+        if kp_shift and e > eb and i == nwin - 1:
+            kp[:, on.PAST:] = torch.roll(kp[:, on.PAST:], kp_shift, dims=1)
+        kp[:, :on.PAST] = False
+        out = m.window(win, kp, lat[i].to(dt))
+        nfr = min(e - on.FUT, T) - s
+        pose[s:s + nfr] = out[:nfr]
+        if commit and nfr == 40:
+            if commit < 0:
+                pose[s + nfr + commit:s + nfr] = win[nfr + commit:nfr]
+            elif s + nfr < T:
+                pose[s + nfr:s + nfr + commit] = 0.0
+    return pose
+
+
+@torch.no_grad()
+def traj_forward(tp, jp, eps, init_xy=None, init_heading=None, mean_drop=0, lstm_skip=None, carry_lost=None):
+    """TrajPredictor.inference with bug knobs -> local [T,B,11], trans [T,B,3], orient quaternion [T,B,4].
+    mean_drop: frames left out of the context mean; lstm_skip: step of the backward LSTM (first layer) that is skipped;
+    carry_lost: chunk edge at which the heading scan restarts from zero."""
+    ce, dd = tp.context_encoder, tp.data_decoder
+    x = ce.in_mlp(jp)
+    for li, net in enumerate(ce.temporal_net):
+        outs = []
+        for cell, rev in ((net.rnn_f, False), (net.rnn_b, True)):
+            h = torch.zeros(x.shape[1], cell.hidden_size, dtype=x.dtype)
+            c = torch.zeros_like(h)
+            o = [None] * x.shape[0]
+            for t in (reversed(range(x.shape[0])) if rev else range(x.shape[0])):
+                if not (rev and li == 0 and t == lstm_skip):
+                    h, c = cell(x[t], (h, c))
+                o[t] = h
+            outs.append(torch.stack(o, 0))
+        x = torch.cat(outs, 2)
+    ctx = ce.out_mlp(x)
+    mean = ctx[:ctx.shape[0] - mean_drop].mean(dim=0) if mean_drop else ctx.mean(dim=0)
+    mu, logvar = torch.chunk(dd.p_z_net(dd.prior_mlp(mean)), 2, dim=-1)
+    z = mu + eps * torch.exp(0.5 * logvar)
+    out = dd.out_fc(dd.out_mlp(torch.cat([z.repeat(ctx.shape[0], 1, 1), ctx], dim=-1)))
+    local = out.clone()
+    local[0, :, :2] = 0.0 if init_xy is None else init_xy
+    local[0, :, -2:] = torch.tensor([0.0, 1.0], dtype=local.dtype) if init_heading is None else rt.heading_to_vec(init_heading)
+    if carry_lost is None:
+        trans, q = tc.local_to_global(local)
+    else:
+        trans, q = codec_carry_lost(local, carry_lost)
+    return local, trans, q
+
+
+def codec_carry_lost(local, edge):
+    """tc.local_to_global with the heading scan restarting from zero at `edge`"""
+    base = torch.tensor(tc.BASE_ORIENT, dtype=local.dtype)
+    heading = torch.cumsum(rt.vec_to_heading(local[..., -2:]), 0)
+    heading = torch.cat([heading[:edge], heading[edge:] - heading[edge - 1]])
+    d_xy = torch.cat([local[:1, ..., :2], tc.rot_2d(local[1:, ..., :2], heading[:-1])], 0)
+    trans = torch.cat([torch.cumsum(d_xy, 0), local[..., 2:3]], -1)
+    q = rt.quat_mul(rt.quat_mul(rt.heading_to_quat(heading), rt.rot6d_to_quat(local[..., 3:-2])), base.expand(local.shape[:-1] + (4,)))
+    return trans, q
+
+
+def tf32(x):
+    """round to tf32 (10 explicit mantissa bits, to nearest): what a weight that lost its low half looks like"""
+    i = x.detach().float().contiguous().view(torch.int32)
+    return ((i + 0x1000) & ~0x1fff).view(torch.float32).to(x.dtype)
+
+
+def linear_2xtf32(lin):
+    """lin.forward as a 3xTF32 split without the Xlo Whi term"""
+    wh = tf32(lin.weight)
+    wl = tf32(lin.weight - wh)
+    lin.forward = lambda x: F.linear(tf32(x), wh) + F.linear(tf32(x), wl) + lin.bias
+
+
+# ------------------------------------------------------------------------------------------------ CPU: the bound rejects bugs
+_STATES = {}
+
+
+def states():
+    if not _STATES:
+        _STATES['m'], _STATES['t'] = make_prior_states(1234)
+    return _STATES['m'], _STATES['t']
+
+
+def infiller(dtype=torch.float32):
+    m = on.MotionInfiller()
+    on.load_state(m, states()[0], dtype)
+    return m
+
+
+def trajpred(dtype=torch.float32):
+    t = on.TrajPredictor()
+    on.load_state(t, states()[1], dtype)
+    return t
+
+
+def infill_inputs(B, T, seed, gaps=()):
+    g = torch.Generator().manual_seed(seed)
+    pose = torch.randn(B, T, 69, generator=g) * 0.3
+    mask = (torch.rand(B, T, generator=g) > 0.3).float()
+    mask[:, :10] = 1
+    for b, s, e in gaps:
+        mask[b, s:e] = 0
+    lat = torch.randn(int(np.ceil((T - 10) / 30)), 1, 128, generator=g)
+    return pose * mask[..., None], mask, lat
+
+
+def traj_inputs(B, T, seed):
+    g = torch.Generator().manual_seed(seed)
+    return torch.randn(T, B, 69, generator=g) * 0.3, torch.randn(1, 128, generator=g)
+
+
+_CPU_REF = {}
+
+
+def cpu_infill_ref():
+    """float32 and float64 oracle on the CPU at 2 x 100: three windows, the last one ragged"""
+    if not _CPU_REF.get('infill'):
+        pose, mask, lat = infill_inputs(2, 100, 7, gaps=[(0, 35, 52), (1, 62, 95)])
+        o32 = infill_sweep(infiller(), pose, mask, lat)
+        o64 = infill_sweep(infiller(torch.float64), pose, mask, lat)
+        _CPU_REF['infill'] = (pose, mask, lat, o64, block_bound(o32, o64, window_blocks(100), peak_floor(o64)))
+    return _CPU_REF['infill']
+
+
+def cpu_traj_ref(B, T):
+    """float32 and float64 oracle on the CPU"""
+    if not _CPU_REF.get(('traj', B, T)):
+        jp, eps = traj_inputs(B, T, 11)
+        r32 = traj_forward(trajpred(), jp, eps)
+        r64 = traj_forward(trajpred(torch.float64), jp.double(), eps.double())
+        b = traj_bounds(r32[0], r64[0], r32[1], r64[1], quat_rotmat(r32[2]), quat_rotmat(r64[2]))
+        _CPU_REF[('traj', B, T)] = (jp, eps, r64, b)
+    return _CPU_REF[('traj', B, T)]
+
+
+def test_oracle_restatements_match_the_oracle():
+    """the sweeps above, without bugs, are oracle.nets bit for bit (float32)"""
+    pose, mask, lat = infill_inputs(2, 100, 7)
+    ref = infiller().inference({'in_body_pose': pose, 'frame_mask': mask, 'in_motion_latent': lat[:, 0]})['infer_out_body_pose']
+    assert torch.equal(infill_sweep(infiller(), pose, mask, lat), ref[:, 0].transpose(0, 1))
+    jp, eps = traj_inputs(2, 40, 3)
+    local, trans, q = traj_forward(trajpred(), jp, eps, torch.ones(2, 2), torch.tensor([0.3, -2.0]))
+    rl, rtr, raa = trajpred().inference(jp, eps, torch.ones(2, 2), torch.tensor([0.3, -2.0]))
+    assert torch.equal(local, rl) and torch.equal(trans, rtr) and torch.equal(rt.quat_to_aa(q), raa)
+
+
+INFILL_TF32 = ['context_encoder.temporal_net.layers.0.self_attn.in_proj_weight',        # QKV projection
+               'data_decoder.temporal_net.layers.1.multihead_attn.in_proj_weight',
+               'context_encoder.temporal_net.layers.0.linear1.weight',                   # FFN
+               'data_decoder.temporal_net.layers.1.linear2.weight',
+               'data_decoder.out_fc.weight']
+
+
+def _infill_bug(name):
+    m = infiller()
+    mods = dict(m.named_modules())
+    kw = {}
+    if name.startswith('tf32:'):
+        p = dict(m.named_parameters())[name[5:]]
+        with torch.no_grad():
+            p.copy_(tf32(p))
+    elif name.startswith('2xtf32:'):
+        linear_2xtf32(mods[name[7:]])
+    elif name == 'last_window_mask_shift':
+        kw['kp_shift'] = 1
+    elif name.startswith('commit'):
+        kw['commit'] = int(name[6:]) - 40
+    elif name == 'decoder_pe_offset_9':
+        pe = m.data_decoder.pos_enc
+        fwd = pe.forward
+        pe.forward = lambda x, pos_offset=0: fwd(x, pos_offset - 1 if pos_offset else 0)
+    elif name == 'layernorm_eps_1e-6':
+        for mod in m.modules():
+            if isinstance(mod, torch.nn.LayerNorm):
+                mod.eps = 1e-6
+    return m, kw
+
+
+INFILL_BUGS = (['tf32:' + n for n in INFILL_TF32] +
+               ['2xtf32:context_encoder.temporal_net.layers.0.linear1', '2xtf32:data_decoder.temporal_net.layers.1.linear2',
+                'last_window_mask_shift', 'commit39', 'commit41', 'decoder_pe_offset_9', 'layernorm_eps_1e-6'])
+
+
+@pytest.mark.parametrize('bug', INFILL_BUGS)
+def test_bound_rejects_modelled_infiller_bug(bug):
+    pose, mask, lat, o64, bnd = cpu_infill_ref()
+    m, kw = _infill_bug(bug)
+    r = worst(infill_sweep(m, pose, mask, lat, **kw), o64, bnd)
+    print(f'{bug}: worst |o - o64| / bound = {r:.3g}')
+    assert r > 1.0, f'{bug} stays within the bound ({r:.3g})'
+
+
+# An LSTM input projection (weight_ih) rounded to tf32 is not among these: with the seeded weights it moves the trajectory outputs
+# by less than the float32 oracle's own rounding (0.25-0.5 of the bound at T = 8, 40 and 600), so no bound on the outputs can see
+# it.  The trajectory predictor runs its Linear layers on the FP32 kernels, which test_linear_layers_match_float64 checks directly.
+TRAJ_BUGS = ['tf32:data_decoder.out_fc.weight', 'tf32:data_decoder.out_mlp.affine_layers.0.weight',
+             '2xtf32:data_decoder.out_mlp.affine_layers.1', '2xtf32:context_encoder.out_mlp.affine_layers.0', 'context_mean_over_T-1',
+             'backward_lstm_step_skipped', 'heading_carry_lost_at_512']
+
+
+@pytest.mark.parametrize('bug', TRAJ_BUGS)
+def test_bound_rejects_modelled_trajectory_bug(bug):
+    """at 1 x 600 (the heading scan crosses a chunk edge); the context mean at 2 x 8, where one frame is an eighth of it"""
+    jp, eps, r64, bnd = cpu_traj_ref(2, 8) if bug == 'context_mean_over_T-1' else cpu_traj_ref(1, 600)
+    t = trajpred()
+    kw = {}
+    if bug.startswith('tf32:'):
+        p = dict(t.named_parameters())[bug[5:]]
+        with torch.no_grad():
+            p.copy_(tf32(p))
+    elif bug.startswith('2xtf32:'):
+        linear_2xtf32(dict(t.named_modules())[bug[7:]])
+    elif bug == 'context_mean_over_T-1':
+        kw['mean_drop'] = 1
+    elif bug == 'backward_lstm_step_skipped':
+        kw['lstm_skip'] = 300
+    elif bug == 'heading_carry_lost_at_512':
+        kw['carry_lost'] = SCAN_CHUNK
+    local, trans, q = traj_forward(t, jp, eps, **kw)
+    rs = {'local': worst(local, r64[0], bnd['local']), 'trans': worst(trans, r64[1], bnd['trans']),
+          'orient': worst(quat_rotmat(q), quat_rotmat(r64[2]), bnd['orient'])}
+    print(f'{bug}: worst |o - o64| / bound = ' + ', '.join(f'{k} {v:.3g}' for k, v in rs.items()))
+    assert max(rs.values()) > 1.0, f'{bug} stays within the bound ({rs})'
+
+
+# ------------------------------------------------------------------------------------------------ GPU: the library
+def _lib():
+    import ctypes
+    from glamr_b200 import lib as L
+    from glamr_b200 import motion_traj as mt
+    lib = L.load()
+    mt._declare(lib)
+    vp, ci = ctypes.c_void_p, ctypes.c_int
+    lib.glamr_linear_forward.argtypes = [ci] * 3 + [vp] * 3 + [ci, vp, ci, vp]
+    lib.glamr_traj_local2global.argtypes = [ci, ci, vp, ci, vp, vp, vp, vp]
+    return lib
+
+
+def _ptr(x):
+    return None if x is None else x.data_ptr()
+
+
+def _stream():
+    return torch.cuda.current_stream().cuda_stream
+
+
+def _check(rc, what):
+    from glamr_b200 import lib as L
+    L.check(rc, what)
+
+
+LIN_M = (1, 7, 8, 9, 127, 128, 129, 255, 256, 257, 3200)
+LIN_N = (11, 31, 32, 33, 69, 128, 129, 512)
+LIN_K = (3, 31, 32, 33, 69, 256, 384, 512)
+
+
+def linear_shapes():
+    """every M with every N and every K (the other dimension rotating), relu alternating"""
+    out = []
+    for i, M in enumerate(LIN_M):
+        for j, N in enumerate(LIN_N):
+            out.append((M, N, LIN_K[(i + j) % len(LIN_K)], (i + j) & 1))
+        for j, K in enumerate(LIN_K):
+            out.append((M, LIN_N[(i + j + 3) % len(LIN_N)], K, (i + j + 1) & 1))
+    return out
+
+
+def run_linear_sweep():
+    """glamr_linear_forward in mode 1 (tensor cores) and 0 (FP32) at every shape -> worst |y - y64| / bound per mode"""
+    lib = _lib()
+    res = {}
+    for mode in (1, 0):
+        rs = []
+        for M, N, K, relu in linear_shapes():
+            g = torch.Generator().manual_seed(M * 7919 + N * 31 + K)
+            X = torch.randn(M, K, generator=g).to(DEV)
+            W = (torch.randn(N, K, generator=g) / K ** 0.5).to(DEV)
+            b = torch.randn(N, generator=g).to(DEV)
+            ref = X.double() @ W.double().T + b.double()
+            scale = X.double().abs() @ W.double().abs().T + b.double().abs()
+            if relu:
+                ref = ref.clamp_min(0)
+            Y = torch.full((M, N), float('nan'), device=DEV)
+            _check(lib.glamr_linear_forward(M, N, K, X.data_ptr(), W.data_ptr(), b.data_ptr(), relu, Y.data_ptr(), mode, _stream()), 'linear')
+            rs.append(float(((Y.double() - ref).abs() / (C_LIN * 2.0 ** -22 * scale)).max()))
+        res[f'mode{mode}'] = max(rs) if all(r == r for r in rs) else float('nan')
+    return res
+
+
+def run_stale_image():
+    """glamr_linear_forward, W rewritten in place between two calls: the second result must follow the new W"""
+    lib = _lib()
+    res = {}
+    for M, N, K in [(300, 256, 256), (64, 69, 256)]:
+        g = torch.Generator().manual_seed(M + N)
+        X = torch.randn(M, K, generator=g).to(DEV)
+        W = (torch.randn(N, K, generator=g) / K ** 0.5).to(DEV)
+        W2 = (torch.randn(N, K, generator=g) / K ** 0.5).to(DEV)
+        ptr = W.data_ptr()
+        for step, Wv in enumerate((W, W2)):
+            W.copy_(Wv)
+            assert W.data_ptr() == ptr
+            Y = torch.full((M, N), float('nan'), device=DEV)
+            _check(lib.glamr_linear_forward(M, N, K, X.data_ptr(), W.data_ptr(), None, 0, Y.data_ptr(), 1, _stream()), 'linear')
+            ref = X.double() @ W.double().T
+            scale = X.double().abs() @ W.double().abs().T
+            res[f'{M}x{N}x{K} call {step + 1}'] = float(((Y.double() - ref).abs() / (C_LIN * 2.0 ** -22 * scale)).max())
+    return res
+
+
+# window key masks [B,50] (True = not usable as a key)
+def window_masks(B, g):
+    allv = torch.zeros(B, 50, dtype=torch.bool)
+    past = torch.ones(B, 50, dtype=torch.bool)
+    past[:, :10] = False
+    single = torch.ones(B, 50, dtype=torch.bool)
+    single[torch.arange(B), torch.randint(0, 50, (B,), generator=g)] = False
+    alt = torch.zeros(B, 50, dtype=torch.bool)
+    alt[:, 1::2] = True
+    rnd = torch.rand(B, 50, generator=g) > 0.5
+    rnd[:, 0] = False
+    return {'all_visible': allv, 'past_only': past, 'single_key': single, 'alternating': alt, 'random': rnd}
+
+
+WINDOW_B = (1, 5, 6, 9, 64)
+
+
+def run_window_cases(cases, net=None, between=None):
+    """glamr_infiller_window_forward vs MotionInfiller.window in float64, per (B, mask, eps mode) case -> worst ratio per case.
+    between: called after each library call (the image-ownership check destroys another net there)"""
+    from glamr_b200 import motion_traj as mt
+    lib = _lib()
+    if net is None:
+        net = mt._Net(states()[0], torch.device(DEV))
+    m32, m64 = infiller(), infiller(torch.float64).to(DEV)
+    res = {}
+    for B, mname, emode in cases:
+        g = torch.Generator().manual_seed(B * 100 + len(mname))
+        pose = torch.randn(50, B, 69, generator=g) * 0.3
+        kp = window_masks(B, g)[mname]
+        eps = None if emode == 'null' else torch.randn(1 if emode == 'rows1' else B, 128, generator=g)
+        ws = torch.empty(int(lib.glamr_infiller_workspace_floats(B)), device=DEV)
+        out = torch.full((40, B, 69), float('nan'), device=DEV)
+        pose_d, kp_d, eps_d = pose.to(DEV), kp.to(torch.uint8).to(DEV), None if eps is None else eps.to(DEV)
+        _check(lib.glamr_infiller_window_forward(net.h, B, pose_d.data_ptr(), kp_d.data_ptr(), _ptr(eps_d),
+                                                 1 if emode == 'rows1' else B, out.data_ptr(), ws.data_ptr(), ws.numel(), _stream()), 'window')
+        torch.cuda.synchronize()
+        if between is not None:
+            between()
+        e0 = torch.zeros(1, 128) if eps is None else eps
+        with torch.no_grad():
+            o32 = m32.window(pose, kp, e0)
+            o64 = m64.window(pose.double().to(DEV), kp.to(DEV), e0.double().to(DEV)).cpu()
+        bnd = block_bound(o32, o64, torch.zeros(40, dtype=torch.long), peak_floor(o64))
+        res[f'B{B} {mname} eps {emode}'] = worst(out, o64, bnd)
+    return res
+
+
+def window_cases():
+    names = ('all_visible', 'past_only', 'single_key', 'alternating', 'random')
+    modes = ('rows1', 'rowsB', 'null')
+    return [(B, n, modes[(i + j) % 3]) for i, B in enumerate(WINDOW_B) for j, n in enumerate(names)]
+
+
+def run_image_ownership():
+    """the image path of the infiller window with two nets alive, one destroyed between calls: results must not change"""
+    from glamr_b200 import motion_traj as mt
+    net = mt._Net(states()[0], torch.device(DEV))
+    other = [mt._Net(states()[0], torch.device(DEV))]
+    cases = [(1, 'random', 'rowsB'), (6, 'past_only', 'null'), (64, 'alternating', 'rows1')]
+    warm = run_window_cases(cases[:1], net=other[0])           # `other` builds images of its own weights
+
+    def destroy_other():
+        if other:
+            other.pop()
+            gc.collect()
+    first = run_window_cases(cases, net=net, between=destroy_other)
+    again = run_window_cases(cases, net=net)
+    return {**{'other ' + k: v for k, v in warm.items()}, **first, **{'again ' + k: v for k, v in again.items()}}
+
+
+def _child(what, env):
+    """run one of the variant functions in a fresh python process (the dispatch switches are read once per process)"""
+    e = dict(os.environ, **env)
+    e['PYTHONPATH'] = os.pathsep.join([REPO, os.path.join(REPO, 'tests')] + ([e['PYTHONPATH']] if e.get('PYTHONPATH') else []))
+    p = subprocess.run([sys.executable, os.path.abspath(__file__), what], env=e, capture_output=True, text=True, timeout=900)
+    assert p.returncode == 0, p.stdout[-3000:] + p.stderr[-3000:]
+    return json.loads(p.stdout.strip().splitlines()[-1])
+
+
+LINEAR_VARIANTS = {
+    'default': {},                                               # skinny (VEC and not) at M <= 256, wgmma NT=128 / FP32 tile above
+    'tiles': {'GLAMR_NET_SKINNY': '0'},                          # wgmma NT=32 at M <= 128, NT=128 above; FP32 tile everywhere
+    'nt32': {'GLAMR_NET_SKINNY': '0', 'GLAMR_TC_NTILE': '32'},
+    'nt128': {'GLAMR_NET_SKINNY': '0', 'GLAMR_TC_NTILE': '128'},
+    'wimg': {'GLAMR_NET_SKINNY': '0', 'GLAMR_NET_WIMG': '1'},     # pre-split weight image by bulk copy, NT=32 and 128
+}
+
+
+@pytest.mark.gpu
+@pytest.mark.parametrize('variant', list(LINEAR_VARIANTS))
+def test_linear_layers_match_float64(variant):
+    """every dispatch variant of the prior's Linear at shapes across every tile edge; Y is NaN before each call"""
+    res = _child('linear', LINEAR_VARIANTS[variant])
+    print(variant, res)
+    for k, v in res.items():
+        assert v <= 1.0, f'{variant} {k}: worst |y - y64| / bound = {v}'
+
+
+@pytest.mark.gpu
+def test_linear_weight_rewritten_in_place_is_not_served_stale():
+    """GLAMR_NET_WIMG=1: the weight image of a caller's buffer must not outlive the call"""
+    res = _child('stale', {'GLAMR_NET_SKINNY': '0', 'GLAMR_NET_WIMG': '1'})
+    print(res)
+    for k, v in res.items():
+        assert v <= 1.0, f'{k}: worst |y - y64| / bound = {v}'
+
+
+@pytest.mark.gpu
+def test_weight_images_belong_to_their_net():
+    """GLAMR_NET_WIMG=1: destroying one net leaves another net's images (and results) intact"""
+    res = _child('images', {'GLAMR_NET_SKINNY': '0', 'GLAMR_NET_WIMG': '1'})
+    print(res)
+    for k, v in res.items():
+        assert v <= 1.0, f'{k}: worst |o - o64| / bound = {v}'
+
+
+@pytest.mark.gpu
+def test_infiller_window_matches_float64():
+    """one window at B across the skinny / tile boundary of its 50 B, 30 B and 2 B-row GEMMs, five key masks, three eps modes"""
+    res = run_window_cases(window_cases())
+    print(max(res.values()), res)
+    for k, v in res.items():
+        assert v <= 1.0, f'{k}: worst |o - o64| / bound = {v}'
+
+
+@pytest.fixture(scope='module')
+def cuda_prior(smpl_assets):
+    from glamr_b200.motion_traj import MotionTrajJointModel
+    from glamr_b200.smpl import SMPL
+    return MotionTrajJointModel(None, torch.device(DEV), None, smpl=SMPL(smpl_assets, device=DEV), states=states())
+
+
+SWEEP_CASES = [  # B, T, gaps (sequence, first frame, end), 3-D latents
+    (1, 11, [], False), (3, 39, [(1, 12, 30)], True), (1, 40, [(0, 35, 40)], False), (3, 41, [(2, 10, 41)], False),
+    (1, 50, [(0, 5, 45)], True), (3, 70, [(0, 38, 62)], False), (64, 71, [(5, 30, 71)], True), (3, 100, [(0, 40, 75), (1, 65, 100)], False),
+    (1, 1100, [(0, 100, 170), (0, 525, 700)], False)]
+
+
+@pytest.mark.gpu
+@pytest.mark.parametrize('B,T,gaps,lat3', SWEEP_CASES, ids=[f'{c[0]}x{c[1]}' for c in SWEEP_CASES])
+def test_infiller_sweep_matches_float64(B, T, gaps, lat3, cuda_prior):
+    """the autoregressive window sweep: a single frame past the first 10, ragged last windows, gaps that cross window edges or
+    start inside a window's 10 past frames, and 2-D ([windows,128]) and 3-D ([B,windows,128]) latents"""
+    pose, mask, lat = infill_inputs(B, T, T + B, gaps)
+    nwin = lat.shape[0]
+    if lat3:
+        lat = torch.randn(nwin, B, 128, generator=torch.Generator().manual_seed(T))
+    batch = {'in_body_pose': pose.to(DEV), 'frame_mask': mask.to(DEV),
+             'in_motion_latent': (lat.transpose(0, 1) if lat3 else lat[:, 0]).contiguous().to(DEV)}
+    got = cuda_prior.mfiller.inference(batch)['infer_out_body_pose'][:, 0].transpose(0, 1)
+    o32 = infill_sweep(infiller(), pose, mask, lat)
+    m64 = infiller(torch.float64).to(DEV)
+    o64 = infill_sweep(m64, pose.to(DEV), mask.to(DEV), lat.to(DEV)).cpu()
+    r = worst(got, o64, block_bound(o32, o64, window_blocks(T), peak_floor(o64)))
+    print(f'sweep {B}x{T}: {r:.3g}')
+    assert r <= 1.0, f'worst |o - o64| / bound = {r}'
+
+
+TRAJ_CASES = [(1, 1), (2, 2), (4, 5), (1, 256), (2, 257), (4, 300), (1, 511), (2, 512), (1, 513), (2, 1025), (1, 1100)]
+
+
+@pytest.mark.gpu
+@pytest.mark.parametrize('B,T', TRAJ_CASES, ids=[f'{b}x{t}' for b, t in TRAJ_CASES])
+def test_trajectory_predictor_matches_float64(B, T):
+    """glamr_trajpred_forward on the same float32 joint positions as the oracle (no FK): local element-wise, trans and
+    orientation with the block bound; eps rows 1 / B / NULL and init_xy / init_heading given or NULL, rotating over the cases"""
+    from glamr_b200 import motion_traj as mt
+    lib = _lib()
+    i = TRAJ_CASES.index((B, T))
+    g = torch.Generator().manual_seed(T * 10 + B)
+    jp = torch.randn(T, B, 69, generator=g) * 0.3
+    emode = ('rows1', 'rowsB', 'null')[i % 3]
+    eps = None if emode == 'null' else torch.randn(1 if emode == 'rows1' else B, 128, generator=g)
+    ixy = torch.randn(B, 2, generator=g) if i % 2 else None
+    ih = torch.randn(B, generator=g) * 3 if i % 4 < 2 else None
+    net = mt._Net(states()[1], torch.device(DEV))
+    ws = torch.empty(int(lib.glamr_trajpred_workspace_floats(T, B)), device=DEV)
+    outs = [torch.full((T, B, n), float('nan'), device=DEV) for n in (11, 3, 3)]
+    dv = lambda x: None if x is None else x.to(DEV)
+    jp_d, eps_d, ixy_d, ih_d = dv(jp), dv(eps), dv(ixy), dv(ih)
+    _check(lib.glamr_trajpred_forward(net.h, T, B, jp_d.data_ptr(), _ptr(eps_d), 1 if emode == 'rows1' else B, _ptr(ixy_d), _ptr(ih_d),
+                                      *[o.data_ptr() for o in outs], ws.data_ptr(), ws.numel(), _stream()), 'trajpred')
+    e0 = torch.zeros(1, 128) if eps is None else eps
+    r32 = traj_forward(trajpred(), jp, e0, ixy, ih)
+    d64 = lambda x: None if x is None else x.double()
+    r64 = traj_forward(trajpred(torch.float64), jp.double(), e0.double(), d64(ixy), d64(ih))
+    b = traj_bounds(r32[0], r64[0], r32[1], r64[1], quat_rotmat(r32[2]), quat_rotmat(r64[2]))
+    rs = {'local': worst(outs[0], r64[0], b['local']), 'trans': worst(outs[1], r64[1], b['trans']),
+          'orient': worst(rodrigues(outs[2]), quat_rotmat(r64[2]), b['orient'])}
+    print(f'trajpred {B}x{T} eps {emode}:', rs)
+    for k, v in rs.items():
+        assert v <= 1.0, f'{k}: worst |o - o64| / bound = {v}'
+
+
+def codec_local(T, B, seed):
+    """seeded local trajectories whose headings accumulate to hundreds of radians"""
+    g = torch.Generator().manual_seed(seed)
+    loc = torch.randn(T, B, 11, generator=g) * 0.05
+    loc[..., 2] += 0.9
+    loc[..., 3:9] = torch.randn(T, B, 6, generator=g)
+    dh = 0.4 + 0.3 * torch.randn(T, B, generator=g)
+    loc[..., 9], loc[..., 10] = torch.cos(dh), torch.sin(dh)
+    return loc
+
+
+@pytest.mark.gpu
+@pytest.mark.parametrize('T', [511, 512, 513, 1024, 1025])
+@pytest.mark.parametrize('local_heading', [0, 1])
+def test_trajectory_codec_matches_float64(T, local_heading):
+    lib = _lib()
+    B = 2
+    loc = codec_local(T, B, T + local_heading)
+    trans = torch.full((T, B, 3), float('nan'), device=DEV)
+    q = torch.full((T, B, 4), float('nan'), device=DEV)
+    scratch = torch.empty(B * T * 3, device=DEV)
+    loc_d = loc.to(DEV)
+    _check(lib.glamr_traj_local2global(T, B, loc_d.data_ptr(), local_heading, trans.data_ptr(), q.data_ptr(), scratch.data_ptr(), _stream()),
+           'local2global')
+    t32, q32 = tc.local_to_global(loc, bool(local_heading))
+    t64, q64 = tc.local_to_global(loc.double(), bool(local_heading))
+    b = traj_bounds(None, loc.double(), t32, t64, quat_rotmat(q32), quat_rotmat(q64), bool(local_heading))
+    rs = {'trans': worst(trans, t64, b['trans']), 'orient': worst(quat_rotmat(q), quat_rotmat(q64), b['orient'])}
+    print(f'codec T {T} local_heading {local_heading}:', rs)
+    for k, v in rs.items():
+        assert v <= 1.0, f'{k}: worst |o - o64| / bound = {v}'
+
+
+def e2e_case(name):
+    if name == 'c3_64x120':
+        from helpers import c3_prior_inputs
+        return c3_prior_inputs()
+    pose, mask, lat = infill_inputs(2, 600, 600, gaps=[(0, 100, 260), (1, 280, 330), (1, 500, 600)])
+    g = torch.Generator().manual_seed(2)
+    return {'in_body_pose': pose, 'frame_mask': mask, 'in_motion_latent': lat[:, 0], 'in_traj_latent': torch.randn(1, 128, generator=g)}
+
+
+@pytest.mark.gpu
+@pytest.mark.parametrize('case', ['c3_64x120', 'gaps_2x600'])
+def test_prior_end_to_end_matches_float64(case, cuda_prior, smpl_assets):
+    """MotionTrajJointModel.inference against MotionTrajJoint in float64 (SMPL FK in float64 too), every row element-wise"""
+    from oracle.smpl import OracleSMPL
+    batch = e2e_case(case)
+    out = cuda_prior.inference({k: v.to(DEV) for k, v in batch.items()})
+    sm, st = states()
+    r32 = on.MotionTrajJoint(sm, st, OracleSMPL(smpl_assets)).inference(batch)
+    r64 = on.MotionTrajJoint(sm, st, OracleSMPL(smpl_assets, dtype=torch.float64), torch.float64).inference(batch)
+    T = batch['in_body_pose'].shape[1]
+    bt = lambda x: x[:, 0].transpose(0, 1).cpu()          # [B,1,T,F] -> [T,B,F]
+    pose64 = bt(r64['infer_out_body_pose'])
+    rs = {'pose': worst(bt(out['infer_out_body_pose']), pose64, block_bound(bt(r32['infer_out_body_pose']), pose64, window_blocks(T), peak_floor(pose64)))}
+    l32, l64 = r32['infer_out_local_traj_tp'][:, :, 0], r64['infer_out_local_traj_tp'][:, :, 0].cpu()
+    b = traj_bounds(l32, l64, bt(r32['infer_out_trans']), bt(r64['infer_out_trans']), rodrigues(bt(r32['infer_out_orient'])),
+                    rodrigues(bt(r64['infer_out_orient'])))
+    rs['local'] = worst(out['infer_out_local_traj_tp'][:, :, 0], l64, b['local'])
+    rs['trans'] = worst(bt(out['infer_out_trans']), bt(r64['infer_out_trans']), b['trans'])
+    rs['orient'] = worst(rodrigues(bt(out['infer_out_orient'])), rodrigues(bt(r64['infer_out_orient'])), b['orient'])
+    print(f'end to end {case}:', rs)
+    for k, v in rs.items():
+        assert v <= 1.0, f'{k}: worst |o - o64| / bound = {v}'
+
+
+@pytest.mark.gpu
+def test_graph_replay_is_bit_identical_to_eager(cuda_prior):
+    """_GraphCache(enabled=True) on both nets: replays (same inputs, then new inputs through the copy-in) equal eager runs"""
+    from glamr_b200.motion_traj import _GraphCache
+    mf, tp = cuda_prior.mfiller, cuda_prior.traj_predictor
+    saved = mf.graphs, tp.graphs
+    try:
+        for B, T in [(1, 100), (4, 71)]:
+            ins = []
+            for seed in (1, 2):
+                pose, mask, lat = infill_inputs(B, T, seed, gaps=[(0, 20, 45)])
+                ins.append({'in_body_pose': pose.to(DEV), 'frame_mask': mask.to(DEV), 'in_motion_latent': lat[:, 0].to(DEV),
+                            'in_traj_latent': torch.randn(1, 128, generator=torch.Generator().manual_seed(seed)).to(DEV)})
+            mf.graphs, tp.graphs = _GraphCache(enabled=False), _GraphCache(enabled=False)
+            eager = [(mf.inference(x)['infer_out_body_pose'], tp.inference({'in_body_pose': x['in_body_pose'], 'in_traj_latent': x['in_traj_latent']}))
+                     for x in ins]
+            mf.graphs, tp.graphs = _GraphCache(enabled=True), _GraphCache(enabled=True)
+            for k, x in enumerate([ins[0], ins[0], ins[1]]):     # warm-up + capture, replay, replay with new inputs
+                body = mf.inference(x)['infer_out_body_pose']
+                tr = tp.inference({'in_body_pose': x['in_body_pose'], 'in_traj_latent': x['in_traj_latent']})
+                e_body, e_tr = eager[0 if k < 2 else 1]
+                assert torch.equal(body, e_body), (B, T, k)
+                for key in ('infer_out_local_traj_tp', 'infer_out_trans', 'infer_out_orient'):
+                    assert torch.equal(tr[key], e_tr[key]), (B, T, k, key)
+            assert all(e['graph'] is not None for e in list(mf.graphs.entries.values()) + list(tp.graphs.entries.values()))
+    finally:
+        mf.graphs, tp.graphs = saved
+
+
+if __name__ == '__main__':          # the variants that need their own process (dispatch switches in the environment)
+    torch.set_num_threads(max(1, min(8, os.cpu_count() or 1)))
+    fn = {'linear': run_linear_sweep, 'stale': run_stale_image, 'images': run_image_ownership}[sys.argv[1]]
+    print(json.dumps(fn()))
