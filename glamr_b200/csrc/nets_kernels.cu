@@ -6,6 +6,7 @@
 // shared memory) and the LSTM recurrence (W_hh resident in registers + shared memory for the whole sequence) are FP32
 // SIMT kernels.  Outputs match the reference's fp32 networks to <= 1e-4 (tests/golden/nets.npz).
 // Weights are addressed by their reference state-dict names so Lightning checkpoints map 1:1.
+#include <limits.h>
 #include <math.h>
 #include <stdlib.h>
 #include <string.h>
@@ -1035,21 +1036,15 @@ extern "C" int glamr_infiller_forward(const glamr_net* n, int T, int B, float* p
 
 extern "C" size_t glamr_trajpred_workspace_floats(int T, int B) { return (size_t)T * B * (512 + 256 + 2 * 512 + 256 + 384 + 512 + 256 + 64) + (size_t)B * 2048 + 65536; }
 
-// TrajPredVAE.inference (multi_step False, sample_num 1): joint positions -> local trajectory -> global trajectory.
-//   in_joint_pos [T,B,69]   eps [B or 1,128] or NULL   init_xy [B,2] / init_heading [B] or NULL
-//   out_local_traj [T,B,11]  out_trans [T,B,3]  out_orient_aa [T,B,3]
-extern "C" int glamr_trajpred_forward(const glamr_net* n, int T, int B, const float* in_joint_pos, const float* eps, int eps_rows,
-                                      const float* init_xy, const float* init_heading, float* out_local_traj, float* out_trans,
-                                      float* out_orient_aa, float* workspace, size_t workspace_floats, void* stream);
-
 extern "C" int glamr_traj_local2global(int T, int B, const float* local_traj, int local_heading, float* trans, float* orient_q,
                                        float* scratch, void* stream);
 
-extern "C" int glamr_trajpred_forward(const glamr_net* n, int T, int B, const float* in_joint_pos, const float* eps, int eps_rows,
-                                      const float* init_xy, const float* init_heading, float* out_local_traj, float* out_trans,
-                                      float* out_orient_aa, float* workspace, size_t workspace_floats, void* stream) {
-  if (!n || T <= 0 || B <= 0 || !in_joint_pos || !out_local_traj || !out_trans || !out_orient_aa || !workspace) return GLAMR_EINVAL;
-  cudaStream_t s = (cudaStream_t)stream;
+// The trajectory predictor's network for R independent rows of T frames (traj_pred_vae.py:72-92 context encoder, :281-297
+// prior + z, :298-333 decoder up to out_fc): in [T,R,69] -> raw [T,R,11], the decoder output before any frame-0 override.
+// eps [R or 1,128] (eps_rows = R or 1) or NULL (-> z = mu).  Scratch comes from A.  The single-pass and the windowed entry
+// points both run the network through here.
+static int trajpred_network(const glamr_net* n, int T, int R, const float* in, const float* eps, int eps_rows, float* raw, Arena& A,
+                            cudaStream_t s) {
   ScopedFp32Gemm fp32_only;
   int e = 0;
   const std::string ce = "context_encoder.", dd = "data_decoder.";
@@ -1071,21 +1066,18 @@ extern "C" int glamr_trajpred_forward(const glamr_net* n, int T, int B, const fl
   const float* dm1w = W(n, dd + "out_mlp.affine_layers.1.weight", 256 * 512, &e), * dm1b = W(n, dd + "out_mlp.affine_layers.1.bias", 256, &e);
   const float* ofw = W(n, dd + "out_fc.weight", 11 * 256, &e), * ofb = W(n, dd + "out_fc.bias", 11, &e);
   if (e) return GLAMR_EINVAL;
-  Arena A{workspace, workspace_floats, 0};
-  const int M = T * B;
+  const int M = T * R;
   float* h512 = A.take((size_t)M * 512);
   float* x = A.take((size_t)M * 256);
   float* xp = A.take((size_t)M * 2 * 512);
   float* y = A.take((size_t)M * 256);
   float* cat = A.take((size_t)M * 384);
-  float* hm = A.take((size_t)B * 256);
-  float* hp = A.take((size_t)B * 512);
-  float* hq = A.take((size_t)B * 256);
-  float* pz = A.take((size_t)B * 256);
-  float* z = A.take((size_t)B * 128);
-  float* oq = A.take((size_t)M * 4);
-  float* sc = A.take((size_t)M * 3);
-  if (!sc) return GLAMR_ENOSPACE;
+  float* hm = A.take((size_t)R * 256);
+  float* hp = A.take((size_t)R * 512);
+  float* hq = A.take((size_t)R * 256);
+  float* pz = A.take((size_t)R * 256);
+  float* z = A.take((size_t)R * 128);
+  if (!z) return GLAMR_ENOSPACE;
   int rc;
   static bool attr = false;
   const size_t lstm_smem = ((size_t)(LH - LREG) * LG + LH + LG) * sizeof(float);
@@ -1094,35 +1086,137 @@ extern "C" int glamr_trajpred_forward(const glamr_net* n, int T, int B, const fl
     attr = true;
   }
   // ---- context encoder (traj_pred_vae.py:72-92)
-  if ((rc = gemm(s, M, 512, 69, in_joint_pos, 69, im0w, im0b, nullptr, h512, 512, 1))) return rc;
+  if ((rc = gemm(s, M, 512, 69, in, 69, im0w, im0b, nullptr, h512, 512, 1))) return rc;
   if ((rc = gemm(s, M, 256, 512, h512, 512, im1w, im1b, nullptr, x, 256, 1))) return rc;
   for (int l = 0; l < 2; ++l) {
     for (int d = 0; d < 2; ++d)   // xproj[t][b][d][:] = W_ih x + b_ih + b_hh
       if ((rc = gemm(s, M, 512, 256, x, 256, wih[l][d], bih[l][d], bhh[l][d], xp + d * 512, 1024, 0))) return rc;
-    lstm_recurrence_kernel<<<dim3(B, 2), LG, lstm_smem, s>>>(T, B, xp, whh[l][0], whh[l][1], y);
+    lstm_recurrence_kernel<<<dim3(R, 2), LG, lstm_smem, s>>>(T, R, xp, whh[l][0], whh[l][1], y);
     GLAMR_LAUNCH_CHECK();
     float* tmp = x; x = y; y = tmp;
   }
   if ((rc = gemm(s, M, 512, 256, x, 256, cm0w, cm0b, nullptr, h512, 512, 1))) return rc;
   if ((rc = gemm(s, M, 256, 512, h512, 512, cm1w, cm1b, nullptr, y, 256, 1))) return rc;      // y = context
   // ---- prior + z (:281-297)
-  mean_time_kernel<<<(B * 256 + 127) / 128, 128, 0, s>>>(T, B, 256, y, hm);
+  mean_time_kernel<<<(R * 256 + 127) / 128, 128, 0, s>>>(T, R, 256, y, hm);
   GLAMR_LAUNCH_CHECK();
-  if ((rc = gemm(s, B, 512, 256, hm, 256, pm0w, pm0b, nullptr, hp, 512, 1))) return rc;
-  if ((rc = gemm(s, B, 256, 512, hp, 512, pm1w, pm1b, nullptr, hq, 256, 1))) return rc;
-  if ((rc = gemm(s, B, 256, 256, hq, 256, pzw, pzb, nullptr, pz, 256, 0))) return rc;
-  sample_z_kernel<<<(B * 128 + 127) / 128, 128, 0, s>>>(B, 128, pz, 256, pz + 128, 256, eps, eps_rows == 1 ? 0 : 128, z);
+  if ((rc = gemm(s, R, 512, 256, hm, 256, pm0w, pm0b, nullptr, hp, 512, 1))) return rc;
+  if ((rc = gemm(s, R, 256, 512, hp, 512, pm1w, pm1b, nullptr, hq, 256, 1))) return rc;
+  if ((rc = gemm(s, R, 256, 256, hq, 256, pzw, pzb, nullptr, pz, 256, 0))) return rc;
+  sample_z_kernel<<<(R * 128 + 127) / 128, 128, 0, s>>>(R, 128, pz, 256, pz + 128, 256, eps, eps_rows == 1 ? 0 : 128, z);
   GLAMR_LAUNCH_CHECK();
   // ---- decoder (:298-333)
-  concat_z_kernel<<<256, 256, 0, s>>>(M, B, 128, 256, z, y, cat);
+  concat_z_kernel<<<256, 256, 0, s>>>(M, R, 128, 256, z, y, cat);
   GLAMR_LAUNCH_CHECK();
   if ((rc = gemm(s, M, 512, 384, cat, 384, dm0w, dm0b, nullptr, h512, 512, 1))) return rc;
   if ((rc = gemm(s, M, 256, 512, h512, 512, dm1w, dm1b, nullptr, x, 256, 1))) return rc;
-  if ((rc = gemm(s, M, 11, 256, x, 256, ofw, ofb, nullptr, out_local_traj, 11, 0))) return rc;
+  return gemm(s, M, 11, 256, x, 256, ofw, ofb, nullptr, raw, 11, 0);
+}
+
+// TrajPredVAE.inference (multi_step False, sample_num 1): joint positions -> local trajectory -> global trajectory.
+//   in_joint_pos [T,B,69]   eps [B or 1,128] or NULL   init_xy [B,2] / init_heading [B] or NULL
+//   out_local_traj [T,B,11]  out_trans [T,B,3]  out_orient_aa [T,B,3]
+extern "C" int glamr_trajpred_forward(const glamr_net* n, int T, int B, const float* in_joint_pos, const float* eps, int eps_rows,
+                                      const float* init_xy, const float* init_heading, float* out_local_traj, float* out_trans,
+                                      float* out_orient_aa, float* workspace, size_t workspace_floats, void* stream) {
+  if (!n || T <= 0 || B <= 0 || !in_joint_pos || !out_local_traj || !out_trans || !out_orient_aa || !workspace) return GLAMR_EINVAL;
+  cudaStream_t s = (cudaStream_t)stream;
+  Arena A{workspace, workspace_floats, 0};
+  const int M = T * B;
+  int rc;
+  if ((rc = trajpred_network(n, T, B, in_joint_pos, eps, eps_rows, out_local_traj, A, s))) return rc;
+  float* oq = A.take((size_t)M * 4);
+  float* sc = A.take((size_t)M * 3);
+  if (!sc) return GLAMR_ENOSPACE;
   traj_first_frame_kernel<<<(B + 127) / 128, 128, 0, s>>>(B, out_local_traj, init_xy, init_heading);
   GLAMR_LAUNCH_CHECK();
   if ((rc = glamr_traj_local2global(T, B, out_local_traj, 1, out_trans, oq, sc, stream))) return rc;
   quat_rows_to_aa_kernel<<<(M + 127) / 128, 128, 0, s>>>(M, oq, out_orient_aa);
+  GLAMR_LAUNCH_CHECK();
+  return GLAMR_OK;
+}
+
+// ------------------------------------------------------------------------------------------------ windowed trajectory prediction
+// TrajPredVAE.inference_multi_step (traj_pred_vae.py:484-520, sample_num 1): the track is cut into C = ceil(T / W) windows of W
+// frames, the last one zero-padded in joint-position space, and every window runs the network on its own.  A window reads no
+// other window's output (the stitch below rewrites only frame 0's heading vector, from columns 3:9 that nothing rewrites), so
+// all of them go through the network as R = C * B rows of one batch.  Rows are window-major: row c * B + b is window c of
+// sequence b, which makes eps [C,B,128] the rows' eps as laid out.
+
+// [T,B,69] -> [W,C*B,69]: window c, frame t of sequence b = global frame c W + t, zero past T
+__global__ void traj_window_gather_kernel(int T, int B, int W, int C, const float* __restrict__ jp, float* __restrict__ win) {
+  const size_t total = (size_t)W * C * B * 69;
+  for (size_t e = (size_t)blockIdx.x * blockDim.x + threadIdx.x; e < total; e += (size_t)gridDim.x * blockDim.x) {
+    const size_t row = e / 69;                       // t * (C B) + c B + b
+    const int k = (int)(e - row * 69);
+    const int t = (int)(row / ((size_t)C * B));
+    const int cb = (int)(row - (size_t)t * C * B);
+    const int c = cb / B, b = cb - c * B;
+    const int tg = c * W + t;
+    win[e] = tg < T ? jp[((size_t)tg * B + b) * 69 + k] : 0.0f;
+  }
+}
+
+// raw [W,C*B,11] -> local [T,B,11] (get_res_from_cur_data, :500-506).  Window 0 contributes its overridden output (frame 0:
+// xy = 0, heading vector (0, 1): no init_xy / init_heading reaches a window, :319-327); window c >= 1 its raw output with
+// frame 0's heading vector replaced by heading_to_vec(get_heading(rot6d_to_quat(.))) of global frame c W - 1's columns 3:9.
+// Padded frames are dropped.  One thread per output row.
+__global__ void traj_window_stitch_kernel(int T, int B, int W, int C, const float* __restrict__ raw, float* __restrict__ local) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= T * B) return;
+  const int t = i / B, b = i - t * B;
+  const int c = t / W, tw = t - c * W;
+  const float* src = raw + ((size_t)tw * C * B + (size_t)c * B + b) * 11;
+  float l[11];
+#pragma unroll
+  for (int k = 0; k < 11; ++k) l[k] = src[k];
+  if (tw == 0) {
+    if (c == 0) {
+      l[0] = 0.0f; l[1] = 0.0f; l[9] = 0.0f; l[10] = 1.0f;
+    } else {
+      const float* prev = raw + ((size_t)(W - 1) * C * B + (size_t)(c - 1) * B + b) * 11;
+      float R[9], q[4];
+      rot6d_to_rotmat(prev + 3, R);
+      rotmat_to_quat(R, q);
+      const float h = 2.0f * safe_atan2(q[3], q[0]);
+      l[9] = cosf(h); l[10] = sinf(h);
+    }
+  }
+  float* dst = local + (size_t)i * 11;
+#pragma unroll
+  for (int k = 0; k < 11; ++k) dst[k] = l[k];
+}
+
+extern "C" size_t glamr_trajpred_windows_workspace_floats(int T, int B, int W) {
+  if (T <= 0 || B <= 0 || W <= 0) return 0;
+  const size_t C = ((size_t)T + W - 1) / W, R = C * B;
+  return (size_t)W * R * (69 + 11) + (size_t)T * B * 7 + 4 * 64 + glamr_trajpred_workspace_floats(W, (int)R);
+}
+
+//   in_joint_pos [T,B,69]   eps [C,B,128] or NULL (z = mu)   out_local_traj [T,B,11]  out_trans [T,B,3]  out_orient_aa [T,B,3]
+extern "C" int glamr_trajpred_windows_forward(const glamr_net* n, int T, int B, int W, const float* in_joint_pos, const float* eps,
+                                              float* out_local_traj, float* out_trans, float* out_orient_aa, float* workspace,
+                                              size_t workspace_floats, void* stream) {
+  if (!n || T <= 0 || B <= 0 || W <= 0 || !in_joint_pos || !out_local_traj || !out_trans || !out_orient_aa || !workspace) return GLAMR_EINVAL;
+  const int C = (T + W - 1) / W;
+  if ((size_t)C * B > (size_t)INT_MAX / W) return GLAMR_EINVAL;
+  const int R = C * B;
+  if (workspace_floats < glamr_trajpred_windows_workspace_floats(T, B, W)) return GLAMR_ENOSPACE;
+  cudaStream_t s = (cudaStream_t)stream;
+  Arena A{workspace, workspace_floats, 0};
+  float* win = A.take((size_t)W * R * 69);
+  float* raw = A.take((size_t)W * R * 11);
+  float* oq = A.take((size_t)T * B * 4);
+  float* sc = A.take((size_t)T * B * 3);
+  if (!sc) return GLAMR_ENOSPACE;
+  traj_window_gather_kernel<<<1024, 256, 0, s>>>(T, B, W, C, in_joint_pos, win);
+  GLAMR_LAUNCH_CHECK();
+  int rc;
+  if ((rc = trajpred_network(n, W, R, win, eps, R, raw, A, s))) return rc;
+  traj_window_stitch_kernel<<<(T * B + 127) / 128, 128, 0, s>>>(T, B, W, C, raw, out_local_traj);
+  GLAMR_LAUNCH_CHECK();
+  if ((rc = glamr_traj_local2global(T, B, out_local_traj, 1, out_trans, oq, sc, stream))) return rc;
+  quat_rows_to_aa_kernel<<<(T * B + 127) / 128, 128, 0, s>>>(T * B, oq, out_orient_aa);
   GLAMR_LAUNCH_CHECK();
   return GLAMR_OK;
 }

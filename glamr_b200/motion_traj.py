@@ -4,7 +4,8 @@
 
 The networks run in ``glamr_infiller_forward`` (the autoregressive sweep of 50-frame windows of
 MotionInfillerVAE.inference_multi_step, motion_infiller_vae.py:618-632, batched over ALL sequences instead of the
-reference's batch of one) and ``glamr_trajpred_forward`` (glamr_b200/csrc/nets_kernels.cu); this module runs SMPL FK for the joint-position features and reshapes the outputs into the reference's
+reference's batch of one) and ``glamr_trajpred_forward`` / ``glamr_trajpred_windows_forward`` (single pass / every window of
+multi_step_trajpred in one batch; glamr_b200/csrc/nets_kernels.cu); this module runs SMPL FK for the joint-position features and reshapes the outputs into the reference's
 dict layout.  Weights come from the reference's Lightning checkpoints (state_dict names are kept) or from an explicit
 state dict; there is no CPU fallback.
 """
@@ -18,6 +19,7 @@ import torch
 from . import lib as L
 
 PAST, CUR, FUT, NZ = 10, 30, 10, 128
+TRAJ_WINDOW = 100        # seq_len of traj_pred/cfg/traj_pred_demo.yml: the window of multi-step trajectory prediction
 PRIOR_GRAPH_DEFAULT = '0'
 WINDOW = PAST + CUR + FUT
 
@@ -35,6 +37,9 @@ def _declare(lib):
                                                                                                              ctypes.c_void_p, ctypes.c_size_t, ctypes.c_void_p]
     lib.glamr_trajpred_forward.argtypes = [ctypes.c_void_p, ctypes.c_int, ctypes.c_int, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int] + \
         [ctypes.c_void_p] * 6 + [ctypes.c_size_t, ctypes.c_void_p]
+    lib.glamr_trajpred_windows_workspace_floats.restype = ctypes.c_size_t
+    lib.glamr_trajpred_windows_workspace_floats.argtypes = [ctypes.c_int] * 3
+    lib.glamr_trajpred_windows_forward.argtypes = [ctypes.c_void_p] + [ctypes.c_int] * 3 + [ctypes.c_void_p] * 6 + [ctypes.c_size_t, ctypes.c_void_p]
     lib._nets_declared = True
 
 
@@ -168,13 +173,15 @@ class MotionInfillerVAE:
 
 
 class TrajPredVAE:
-    """inference surface of traj_pred/models/traj_pred_vae.py:341-548 (6d local orientation, joint-position input)"""
+    """inference surface of traj_pred/models/traj_pred_vae.py:341-548 (6d local orientation, joint-position input).
+    seq_len: the window of multi-step inference (the predictor config's seq_len)."""
     model_type = 'joint'
     in_joint_pos_only = False
 
-    def __init__(self, state, device, smpl):
+    def __init__(self, state, device, smpl, seq_len=TRAJ_WINDOW):
         self.net = _Net(state, device)
         self.device, self.smpl, self.nz = self.net.device, smpl, NZ
+        self.seq_len = int(seq_len)
         self.graphs = _GraphCache()
 
     def get_latent(self, seq_len):
@@ -187,19 +194,39 @@ class TrajPredVAE:
         joints = self.smpl.get_joints(global_orient=z3, body_pose=flat, root_trans=z3)
         return joints[:, 1:, :].reshape(body_pose.shape[:-1] + (69,))
 
+    def num_windows(self, seq_len):
+        return -(-int(seq_len) // self.seq_len)
+
     def inference(self, batch, sample_num=1, recon=False, recon_only=False, multi_step=False):
-        if recon or recon_only or multi_step or sample_num != 1:
-            raise NotImplementedError('only single-pass sampling (multi_step_trajpred=false, sample_num=1) is implemented on CUDA')
+        """Single pass (multi_step False): one network pass over the whole track; `in_traj_latent` [1 or B,128], `init_xy`
+        [B,2] and `init_heading` [B] are used when given.
+
+        Multi-step (traj_pred_vae.py:484-520): the track is cut into ceil(T / seq_len) windows, the last one zero-padded, each
+        window draws its own z and the windows are stitched with the heading hand-over of the reference.  As in the
+        reference, `in_traj_latent`, `init_xy` and `init_heading` do not reach the windows and are ignored.  The windows' eps
+        come from `in_traj_window_latent` [windows, B, 128] when given, else from torch.randn on the device."""
+        if recon or recon_only or sample_num != 1:
+            raise NotImplementedError('only sampling with sample_num=1 is implemented on CUDA (no reconstruction mode)')
         dev = self.device
         body = batch['in_body_pose'].to(dev, torch.float32).contiguous()           # [B,T,69]
         B, T = body.shape[:2]
         dv = lambda k: batch[k].to(dev, torch.float32).contiguous() if k in batch and batch[k] is not None else None
-        latent, ixy, ih = dv('in_traj_latent'), dv('init_xy'), dv('init_heading')
-        self.net.workspace(self.net.lib.glamr_trajpred_workspace_floats(T, B))
         self.smpl._workspace(B * T, fk_only=True)
-        key = ('traj', B, T, None if latent is None else tuple(latent.shape), ixy is not None, ih is not None)
-        with torch.cuda.device(dev):
-            local, trans, orient = self.graphs.run(key, self._forward, (body, latent, ixy, ih))
+        if multi_step:
+            wlat = dv('in_traj_window_latent')
+            C = self.num_windows(T)
+            if wlat is not None and tuple(wlat.shape) != (C, B, NZ):
+                raise ValueError(f'in_traj_window_latent: {C} windows of {B} sequences need shape {(C, B, NZ)}, got {tuple(wlat.shape)}')
+            self.net.workspace(self.net.lib.glamr_trajpred_windows_workspace_floats(T, B, self.seq_len))
+            key = ('traj_windows', self.seq_len, B, T, wlat is not None)
+            with torch.cuda.device(dev):
+                local, trans, orient = self.graphs.run(key, self._forward_windows, (body, wlat))
+        else:
+            latent, ixy, ih = dv('in_traj_latent'), dv('init_xy'), dv('init_heading')
+            self.net.workspace(self.net.lib.glamr_trajpred_workspace_floats(T, B))
+            key = ('traj', B, T, None if latent is None else tuple(latent.shape), ixy is not None, ih is not None)
+            with torch.cuda.device(dev):
+                local, trans, orient = self.graphs.run(key, self._forward, (body, latent, ixy, ih))
         out = {'infer_out_local_traj_tp': local.view(T, B, 1, 11), 'infer_out_trans_tp': trans.view(T, B, 1, 3),
                'infer_out_orient_tp': orient.view(T, B, 1, 3)}
         out['infer_out_orient'] = out['infer_out_orient_tp'].permute(1, 2, 0, 3).contiguous()
@@ -224,6 +251,22 @@ class TrajPredVAE:
         L.check(lib.glamr_trajpred_forward(self.net.h, T, B, jp.data_ptr(), eps.data_ptr(), rows, None if ixy is None else ixy.data_ptr(),
                                            None if ih is None else ih.data_ptr(), local.data_ptr(), trans.data_ptr(), orient.data_ptr(),
                                            ws.data_ptr(), ws.numel(), torch.cuda.current_stream().cuda_stream), 'glamr_trajpred_forward')
+        return local, trans, orient
+
+    def _forward_windows(self, body, wlat):
+        """joint-position features (SMPL FK on the whole track) + every window of every sequence in one library call"""
+        dev = self.device
+        B, T = body.shape[:2]
+        jp = self.get_joint_pos(body).transpose(0, 1).contiguous()                # [T,B,69]
+        lib = self.net.lib
+        ws = self.net.workspace(lib.glamr_trajpred_windows_workspace_floats(T, B, self.seq_len))
+        local = torch.empty((T, B, 11), dtype=torch.float32, device=dev)
+        trans = torch.empty((T, B, 3), dtype=torch.float32, device=dev)
+        orient = torch.empty((T, B, 3), dtype=torch.float32, device=dev)
+        eps = wlat if wlat is not None else torch.randn((self.num_windows(T), B, NZ), device=dev)
+        L.check(lib.glamr_trajpred_windows_forward(self.net.h, T, B, self.seq_len, jp.data_ptr(), eps.data_ptr(), local.data_ptr(),
+                                                   trans.data_ptr(), orient.data_ptr(), ws.data_ptr(), ws.numel(),
+                                                   torch.cuda.current_stream().cuda_stream), 'glamr_trajpred_windows_forward')
         return local, trans, orient
 
 
@@ -273,7 +316,9 @@ _RESULTS_ROOT = {'motion_infiller': 'results/motion_filler', 'traj_pred': 'resul
 class MTConfig:
     """motion_infiller/utils/config_motion_traj.py:7-45: the joint model's YAML (cwd-relative glob like the reference; the
     shipped joint_motion_traj_demo.yml is built in) and the checkpoint directories of the two networks it names
-    (motion_infiller/utils/config.py:16-26, traj_pred/utils/config.py:16-26)."""
+    (motion_infiller/utils/config.py:16-26, traj_pred/utils/config.py:16-26).  `trajpred_seq_len` is the window of multi-step
+    trajectory prediction: the `seq_len` of the predictor's config (traj_pred/cfg/**/<trajpred_cfg>.yml), TRAJ_WINDOW when the
+    file is not found or does not set it."""
 
     def __init__(self, cfg_id):
         import yaml
@@ -290,14 +335,19 @@ class MTConfig:
         self.seed = y.get('seed', 1)
         self.multi_step_mfiller = y.get('multi_step_mfiller', True)
         self.multi_step_trajpred = y.get('multi_step_trajpred', True)
+        tp_cfg = self.network_cfg('traj_pred', self.model_specs.get('trajpred_cfg', _JOINT_DEMO_YML['model_specs']['trajpred_cfg']))
+        self.trajpred_seq_len = int(tp_cfg.get('seq_len', TRAJ_WINDOW))
+
+    @staticmethod
+    def network_cfg(package, net_cfg_id):
+        """the YAML of a network config (`<package>/cfg/**/<id>.yml`, cwd-relative like the reference) or {} if not found"""
+        import yaml
+        files = glob.glob(f'{package}/cfg/**/{net_cfg_id}.yml', recursive=True)
+        return (yaml.safe_load(open(files[0])) or {}) if len(files) == 1 else {}
 
     @staticmethod
     def network_cfg_dir(package, net_cfg_id):
-        import yaml
-        files = glob.glob(f'{package}/cfg/**/{net_cfg_id}.yml', recursive=True)
-        root = _RESULTS_ROOT[package]
-        if len(files) == 1:
-            root = os.path.expanduser(yaml.safe_load(open(files[0])).get('results_root_dir', root))
+        root = os.path.expanduser(MTConfig.network_cfg(package, net_cfg_id).get('results_root_dir', _RESULTS_ROOT[package]))
         return f'{root}/{net_cfg_id}'
 
 
@@ -305,16 +355,15 @@ class MotionTrajJointModel:
     supports_person_batch = True     # inference() accepts [B, T, 69] with B > 1 (GlobalReconOptimizer.infer_motion_traj_all)
 
     def __init__(self, cfg=None, device=torch.device('cuda'), log=None, smpl=None, states=None):
-        """cfg: config id / object of the joint model (only its checkpoint locations are used).  states: optional
-        (infiller_state_dict, trajpred_state_dict); otherwise the reference's checkpoint files are loaded."""
+        """cfg: config id / object of the joint model (its checkpoint locations, `multi_step_trajpred` and
+        `trajpred_seq_len`; None = the shipped joint config's settings).  states: optional (infiller_state_dict,
+        trajpred_state_dict); otherwise the reference's checkpoint files are loaded."""
         self.device, self.log = L.require_cuda(device), log
         if isinstance(cfg, str):
             cfg = MTConfig(cfg)
         self.cfg = cfg
         self.multi_step_mfiller = getattr(cfg, 'multi_step_mfiller', True)
         self.multi_step_trajpred = getattr(cfg, 'multi_step_trajpred', False)
-        if self.multi_step_trajpred:
-            raise NotImplementedError('multi_step_trajpred: chunked trajectory prediction is not implemented on CUDA (the shipped joint config disables it)')
         if smpl is None:
             from .smpl import SMPL
             smpl = SMPL(device=self.device)
@@ -329,7 +378,7 @@ class MotionTrajJointModel:
                     log.info(f'loading {package} from check point {path}')
                 states.append(load_lightning_state_dict(path))
         self.mfiller = MotionInfillerVAE(states[0], self.device)
-        self.traj_predictor = TrajPredVAE(states[1], self.device, self.smpl)
+        self.traj_predictor = TrajPredVAE(states[1], self.device, self.smpl, getattr(cfg, 'trajpred_seq_len', TRAJ_WINDOW))
 
     def get_motion_latent(self, seq_len):
         return self.mfiller.get_latent(seq_len)
@@ -338,16 +387,18 @@ class MotionTrajJointModel:
         return self.traj_predictor.get_latent(seq_len)
 
     def inference(self, batch, sample_num=1, recon=False):
-        """motion_traj_joint_model.py:141-145 (+ pred_trajectory :73-133, 'infer' mode)"""
+        """motion_traj_joint_model.py:141-145 (+ pred_trajectory :73-133, 'infer' mode).  With multi_step_trajpred the
+        trajectory's window latents come from `in_traj_window_latent` [windows, B * sample_num, 128] when given."""
         if recon:
             raise NotImplementedError('recon mode needs the posterior encoders (training-side, out of scope)')
         data = self.mfiller.inference(batch, sample_num, recon=False, multi_step=True)
         motion = data['infer_out_body_pose']                                        # [B,S,T,69]
         B, S, T = motion.shape[:3]
         tb = {'in_body_pose': motion.reshape(B * S, T, 69)}
-        if 'in_traj_latent' in data:
-            tb['in_traj_latent'] = data['in_traj_latent']
-        out = self.traj_predictor.inference(tb, sample_num=1)
+        for k in ('in_traj_latent', 'in_traj_window_latent'):
+            if k in data:
+                tb[k] = data[k]
+        out = self.traj_predictor.inference(tb, sample_num=1, multi_step=self.multi_step_trajpred)
         data['infer_out_pose'] = out['infer_out_pose'].view(B, S, T, 72)
         data['infer_out_trans'] = out['infer_out_trans'].view(B, S, T, 3)
         data['infer_out_orient'] = out['infer_out_orient'].view(B, S, T, 3)

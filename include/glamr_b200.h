@@ -131,6 +131,15 @@ int glamr_infiller_forward(const glamr_net_t* n, int T, int B, float* pose_io, c
 int glamr_trajpred_forward(const glamr_net_t* n, int T, int B, const float* in_joint_pos, const float* eps, int eps_rows,
                            const float* init_xy, const float* init_heading, float* out_local_traj, float* out_trans,
                            float* out_orient_aa, float* workspace, size_t workspace_floats, void* stream);
+/* Windowed prediction (traj_pred_vae.py:484-520, multi_step_trajpred): the track is cut into C = ceil(T/W) windows of W frames,
+ * the last one zero-padded, and all C*B windows run as rows of one batch.  Each window draws its own z; no init_xy /
+ * init_heading reaches a window.  The windows are stitched with the reference's heading hand-over at each window start.
+ *   in_joint_pos [T,B,69]   eps [C,B,128] or NULL (z = mu)   outputs as glamr_trajpred_forward
+ *   workspace >= glamr_trajpred_windows_workspace_floats(T, B, W) floats */
+size_t glamr_trajpred_windows_workspace_floats(int T, int B, int W);
+int glamr_trajpred_windows_forward(const glamr_net_t* n, int T, int B, int W, const float* in_joint_pos, const float* eps,
+                                   float* out_local_traj, float* out_trans, float* out_orient_aa, float* workspace,
+                                   size_t workspace_floats, void* stream);
 
 /* ------------------------------------------------------------------------------------------------------------
  * Global optimisation  --  stands behind GlobalReconOptimizer.forward / compute_loss / optimize_main
