@@ -29,12 +29,8 @@
 #endif
 
 // Which implementation runs when the environment does not say otherwise.  A path becomes the default only after its parity
-// tests passed on the GPU (GLAMR_ITER_PATH=fused|legacy, GLAMR_LBS_PATH=tc|simt select explicitly for A/B runs).
-#define GLAMR_DEFAULT_ITER_FUSED 0
+// tests passed on the GPU (GLAMR_LBS_PATH=tc|tcblend|simt and GLAMR_NET_WIMG=0|1 select explicitly for A/B runs).
 #define GLAMR_DEFAULT_LBS_TC 2        /* 2 = tensor-core blend + tensor-core skinning, 1 = tensor-core blend + SIMT skinning, 0 = FP32 SIMT kernel */
-#define GLAMR_DEFAULT_BLEND_EARLY 0    /* 1: pipelined blend at the top of the evaluation into a second v_posed buffer (GLAMR_BLEND_EARLY=1) */
-#define GLAMR_DEFAULT_BLEND_SPLIT 0    /* percent of the pipelined blend launched at the top of the evaluation (GLAMR_BLEND_SPLIT) */
-#define GLAMR_DEFAULT_SMEM_CARVEOUT 3   /* bit mask, see smem_carveout_mask() in smpl_kernels.cu */
 #define GLAMR_DEFAULT_NET_WIMG 0       /* prior-network GEMMs: weight operand as a pre-split image fetched by bulk TMA (GLAMR_NET_WIMG=1) */
 
 namespace glamr {

@@ -115,9 +115,8 @@ GLAMR_HD void traj_pre(const OptCtx& c, int p, int i) {
 #pragma unroll
   for (int k = 0; k < 11; ++k) c.sc.traj_local[(size_t)n * 11 + k] = tl[k];
 }
-// d_xy rotated by heading h (traj_utils.py:76-77).  traj_mid and forward_pose_kernel both call this, with the products and their
-// sums spelled out as fmaf: left to the compiler, the two call sites were contracted differently and root_trans_world.y of the
-// fused head came out one rounding away from the default one
+// d_xy rotated by heading h (traj_utils.py:76-77).  traj_mid and the host harness call this, with the products and their sums spelled
+// out as fmaf so that the contraction does not depend on the compiler or the call site
 GLAMR_HD void rotate_dxy(float h, float& x, float& y) {
   const float ct = cosf(h), st = sinf(h);
   const float rx = fmaf(x, ct, -(y * st)), ry = fmaf(x, st, y * ct);
@@ -150,7 +149,7 @@ GLAMR_HD bool traj_codec_frame(const OptCtx& c, const glamr_person_t& ps, int i)
 }
 // world pose of absolute frame t from its traj_local row `tl`, scanned heading and scanned xy (ignored for frames the codec does not
 // produce); writes orient/trans base + world of frame-person n, returns nothing else
-GLAMR_HD void traj_post_vals(const OptCtx& c, int p, int t, const float* tl, float heading, float x, float y, float* ow_out) {
+GLAMR_HD void traj_post_vals(const OptCtx& c, int p, int t, const float* tl, float heading, float x, float y) {
   const glamr_person_t& ps = c.pb.persons[p];
   const int T = c.pb.T;
   const int n = p * T + t;
@@ -205,7 +204,6 @@ GLAMR_HD void traj_post_vals(const OptCtx& c, int p, int t, const float* tl, flo
     c.sc.trans_base[(size_t)n * 3 + k] = tb[k];
     c.sc.orient_world[(size_t)n * 3 + k] = ow[k];
     c.sc.trans_world[(size_t)n * 3 + k] = tw[k];
-    if (ow_out) ow_out[k] = ow[k];
   }
 }
 GLAMR_HD void traj_post(const OptCtx& c, int p, int t) {
@@ -214,10 +212,10 @@ GLAMR_HD void traj_post(const OptCtx& c, int p, int t) {
   const int i = t - ps.start;
   float* tl = c.sc.traj_local + (size_t)n * 11;
   if (traj_codec_frame(c, ps, i)) {
-    traj_post_vals(c, p, t, tl, c.sc.heading[n], c.sc.xy[2 * (size_t)n], c.sc.xy[2 * (size_t)n + 1], nullptr);
+    traj_post_vals(c, p, t, tl, c.sc.heading[n], c.sc.xy[2 * (size_t)n], c.sc.xy[2 * (size_t)n + 1]);
   } else {
     for (int k = 0; k < 11; ++k) tl[k] = 0.0f;
-    traj_post_vals(c, p, t, tl, 0.0f, 0.0f, 0.0f, nullptr);
+    traj_post_vals(c, p, t, tl, 0.0f, 0.0f, 0.0f);
   }
 }
 

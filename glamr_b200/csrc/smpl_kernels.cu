@@ -366,8 +366,8 @@ extern "C" int glamr_exp_blend_phases(long long* out) {    // the per-CTA sums o
 #define BLEND_CLOCK_STORE() do { } while (0)
 #endif
 
-// mtile0 / mtiles: the 128-frame tiles of this launch (the optimiser may split the blend in two launches); half_last: the last of them
-// holds at most 64 frames
+// mtile0 / mtiles: the 128-frame tiles [mtile0, mtile0 + mtiles) of this launch (the host launches them all, from mtile0 = 0);
+// half_last: the last of them holds at most 64 frames
 __global__ void __launch_bounds__(kTcThreads, 1) lbs_blend_tc_kernel(SmplDev m, SmplWorkspace w, int mtile0, int mtiles, int half_last) {
   extern __shared__ __align__(128) unsigned char tc_raw[];
   __half* As = reinterpret_cast<__half*>(tc_raw);                                 // [stages][hi | lo][2][128][8]
@@ -858,29 +858,16 @@ int launch_pose_prep(const SmplDev& m, int n, const float* orient, const float* 
 // default they run with a small shared-memory split, and the GEMM kernel that follows each of them in its stream (2 x 96-101 KB per SM)
 // can only be placed on an SM after the small kernel's CTAs have drained and the SM has been re-configured.  Asking for the maximal
 // shared-memory split on the small SMPL kernels too removes that hand-over: 193.0 -> 157.4 us per iteration at 4 x 300 frame-persons
-// (no change at 1 x 300).  The optimiser's own small kernels lose more from the smaller L1 than they gain (bit 4: +6 us at 1 x 300).
-// GLAMR_SMEM_CARVEOUT bit mask: which kernels ask for the maximal shared-memory split (cudaFuncAttributePreferredSharedMemoryCarveout):
-// 1 = the two LBS GEMM kernels, 2 = the small SMPL kernels next to them, 4 = the optimiser's small kernels (globalopt_kernels.cu)
-int smem_carveout_mask() {
-  static int v = -1;
-  if (v < 0) {
-    const char* e = getenv("GLAMR_SMEM_CARVEOUT");
-    v = e ? atoi(e) : GLAMR_DEFAULT_SMEM_CARVEOUT;
-  }
-  return v;
-}
+// (no change at 1 x 300).  The optimiser's own small kernels lose more from the smaller L1 than they gain (+6 us at 1 x 300), so they
+// keep the default split.
 static int lbs_set_attrs() {
   static bool attrs = false;
   if (!attrs) {
     attrs = true;
-    if (smem_carveout_mask() & 1) {
-      GLAMR_CUDA_TRY(cudaFuncSetAttribute(lbs_blend_tc_kernel, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared));
-      GLAMR_CUDA_TRY(cudaFuncSetAttribute(lbs_skin_tc_kernel, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared));
-    }
-    if (smem_carveout_mask() & 2) {
-      GLAMR_CUDA_TRY(cudaFuncSetAttribute(blend_features_kernel, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared));
-      GLAMR_CUDA_TRY(cudaFuncSetAttribute(pose_prep_kernel, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared));
-    }
+    GLAMR_CUDA_TRY(cudaFuncSetAttribute(lbs_blend_tc_kernel, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared));
+    GLAMR_CUDA_TRY(cudaFuncSetAttribute(lbs_skin_tc_kernel, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared));
+    GLAMR_CUDA_TRY(cudaFuncSetAttribute(blend_features_kernel, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared));
+    GLAMR_CUDA_TRY(cudaFuncSetAttribute(pose_prep_kernel, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared));
     GLAMR_CUDA_TRY(cudaFuncSetAttribute(lbs_blend_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kTcSmemBytes));
     GLAMR_CUDA_TRY(cudaFuncSetAttribute(lbs_skin_kernel<4>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSkinSmemBytes));
     GLAMR_CUDA_TRY(cudaFuncSetAttribute(lbs_skin_kernel<0>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSkinSmemBytes));
@@ -897,16 +884,16 @@ static int device_sms() {
   }
   return sms;
 }
-// the blend GEMM over the 128-frame tiles [mt_begin, mt_end) of n frame-persons
-static int launch_blend_gemm(const SmplDev& m, int n, const SmplWorkspace& w, cudaStream_t s, int mt_begin, int mt_end, bool pdl) {
-  const int mtiles = mt_end - mt_begin;
-  const int half_last = (mt_end == (n + kTcM - 1) / kTcM && n - (mt_end - 1) * kTcM <= kTcM / 2) ? 1 : 0;
+// the blend GEMM over all 128-frame tiles of n frame-persons
+static int launch_blend_gemm(const SmplDev& m, int n, const SmplWorkspace& w, cudaStream_t s, bool pdl) {
+  const int mtiles = (n + kTcM - 1) / kTcM;
+  const int half_last = (n - (mtiles - 1) * kTcM <= kTcM / 2) ? 1 : 0;
   const dim3 grid(min(device_sms(), kTcNTiles * mtiles));
   if (pdl) {
-    GLAMR_CUDA_TRY(launch_pdl(4, lbs_blend_tc_kernel, grid, dim3(kTcThreads), kTcSmemBytes, s, m, w, mt_begin, mtiles, half_last));
+    GLAMR_CUDA_TRY(launch_pdl(4, lbs_blend_tc_kernel, grid, dim3(kTcThreads), kTcSmemBytes, s, m, w, 0, mtiles, half_last));
     return GLAMR_OK;
   }
-  lbs_blend_tc_kernel<<<grid, kTcThreads, kTcSmemBytes, s>>>(m, w, mt_begin, mtiles, half_last);
+  lbs_blend_tc_kernel<<<grid, kTcThreads, kTcSmemBytes, s>>>(m, w, 0, mtiles, half_last);
   GLAMR_LAUNCH_CHECK();
   return GLAMR_OK;
 }
@@ -921,19 +908,17 @@ static int launch_skin_tc(const SmplDev& m, int n, const SmplWorkspace& w, float
   return GLAMR_OK;
 }
 // blend features + blend GEMM for local frame-persons [0, n): v_posed (transposed) of the workspace
-// mt_begin / mt_end: the range of 128-frame tiles of the GEMM this call launches (mt_end < 0: all); features: also (re)build the A operand
-int launch_blend(const SmplDev& m, int n, const float* body_pose, const float* betas, const SmplWorkspace& w, cudaStream_t s, int mt_begin,
-                 int mt_end, bool features) {
+// features: (re)build the A operand; gemm: run the GEMM
+int launch_blend(const SmplDev& m, int n, const float* body_pose, const float* betas, const SmplWorkspace& w, cudaStream_t s, bool features,
+                 bool gemm) {
   if (n <= 0) return GLAMR_OK;
   int rc;
   if ((rc = lbs_set_attrs())) return rc;
-  const int mtiles = (n + kTcM - 1) / kTcM;
-  if (mt_end < 0 || mt_end > mtiles) mt_end = mtiles;
   if (features) {
     blend_features_kernel<<<(n + 3) / 4, 128, 0, s>>>(n, body_pose, betas, w);
     GLAMR_LAUNCH_CHECK();
   }
-  if (mt_end > mt_begin) return launch_blend_gemm(m, n, w, s, mt_begin, mt_end, false);
+  if (gemm) return launch_blend_gemm(m, n, w, s, false);
   return GLAMR_OK;
 }
 // skinning of local frame-persons [0, n) from the workspace's v_posed and A
@@ -970,9 +955,8 @@ int launch_lbs(const SmplDev& m, int n_begin, int n_end, const float* betas, con
     if (rc) return rc;
   }
   if (path >= 1 && m.tcB && w.tcA && n_begin == 0) {
-    const int mtiles = (n_end + kTcM - 1) / kTcM;
     int rc;
-    if ((rc = launch_blend_gemm(m, n_end, w, s, 0, mtiles, pdl))) return rc;
+    if ((rc = launch_blend_gemm(m, n_end, w, s, pdl))) return rc;
     if (w.vp_tiled) return launch_skin_tc(m, n_end, w, vertices, s, pdl);
     if (pdl) {
       if (m.K == 4) GLAMR_CUDA_TRY(launch_pdl(4, lbs_skin_kernel<4>, grid, dim3(kLbsThreads), kSkinSmemBytes, s, m, n_begin, n_end, w, vertices));

@@ -51,11 +51,9 @@ struct SmplWorkspace {
   int mpad;         // frames padded to a multiple of 128
   float* skB;       // [ceil(mpad/20)][hi | lo][6 joint groups][20 frames x 12][4]  the relative joint transforms as the B operand of the
                     //              tensor-core skinning (row = frame-in-tile * 12 + element of the 3x4, K = joint), tf32 hi / lo
-  float* vpT2;      // optimiser only: second v_posed buffer (same layout as vpT) or NULL.  The blend of evaluation i + 1 is launched while
-                    //              evaluation i still reads v_posed, so the two alternate: buffer = (step + flip_add) & 1 with the Adam step
-                    //              count read from device memory (*flip_src), which keeps one captured graph valid for every iteration
+  float* vpT2;      // always NULL, see vp_buffer()
   const double* flip_src;
-  int flip_add;     // 0: the buffer of the current step (skinning, in-order blend), 1: the buffer of the next step (pipelined blend)
+  int flip_add;
   int vp_tiled;     // 1: v_posed is stored frame-tiled for lbs_skin_tc_kernel: [ceil(mpad/20)][20736 cols][20 frames] (the 128 vertices x
                     //    20 frames of a skinning tile are one contiguous 30,720 B block = one bulk copy); 0: vpT as described above
 };
@@ -93,7 +91,9 @@ inline SmplWorkspace smpl_carve_workspace(void* base, int n, int S) {
 }
 
 #if defined(__CUDACC__)
-// the v_posed buffer this launch works on (see SmplWorkspace::vpT2)
+// The v_posed buffer of an LBS kernel: always w.vpT, since nothing sets vpT2.  The select stays because ptxas allocates
+// lbs_skin_tc_kernel differently without it (168 instead of 166 registers, two R2UR before every epilogue store), which cost
+// 1.2 us per optimiser iteration at 1 x 300 on an H100 80GB HBM3 (700 W); remove it together with a retune of that kernel.
 __device__ __forceinline__ float* vp_buffer(const SmplWorkspace& w) {
   if (!w.vpT2) return w.vpT;
   return ((((int)*w.flip_src) + w.flip_add) & 1) ? w.vpT2 : w.vpT;
@@ -254,10 +254,9 @@ int launch_pose_prep(const SmplDev& m, int n, const float* orient, const float* 
 int launch_lbs(const SmplDev& m, int n_begin, int n_end, const float* betas, const SmplWorkspace& w, float* vertices,
                cudaStream_t s, bool pdl = false);
 // tensor-core path in two halves (the optimiser pipelines them: the blend depends on body pose / betas only)
-int launch_blend(const SmplDev& m, int n, const float* body_pose, const float* betas, const SmplWorkspace& w, cudaStream_t s, int mt_begin = 0,
-                 int mt_end = -1, bool features = true);
+int launch_blend(const SmplDev& m, int n, const float* body_pose, const float* betas, const SmplWorkspace& w, cudaStream_t s,
+                 bool features = true, bool gemm = true);
 int launch_skin(const SmplDev& m, int n, const SmplWorkspace& w, float* vertices, cudaStream_t s);
-int smem_carveout_mask();                    // GLAMR_SMEM_CARVEOUT (see smpl_kernels.cu)
 int lbs_kernel_count(const SmplDev& m);      // kernels one launch_lbs call launches
 int launch_joints_finalize(const SmplDev& m, int n, int orig_joints, const float* root_trans, const float* root_scale,
                            const SmplWorkspace& w, float* joints, cudaStream_t s);

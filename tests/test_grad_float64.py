@@ -1,9 +1,9 @@
 """The optimiser's analytic gradients against float64 autograd, element by element.
 
 Every iteration of the optimiser is a hand-written backward (frame_residuals_kernel, camera_backward / scatter,
-traj_cam_backward_kernel with its three CTA-wide reverse prefix scans, or the fused residuals_backward_kernel) followed by
-Adam.  Here each gradient element is compared with torch autograd through the full-LBS oracle in float64 (g64), with the
-same autograd in float32 (g32) as the yardstick of what a legitimate float32 implementation deviates by:
+traj_cam_backward_kernel with its three CTA-wide reverse prefix scans) followed by Adam.  Here each gradient element is
+compared with torch autograd through the full-LBS oracle in float64 (g64), with the same autograd in float32 (g32) as the
+yardstick of what a legitimate float32 implementation deviates by:
 
     |g[e] - g64[e]|  <=  C_NOISE * D_V(b(e))  +  C_ULP * 2^-24 * |g64[e]|
     D_V(b) = max(max_{e in b} |g32[e] - g64[e]|,  FLOOR * max_V |g64|)
@@ -17,7 +17,7 @@ FLOOR: |g32 - g64| can vanish by coincidence in a block (e.g. a block whose floa
 the variable's peak is 16 float32 roundings of its largest element, below any per-frame term a kernel could lose and
 above the re-association noise of a float32 sum of a few dozen terms of that size.  C_NOISE = 4, C_ULP = 8: on one H100
 80GB HBM3 (700 W limit) the worst |cuda - g64| over every case, variable and check point was 0.58 of this bound
-(dynamic_p1_t1025, traj_local_rot), 0.37-0.58 per case, on the default and the fused path alike.  The prefix-sum variables
+(dynamic_p1_t1025, traj_local_rot), 0.37-0.58 per case.  The prefix-sum variables
 and the terms sit far lower (scanned variables <= 0.29, terms <= 0.09), their bounds being set by the floors below, which
 rest on the host emulator's sequential float32 scans.  GLAMR_GRAD_REPORT=<file> writes the worst |g - g64| of every case and
 variable next to its bound.  The CPU tests below show that a second
@@ -503,21 +503,11 @@ def test_bound_accepts_the_float32_reference_itself(emu):
 
 
 # ------------------------------------------------------------------------------------------------ GPU
-def _set_iter_path(path):
-    old = os.environ.get('GLAMR_ITER_PATH')
-    if path is None:
-        os.environ.pop('GLAMR_ITER_PATH', None)
-    else:
-        os.environ['GLAMR_ITER_PATH'] = path
-    return old
-
-
-def _make_model(cfg, assets, mt, path=None, rank_range=None):
-    """GlobalReconOptimizer on cuda:0; path: GLAMR_ITER_PATH while the handle is created; rank_range (rank, (n_begin, n_end)):
-    this instance evaluates only that frame-person range, as rank `rank` of a sharded run (world stays 1: no collective)"""
+def _make_model(cfg, assets, mt, rank_range=None):
+    """GlobalReconOptimizer on cuda:0; rank_range (rank, (n_begin, n_end)): this instance evaluates only that frame-person range,
+    as rank `rank` of a sharded run (world stays 1: no collective)"""
     from glamr_b200.recon import GlobalReconOptimizer
     model = GlobalReconOptimizer(copy.deepcopy(cfg), torch.device(DEV), None, smpl=assets, mt_model=mt)
-    model._iter_path = path
     if rank_range is not None:
         orig = model._attach
 
@@ -529,11 +519,7 @@ def _make_model(cfg, assets, mt, path=None, rank_range=None):
 
 
 def _init(model, in_dict):
-    old = _set_iter_path(model._iter_path)
-    try:
-        return model.init_data(copy.deepcopy(in_dict))
-    finally:
-        _set_iter_path(old)
+    return model.init_data(copy.deepcopy(in_dict))
 
 
 def _closure(model):
@@ -554,12 +540,12 @@ def _snapshot(data):
     return out
 
 
-def gpu_run(name, assets, path=None):
+def gpu_run(name, assets):
     """first closure of every stage and the closure after its Adam steps on the CUDA path: packed gradients, term values,
     theta and the state the oracle needs"""
     from glamr_b200 import lib as L
     cfg, in_dict, make_prior = case(name, assets)
-    model = _make_model(cfg, assets, make_prior(DEV), path)
+    model = _make_model(cfg, assets, make_prior(DEV))
     data = _init(model, in_dict)
     P = len(data['person_data'])
     recs = []
@@ -648,31 +634,6 @@ def test_gpu_gradients_within_float64_bound(name, gpu_refs):
     """default iteration path: every variable's gradient and every term value at the first closure of every stage and after
     the stage's Adam steps"""
     _check_records(name, gpu_refs(name)[2])
-
-
-@pytest.mark.gpu
-@pytest.mark.parametrize('name', ALL)
-def test_gpu_fused_path_within_float64_bound_and_bitwise_equal(name, gpu_refs, smpl_assets):
-    """GLAMR_ITER_PATH=fused (forward_pose_kernel; residuals_backward_kernel with Adam inside, except in the camera-from-persons
-    mode, which keeps the default tail): every check point of every stage is held to the float64 bound at its own theta, terms
-    included, and the packed gradient and theta are bit-identical to the default path's.  Term sums: the default path folds
-    its float64 partial sums over the residual CTAs, the fused tail over the persons, so a float32 term sum may differ by the
-    rounding of that re-association: 2 float32 ulp"""
-    lay, cfg, recs, template = gpu_refs(name)
-    _, _, fused = gpu_run(name, smpl_assets, path='fused')
-    for r, f in zip(recs, fused):
-        if torch.equal(r['theta'], f['theta']):
-            f['ref'] = r['ref']
-    _references_of(name, cfg, smpl_assets, lay, fused, template)
-    _check_records(name, fused, ' (fused)')
-    for r, f in zip(recs, fused):
-        what = f'{name} {r["stage"]} {r["point"]}'
-        assert torch.equal(r['theta'], f['theta']), f'{what}: theta differs, max {float((r["theta"] - f["theta"]).abs().max()):.3e}'
-        diff = (r['grad'] != f['grad']).nonzero().flatten()
-        assert diff.numel() == 0, f'{what}: {diff.numel()} gradient elements differ, first at {int(diff[0])}, max |d| ' \
-                                  f'{float((r["grad"] - f["grad"]).abs().max()):.3e}'
-        s0, s1 = r['sums'].double(), f['sums'].double()
-        assert bool(((s0 - s1).abs() <= 2 * EPS32 * s0.abs()).all()), f'{what}: term sums {s0.tolist()} vs {s1.tolist()}'
 
 
 SPLITS = {'dynamic_p1_t1025': [512],                    # inside the person, at its exist frame 512
@@ -792,15 +753,15 @@ class AdamProbe:
         torch.cuda.synchronize()
         return (m._theta.cpu().clone(), m._read(L.R_ADAM_M, self.n).cpu(), m._read(L.R_ADAM_V, self.n).cpu())
 
-    def step(self, lr, fused):
-        """one Adam step: fused, one glamr_opt_iterate iteration (evaluation + Adam in residuals_backward_kernel); else
-        glamr_opt_apply (apply_kernel) on the gradient already in the model's reduce buffer -> (before, after, g, device step)"""
+    def step(self, lr, via_iterate):
+        """one Adam step: via_iterate, one eager glamr_opt_iterate iteration (evaluation + apply_kernel); else glamr_opt_apply
+        (apply_kernel) on the gradient already in the model's reduce buffer -> (before, after, g, device step)"""
         from glamr_b200 import lib as L
         m = self.model
         before = self.state()
         self.hist.fill_(float('nan'))
         with torch.cuda.device(DEV):
-            if fused:
+            if via_iterate:
                 L.check(m._lib.glamr_opt_iterate(m._opt, L.ptr(m._theta), L.ptr(m._reduce), float(lr), L.ptr(self.hist), L.NUM_TERMS + 1,
                                                  1, 0, L.stream_ptr()), 'glamr_opt_iterate')
             else:
@@ -853,35 +814,34 @@ def test_gpu_adam_step_matches_float64_adam(smpl_assets):
         model._set_stage(data, specs['opt_variables'], specs['loss_cfg'], stage, reset_adam=True, begin=True)
         for k in range(1, ADAM_K + 1):
             model._backward()
-            before, after, g, step = probe.step(specs['opt_lr'], fused=False)
+            before, after, g, step = probe.step(specs['opt_lr'], via_iterate=False)
             assert step == k, f'{stage}: device step {step}, expected {k}'
             if k in (1, ADAM_K):
                 _check_adam_step(f'{stage} step {k}', model, specs['opt_lr'], before, after, g, step)
 
 
 @pytest.mark.gpu
-def test_gpu_fused_adam_matches_float64_adam_and_apply_kernel(smpl_assets):
-    """adam_range inside residuals_backward_kernel (person blocks and the camera block): at step 1, step k and after a stage
-    change it matches float64 Adam like apply_kernel, and a default-path twin that applies the gradient each fused step
-    consumed, from the same theta, ends every step with bit-identical theta, m and v and the same device step count"""
+def test_gpu_iterate_matches_backward_for_apply_and_apply(smpl_assets):
+    """glamr_opt_iterate (one eager iteration per call) at step 1, step k and after a stage change matches float64 Adam, and a
+    twin handle driven by glamr_opt_backward_for_apply + glamr_opt_apply from the same theta ends every step with the same
+    gradient, bit-identical theta, m and v and the same device step count"""
     cfg, in_dict, make_prior = case(ADAM_CASE, smpl_assets)
-    assert not cfg.grecon_model_specs.get('flag_opt_cam_from_person_pose', False)     # the fused tail with Adam inside runs
-    fused, twin = _make_model(cfg, smpl_assets, make_prior(DEV), 'fused'), _make_model(cfg, smpl_assets, make_prior(DEV), 'legacy')
-    df, dt = _init(fused, in_dict), _init(twin, in_dict)
-    pf, pt = AdamProbe(fused), AdamProbe(twin)
+    model, twin = _make_model(cfg, smpl_assets, make_prior(DEV)), _make_model(cfg, smpl_assets, make_prior(DEV))
+    dm, dt = _init(model, in_dict), _init(twin, in_dict)
+    pm, pt = AdamProbe(model), AdamProbe(twin)
     for stage, specs in list(cfg.opt_stage_specs.items())[:2]:
-        for m, d in ((fused, df), (twin, dt)):
+        for m, d in ((model, dm), (twin, dt)):
             m._cur_vars, m._cur_stage, m._loss_cfg = specs['opt_variables'], stage, specs['loss_cfg']
             m._set_stage(d, specs['opt_variables'], specs['loss_cfg'], stage, reset_adam=True, begin=True)
-        assert torch.equal(fused._theta, twin._theta), f'{stage}: the two handles start the stage from different theta'
+        assert torch.equal(model._theta, twin._theta), f'{stage}: the two handles start the stage from different theta'
         for k in range(1, ADAM_K + 1):
-            before, after, g, step = pf.step(specs['opt_lr'], fused=True)
+            before, after, g, step = pm.step(specs['opt_lr'], via_iterate=True)
             assert step == k, f'{stage}: device step {step}, expected {k}'
             if k in (1, ADAM_K):
-                _check_adam_step(f'fused {stage} step {k}', fused, specs['opt_lr'], before, after, g, step)
-            twin._reduce.copy_(fused._reduce)
-            _, after_t, _, step_t = pt.step(specs['opt_lr'], fused=False)
+                _check_adam_step(f'iterate {stage} step {k}', model, specs['opt_lr'], before, after, g, step)
+            twin._backward(for_apply=True)
+            _, after_t, g_t, step_t = pt.step(specs['opt_lr'], via_iterate=False)
             assert step_t == step
-            for label, x, y in zip(('theta', 'm', 'v'), after, after_t):
-                assert torch.equal(x, y), f'{stage} step {k}: {label} of adam_range and apply_kernel differ, max ' \
-                                          f'{float((x - y).abs().max()):.3e}'
+            for label, x, y in zip(('gradient', 'theta', 'm', 'v'), (g, *after), (g_t, *after_t)):
+                assert torch.equal(x, y), f'{stage} step {k}: {label} of glamr_opt_iterate and backward_for_apply + apply differ, ' \
+                                          f'max {float((x - y).abs().max()):.3e}'

@@ -4,8 +4,8 @@ trajectory (flag_infer_motion_traj / flag_pred_traj false), the camera-derived o
 
 CPU: the oracle against the executed reference (tests/golden/globalopt_ts_*.npz), the host-compiled frame functions and
 Adam against oracle autograd, person sharding over two gloo ranks.  GPU (-m gpu): the CUDA path against the fixtures'
-float64 noise floor, iteration-0 gradients against oracle autograd, CUDA graph vs eager, the fused iteration kernels,
-and a run_dataset sweep without any learned prior."""
+float64 noise floor, iteration-0 gradients against oracle autograd, CUDA graph vs eager, and a run_dataset sweep without
+any learned prior."""
 import copy
 import ctypes
 import os
@@ -462,18 +462,6 @@ def test_gpu_cuda_graph_and_eager_agree(smpl_assets):
         for k in ['smpl_orient_world', 'root_trans_world', 'smpl_orient_world_res', 'kp_2d_pred']:
             np.testing.assert_array_equal(outs[0]['person_data'][pid][k], outs[1]['person_data'][pid][k])
     np.testing.assert_array_equal(outs[0]['cam_pose'], outs[1]['cam_pose'])
-
-
-@pytest.mark.gpu
-@pytest.mark.parametrize('name', ['ts_dynamic_cam_p1_t40_gaps', 'ts_static_multi_last_p3_t30_gaps', 'ts_cam_only_p2_t32_gaps'])
-def test_gpu_fused_iteration_kernels_match_reference_golden(name, smpl_assets, monkeypatch):
-    """GLAMR_ITER_PATH=fused (forward_pose_kernel / residuals_backward_kernel) takes the same trajectory source"""
-    monkeypatch.setenv('GLAMR_ITER_PATH', 'fused')
-    gold, cfg, in_dict, model = _make(name, smpl_assets)
-    data = model.init_data(copy.deepcopy(in_dict))
-    _align_half_turns(model, data, gold)
-    _check_init(data, gold)
-    _check_trajectory(model, data, cfg, gold)
 
 
 @pytest.mark.gpu

@@ -3,8 +3,8 @@ offset added in place to root_trans_world, include/glamr_b200.h: heading_vec, ha
 
 CPU: the oracle against the executed reference (tests/golden/globalopt_tv_*.npz), the host-compiled frame functions and Adam
 against oracle autograd, person sharding over two gloo ranks with world_dxy accumulating in the base, and the combinations that
-are refused.  GPU (-m gpu): the CUDA path against the fixtures' float64 noise floor on the default and the fused iteration
-kernels, iteration-0 gradients against oracle autograd, CUDA graph vs eager, and a run_dataset sweep with a vec config."""
+are refused.  GPU (-m gpu): the CUDA path against the fixtures' float64 noise floor, iteration-0 gradients against oracle
+autograd, CUDA graph vs eager, and a run_dataset sweep with a vec config."""
 import copy
 import ctypes
 import os
@@ -375,19 +375,6 @@ def _check_trajectory(model, data, cfg, gold):
 def test_gpu_trajectory_matches_reference_golden(name, smpl_assets):
     """init state, per-iteration residual values and the final state of every frame (world pose, base, heading vectors, world_dxy)
     vs the executed reference, at its float64 noise floor"""
-    gold, cfg, in_dict, model = _make(name, smpl_assets)
-    data = model.init_data(copy.deepcopy(in_dict))
-    _align_half_turns(model, data, gold)
-    _check_init(data, gold)
-    _check_trajectory(model, data, cfg, gold)
-
-
-@pytest.mark.gpu
-@pytest.mark.parametrize('name', ['tv_static_multi_vec_p3_t30_gaps', ALIAS_CASE, 'tv_dynamic_cam_dxy_p1_t40_gaps',
-                                  'tv_static_multi_vec_dxy_p4_t300_gaps'])
-def test_gpu_fused_iteration_kernels_match_reference_golden(name, smpl_assets, monkeypatch):
-    """GLAMR_ITER_PATH=fused (forward_pose_kernel / residuals_backward_kernel) runs the same frame functions"""
-    monkeypatch.setenv('GLAMR_ITER_PATH', 'fused')
     gold, cfg, in_dict, model = _make(name, smpl_assets)
     data = model.init_data(copy.deepcopy(in_dict))
     _align_half_turns(model, data, gold)
