@@ -9,6 +9,7 @@
 //   adam            (loss terms + torch.optim.Adam update, step count on device => CUDA-graph capturable)
 // No atomics: every sum is a fixed-order tree, so iterations are bit-reproducible.
 #include <stdlib.h>
+#include <algorithm>
 #include <string.h>
 
 #include "globalopt_frames.cuh"
@@ -400,11 +401,14 @@ struct glamr_opt {
   // backward kernels of this one (it depends on body pose and betas only); `vpt_ready` says the workspace holds a valid v_posed
   cudaStream_t aux;
   cudaEvent_t ev_fork, ev_join;
+  cudaEvent_t ev_sup;         // the support tiles are skinned: the next blend GEMM may rewrite their v_posed columns
   int vpt_ready;
   int join_pending;           // a glamr_opt_backward_for_apply call left the side stream un-joined (the next call on the handle joins)
   int features_early;         // the pipelined blend's feature kernel runs at the top of the evaluation
   cudaEvent_t ev[24];         // timing == 2: one event after every launch of glamr_opt_backward / glamr_opt_apply
   int n_ev;
+  cudaEvent_t ev_side[3];     // timing == 2: the side stream before the mesh skinning, after it, after the blend GEMM
+  int n_ev_side;
   // glamr_opt_iterate: one captured iteration (backward + apply), valid for the arguments it was captured with
   cudaStream_t cap_stream;
   cudaGraphExec_t iter_exec;
@@ -500,6 +504,7 @@ extern "C" int glamr_opt_kernel_timing(glamr_opt_t* st, int enable) {
     GLAMR_CUDA_TRY(cudaEventCreate(&st->ev_blend0));
     GLAMR_CUDA_TRY(cudaEventCreate(&st->ev_blend1));
     for (int i = 0; i < 24; ++i) GLAMR_CUDA_TRY(cudaEventCreate(&st->ev[i]));
+    for (int i = 0; i < 3; ++i) GLAMR_CUDA_TRY(cudaEventCreate(&st->ev_side[i]));
   }
   st->timing = enable;
   return GLAMR_OK;
@@ -518,8 +523,9 @@ extern "C" int glamr_opt_last_lbs_ms(glamr_opt_t* st, float* ms) {
   return GLAMR_OK;
 }
 
-// The two parts of the last timed evaluation separately: the kernel on the iteration's critical path (skinning on the tensor-core
-// path, the whole LBS kernel on the SIMT path) and the blend on its side stream (0 on the SIMT path).
+// The two parts of the last timed evaluation separately: the kernel on the iteration's critical path (the support tiles' skinning on the
+// tensor-core path, the whole skinning with the tcblend LBS, the whole LBS kernel on the SIMT path) and the side stream's LBS work (mesh
+// skinning + blend on the tensor-core path, the blend with tcblend, 0 on the SIMT path).  Their sum is the whole LBS of the evaluation.
 extern "C" int glamr_opt_last_lbs_parts_ms(glamr_opt_t* st, float* critical_ms, float* blend_ms) {
   if (!st || !critical_ms || !blend_ms || !st->ev_lbs0) return GLAMR_EINVAL;
   GLAMR_CUDA_TRY(cudaEventSynchronize(st->ev_lbs1));
@@ -559,13 +565,19 @@ extern "C" int glamr_opt_time_blend(glamr_opt_t* st, int reps, float* ms) {
   return rc;
 }
 
-// timing == 2: durations (ms) between consecutive marks of the last glamr_opt_backward (+ apply) call sequence
+// timing == 2: durations (ms) between consecutive marks of the last glamr_opt_backward (+ apply) call sequence on the caller's stream,
+// then, when the mesh was skinned on the side stream, the mesh skinning and the blend there (features + GEMM, after the support tiles)
 extern "C" int glamr_opt_kernel_times(glamr_opt_t* st, float* ms, int* n) {
   if (!st || !ms || !n || !st->ev_lbs0) return GLAMR_EINVAL;
   if (st->n_ev < 2) { *n = 0; return GLAMR_OK; }
   GLAMR_CUDA_TRY(cudaEventSynchronize(st->ev[st->n_ev - 1]));
   for (int i = 0; i + 1 < st->n_ev; ++i) GLAMR_CUDA_TRY(cudaEventElapsedTime(&ms[i], st->ev[i], st->ev[i + 1]));
   *n = st->n_ev - 1;
+  if (st->n_ev_side == 3) {
+    GLAMR_CUDA_TRY(cudaEventSynchronize(st->ev_side[2]));
+    for (int i = 0; i < 2; ++i) GLAMR_CUDA_TRY(cudaEventElapsedTime(&ms[*n + i], st->ev_side[i], st->ev_side[i + 1]));
+    *n += 2;
+  }
   return GLAMR_OK;
 }
 
@@ -573,8 +585,15 @@ extern "C" int glamr_opt_destroy(glamr_opt_t* st) {
   if (st && st->iter_exec) cudaGraphExecDestroy(st->iter_exec);
   if (st && st->cap_stream) cudaStreamDestroy(st->cap_stream);
   if (!st) return GLAMR_OK;
-  if (st->ev_lbs0) { cudaEventDestroy(st->ev_lbs0); cudaEventDestroy(st->ev_lbs1); cudaEventDestroy(st->ev_blend0); cudaEventDestroy(st->ev_blend1); for (int i = 0; i < 24; ++i) cudaEventDestroy(st->ev[i]); }
-  if (st->aux) { cudaStreamSynchronize(st->aux); cudaStreamDestroy(st->aux); cudaEventDestroy(st->ev_fork); cudaEventDestroy(st->ev_join); }
+  if (st->ev_lbs0) {
+    cudaEventDestroy(st->ev_lbs0); cudaEventDestroy(st->ev_lbs1); cudaEventDestroy(st->ev_blend0); cudaEventDestroy(st->ev_blend1);
+    for (int i = 0; i < 24; ++i) cudaEventDestroy(st->ev[i]);
+    for (int i = 0; i < 3; ++i) cudaEventDestroy(st->ev_side[i]);
+  }
+  if (st->aux) {
+    cudaStreamSynchronize(st->aux); cudaStreamDestroy(st->aux);
+    cudaEventDestroy(st->ev_fork); cudaEventDestroy(st->ev_join); cudaEventDestroy(st->ev_sup);
+  }
   cudaFree(st->arena);
   free(st);
   return GLAMR_OK;
@@ -617,11 +636,16 @@ extern "C" int glamr_opt_set_problem(glamr_opt_t* st, const glamr_problem_t* pb,
 
 extern "C" size_t glamr_opt_reduce_count(const glamr_opt_t* st) { return st ? (size_t)st->pb.n_params + GLAMR_NUM_TERMS : 0; }
 
+// the tensor-core skinning runs in two launches, the support tiles on the iteration's critical path and the mesh tiles on the side stream
+static bool skin_split(const glamr_opt_t* st) { return lbs_path() >= 1 && st->smpl.tcB != nullptr && st->ws.vp_tiled; }
+
 extern "C" int glamr_opt_launch_count(const glamr_opt_t* st) {
   if (!st) return GLAMR_EINVAL;
   const bool from_persons = st->pb.cam_mode == GLAMR_CAM_FROM_PERSONS;
   const bool has_frames = st->pb.n_end > st->pb.n_begin;
-  const int fwd = 1 + (from_persons ? 1 : 0) + (has_frames ? 1 + (lbs_kernel_count(st->smpl) == 2 ? 3 : 1) : 0);     // forward [+ cam_forward] [+ pose_prep + lbs]
+  // lbs: support + mesh skinning, features, GEMM | skinning, features, GEMM (tcblend) | one kernel (SIMT)
+  const int lbs = skin_split(st) ? 4 : lbs_kernel_count(st->smpl) == 2 ? 3 : 1;
+  const int fwd = 1 + (from_persons ? 1 : 0) + (has_frames ? 1 + lbs : 0);     // forward [+ cam_forward] [+ pose_prep + lbs]
   return fwd + 1 + (from_persons ? 2 : 0) + 1 + 1;                       // residuals [+ camera backward + scatter] + traj/cam backward + apply
 }
 
@@ -636,8 +660,8 @@ static int join_pending(glamr_opt_t* st, cudaStream_t s) {
   return GLAMR_OK;
 }
 
-// defer_join: the caller runs glamr_opt_apply on the same handle next (possibly after an exchange of reduce_buf): the pipelined blend on the
-// side stream is joined there, so that the exchange overlaps its tail instead of waiting for it
+// defer_join: the caller runs glamr_opt_apply on the same handle next (possibly after an exchange of reduce_buf): the pipelined mesh skinning
+// and blend on the side stream are joined after that apply's launch, so that the exchange and the Adam update overlap their tail
 static int backward_impl(glamr_opt_t* st, const float* theta, float* reduce_buf, void* stream, bool use_peers, bool defer_join = false) {
   if (!st || !theta || !reduce_buf) return GLAMR_EINVAL;
   PeerCtx pc = st->peer;
@@ -666,8 +690,11 @@ static int backward_impl(glamr_opt_t* st, const float* theta, float* reduce_buf,
       GLAMR_CUDA_TRY(cudaStreamCreateWithFlags(&st->aux, cudaStreamNonBlocking));
       GLAMR_CUDA_TRY(cudaEventCreateWithFlags(&st->ev_fork, cudaEventDisableTiming));
       GLAMR_CUDA_TRY(cudaEventCreateWithFlags(&st->ev_join, cudaEventDisableTiming));
+      GLAMR_CUDA_TRY(cudaEventCreateWithFlags(&st->ev_sup, cudaEventDisableTiming));
     }
   }
+  const bool split = tc && skin_split(st);
+  st->n_ev_side = 0;
   bool forked = false;
 #ifdef GLAMR_EXPERIMENT
   // experiment build only (tools/iter_skip_exp.py): GLAMR_EXP_SKIP bit 1 = no pipelined blend, 2 = no skinning, 4 = no residual kernel, 8 = no backward kernel
@@ -679,18 +706,24 @@ static int backward_impl(glamr_opt_t* st, const float* theta, float* reduce_buf,
   const float* const beta_l = pb.smpl_beta_all + (size_t)n_begin * kNB;
   // the blend of the NEXT evaluation (it depends on body pose / betas only): side stream, concurrent with this evaluation.  Its GEMM
   // rewrites v_posed, so it starts after the skinning has read it; with features_early its feature kernel is forked at the top
-  // (the GEMM's operand is then ready when the skinning ends)
+  // (the GEMM's operand is then ready when the skinning ends).  split: the mesh tiles' skinning runs on the side stream ahead of the
+  // GEMM, which waits for the support tiles' skinning on the caller's stream as well (wait_for: that event instead of a fork here)
   const bool features_top = st->features_early && !st->timing;
-  auto fork_blend = [&](bool features, bool gemm) -> int {
-    GLAMR_CUDA_TRY(cudaEventRecord(st->ev_fork, s));
-    GLAMR_CUDA_TRY(cudaStreamWaitEvent(st->aux, st->ev_fork, 0));
-    if (st->timing && features) GLAMR_CUDA_TRY(cudaEventRecord(st->ev_blend0, st->aux));
+  auto fork_blend = [&](bool features, bool gemm, cudaEvent_t wait_for = nullptr) -> int {
+    if (wait_for) {
+      GLAMR_CUDA_TRY(cudaStreamWaitEvent(st->aux, wait_for, 0));
+    } else {
+      GLAMR_CUDA_TRY(cudaEventRecord(st->ev_fork, s));
+      GLAMR_CUDA_TRY(cudaStreamWaitEvent(st->aux, st->ev_fork, 0));
+    }
+    if (st->timing && features && !split) GLAMR_CUDA_TRY(cudaEventRecord(st->ev_blend0, st->aux));
     if (!(exp_skip & 1)) {
       const int rc = launch_blend(st->smpl, n_end - n_begin, pose_l, beta_l, wo, st->aux, features, gemm);
       if (rc) return rc;
     }
     if (gemm) {
       if (st->timing) GLAMR_CUDA_TRY(cudaEventRecord(st->ev_blend1, st->aux));
+      if (st->timing == 2 && split) GLAMR_CUDA_TRY(cudaEventRecord(st->ev_side[st->n_ev_side++], st->aux));
       GLAMR_CUDA_TRY(cudaEventRecord(st->ev_join, st->aux));
       forked = true;
     }
@@ -718,10 +751,30 @@ static int backward_impl(glamr_opt_t* st, const float* theta, float* reduce_buf,
     int rc;
     if ((rc = launch_pose_prep(st->smpl, nn, st->sc.orient_world + (size_t)n_begin * 3, pose_l, beta_l, 1, wo_pose, s, true))) return rc;
     GLAMR_MARK();
-    if (tc) {
+    if (split) {
+      // The optimiser reads the support vertices only: their tiles are skinned here, on the critical path, and the mesh tiles (the
+      // rest of the full LBS) on the side stream, ahead of the next evaluation's blend.  The support launch is issued first and the
+      // mesh grid leaves its CTAs' SMs free (both kernels take a whole SM), so the critical path never queues behind the mesh.
+      const int sms = smpl_device_sms(), nft = (nn + kSkF - 1) / kSkF;
+      const int sup_ctas = std::min(sms, (st->smpl.sk_tiles - kNVTiles) * nft);
+      const int mesh_ctas = std::max(sms - sup_ctas, sms / 2);
+      GLAMR_CUDA_TRY(cudaEventRecord(st->ev_fork, s));
       if (st->timing) GLAMR_CUDA_TRY(cudaEventRecord(st->ev_lbs0, s));
       if (!(exp_skip & 2))
-        if ((rc = launch_skin(st->smpl, nn, wo, nullptr, s))) return rc;
+        if ((rc = launch_skin(st->smpl, nn, wo, nullptr, s, kNVTiles, st->smpl.sk_tiles, sms))) return rc;
+      GLAMR_CUDA_TRY(cudaEventRecord(st->ev_sup, s));
+      if (st->timing) GLAMR_CUDA_TRY(cudaEventRecord(st->ev_lbs1, s));
+      GLAMR_CUDA_TRY(cudaStreamWaitEvent(st->aux, st->ev_fork, 0));
+      if (st->timing) GLAMR_CUDA_TRY(cudaEventRecord(st->ev_blend0, st->aux));
+      if (st->timing == 2) GLAMR_CUDA_TRY(cudaEventRecord(st->ev_side[st->n_ev_side++], st->aux));
+      if (!(exp_skip & 2))
+        if ((rc = launch_skin(st->smpl, nn, wo, nullptr, st->aux, 0, kNVTiles, mesh_ctas))) return rc;
+      if (st->timing == 2) GLAMR_CUDA_TRY(cudaEventRecord(st->ev_side[st->n_ev_side++], st->aux));
+      if ((rc = fork_blend(!features_top, true, st->ev_sup))) return rc;
+    } else if (tc) {
+      if (st->timing) GLAMR_CUDA_TRY(cudaEventRecord(st->ev_lbs0, s));
+      if (!(exp_skip & 2))
+        if ((rc = launch_skin(st->smpl, nn, wo, nullptr, s, 0, kNVTiles, smpl_device_sms()))) return rc;
       if (st->timing) GLAMR_CUDA_TRY(cudaEventRecord(st->ev_lbs1, s));
       if ((rc = fork_blend(!features_top, true))) return rc;
     } else {
@@ -777,16 +830,14 @@ static int apply_impl(glamr_opt_t* st, float* theta, const float* reduce_buf, do
   PeerCtx pc = st->peer;
   if (!use_peers) pc.world = 0;
   cudaStream_t s = (cudaStream_t)stream;
-  {
-    const int rc = join_pending(st, s);
-    if (rc) return rc;
-  }
   OptCtx c = make_ctx(st, theta, nullptr);
   const int blocks = (st->pb.n_params + 255) / 256;
   GLAMR_CUDA_TRY(launch_pdl(32, apply_kernel, dim3(blocks < 296 ? blocks : 296), dim3(256), 0, s, c, theta, reduce_buf, lr, st->adam, loss_terms,
                             loss_hist_stride, st->tickets + 1, pc));
   GLAMR_MARK();
-  return GLAMR_OK;
+  // the Adam update touches none of the side stream's buffers (v_posed, the blend features, the skinning operands): it runs beside
+  // the side stream's tail, which rejoins after it
+  return join_pending(st, s);
 }
 extern "C" int glamr_opt_apply(glamr_opt_t* st, float* theta, const float* reduce_buf, double lr, float* loss_terms,
                                int loss_hist_stride, void* stream) {
@@ -862,7 +913,7 @@ extern "C" int glamr_opt_iterate(glamr_opt_t* st, float* theta, float* reduce_bu
   int rc, done = 0;
   const bool peers = st->peer.world > 1;      // W > 1: backward publishes, apply sums the peers' slots (no call in between)
   auto eager = [&](cudaStream_t q) -> int {
-    if ((rc = backward_impl(st, theta, reduce_buf, q, peers))) return rc;
+    if ((rc = backward_impl(st, theta, reduce_buf, q, peers, true))) return rc;      // the side stream rejoins after apply
     return apply_impl(st, theta, reduce_buf, lr, loss_terms, loss_hist_stride, q, peers);
   };
   if (!use_graph || st->timing) {

@@ -367,15 +367,16 @@ extern "C" int glamr_exp_blend_phases(long long* out) {    // the per-CTA sums o
 #endif
 
 // mtile0 / mtiles: the 128-frame tiles [mtile0, mtile0 + mtiles) of this launch (the host launches them all, from mtile0 = 0);
-// half_last: the last of them holds at most 64 frames
-__global__ void __launch_bounds__(kTcThreads, 1) lbs_blend_tc_kernel(SmplDev m, SmplWorkspace w, int mtile0, int mtiles, int half_last) {
+// half_last: the last of them holds at most 64 frames; ntn: the 256-column tiles (the mesh's 81, plus the support columns when the
+// skinning runs on the tensor cores)
+__global__ void __launch_bounds__(kTcThreads, 1) lbs_blend_tc_kernel(SmplDev m, SmplWorkspace w, int mtile0, int mtiles, int half_last, int ntn) {
   extern __shared__ __align__(128) unsigned char tc_raw[];
   __half* As = reinterpret_cast<__half*>(tc_raw);                                 // [stages][hi | lo][2][128][8]
   __half* Bs = As + kTcStages * kTcAStageHalves;                                  // [stages][hi | lo][2][256][8]
   uint64_t* full = reinterpret_cast<uint64_t*>(Bs + kTcStages * kTcBStageHalves); // [stages]
   uint64_t* empty = full + kTcStages;                                             // [stages]
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-  const int ntiles = kTcNTiles * mtiles;
+  const int ntiles = ntn * mtiles;
   pdl_launch_dependents();
   if (tid == 0) {
 #pragma unroll
@@ -467,7 +468,7 @@ __global__ void __launch_bounds__(kTcThreads, 1) lbs_blend_tc_kernel(SmplDev m, 
     for (int h = 0; h < 2; ++h) {
       const int frame = row0 + 8 * h;                                             // < w.mpad by construction
       const float unscale = w.tcUnscale[frame] * m.tcB_unscale;                   // 2^-(e_f + e_B): exact
-      float* out = (w.vp_tiled ? vpb + ((size_t)(frame / kSkF) * kTcCols + (size_t)col0) * kSkF + frame % kSkF
+      float* out = (w.vp_tiled ? vpb + ((size_t)(frame / kSkF) * w.vp_cols + (size_t)col0) * kSkF + frame % kSkF
                                : vpb + (size_t)col0 * w.mpad + frame) + (size_t)(2 * (lane & 3)) * cstride;
 #pragma unroll
       for (int i = 0; i < kTcN / 8; ++i) {
@@ -598,6 +599,10 @@ __global__ void __launch_bounds__(kLbsThreads) lbs_skin_kernel(SmplDev m, int n_
 // bounded the SIMT skinning (12 LDS.128 per vertex-frame).  The epilogue has no branch before a row's stores: written with a
 // lane-dependent branch and a shuffle and store check per output, every output waited on the one before and the epilogue took
 // ~70 % of an item (tools/skin_phases_exp.py).  warp 8 = producer.
+// A launch skins the vertex tiles [vt0, vt1): mesh tiles (< kNVTiles) store into `vertices` when it is given, support tiles (the support
+// vertices again, slot by slot, with their copied weights and v_posed columns; smpl_model.cuh) into vcompact.  The optimiser skins the
+// support tiles on its critical path and the mesh tiles beside it; a mesh-only or support-only launch does exactly what the same items of
+// an all-tiles launch do, so a support vertex comes out bit for bit as its mesh vertex.
 // Persistent: a work item is one (vertex tile, frame tile) pair, numbered vertex-tile major, and CTA b of a grid of at most one CTA per
 // SM (the register file holds one) runs the contiguous item range [b items / grid, (b + 1) items / grid).  Every CTA gets within one
 // item of the average, which a fixed number of frame tiles per CTA could not give for every n, and its range spans at most two vertex
@@ -636,7 +641,8 @@ extern "C" int glamr_exp_skin_phases(long long* out) {     // the per-CTA sums o
 #define SKIN_CLOCK_STORE(items) do { } while (0)
 #endif
 
-__global__ void __launch_bounds__(kSkinTcThreads, 1) lbs_skin_tc_kernel(SmplDev m, int n, SmplWorkspace w, float* __restrict__ vertices) {
+__global__ void __launch_bounds__(kSkinTcThreads, 1) lbs_skin_tc_kernel(SmplDev m, int n, SmplWorkspace w, float* __restrict__ vertices,
+                                                                        int vt0, int vt1) {
   extern __shared__ __align__(128) unsigned char sk_raw[];
   float* Ws = reinterpret_cast<float*>(sk_raw);                       // [hi | lo][6][128][4]
   float* Bs = Ws + kSkWImageFloats;                                   // [2][hi | lo][6][240][4]
@@ -648,7 +654,7 @@ __global__ void __launch_bounds__(kSkinTcThreads, 1) lbs_skin_tc_kernel(SmplDev 
   uint64_t* v_empty = full_w + 7;         // [2] the 8 consumer warps are done with the v_posed block
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const int nft = (n + kSkF - 1) / kSkF;
-  const int items = kNVTiles * nft;
+  const int items = (vt1 - vt0) * nft;
   const int i0 = (int)((long long)blockIdx.x * items / gridDim.x), i1 = (int)((long long)(blockIdx.x + 1) * items / gridDim.x);
   pdl_launch_dependents();
   if (tid == 0) {
@@ -666,11 +672,11 @@ __global__ void __launch_bounds__(kSkinTcThreads, 1) lbs_skin_tc_kernel(SmplDev 
   if (warp == 8) {
     if (lane == 0) {
       mbar_expect_tx(full_w, kSkWBytes);
-      tma_bulk_g2s(Ws, m.skW + (size_t)(i0 / nft) * kSkWImageFloats, kSkWBytes, full_w);     // model constant: before the dependency wait
+      tma_bulk_g2s(Ws, m.skW + (size_t)(vt0 + i0 / nft) * kSkWImageFloats, kSkWBytes, full_w);   // model constant: before the dependency wait
       pdl_wait();                                                                           // skB (pose prep) and v_posed (blend) below
       const float* const vpb = vp_buffer(w);
       for (int i = i0, it = 0; i < i1; ++i, ++it) {
-        const int vtile = i / nft, ftile = i - vtile * nft, vb = it & 1;
+        const int vtile = vt0 + i / nft, ftile = i - (vtile - vt0) * nft, vb = it & 1;
         const bool new_w = it > 0 && ftile == 0;                                            // the range crossed into the next vertex tile
         if (it >= 2) mbar_wait(&b_empty[vb], ((it - 2) >> 1) & 1);
         if (new_w) mbar_wait(&b_empty[vb ^ 1], ((it - 1) >> 1) & 1);                       // Ws is read until the previous item's wgmmas retire
@@ -679,7 +685,7 @@ __global__ void __launch_bounds__(kSkinTcThreads, 1) lbs_skin_tc_kernel(SmplDev 
         if (new_w) tma_bulk_g2s(Ws, m.skW + (size_t)vtile * kSkWImageFloats, kSkWBytes, &full_b[vb]);
         if (it >= 2) mbar_wait(&v_empty[vb], ((it - 2) >> 1) & 1);
         mbar_expect_tx(&full_v[vb], kSkVBytes);
-        tma_bulk_g2s(Vs + vb * kSkVpTileFloats, vpb + ((size_t)ftile * kTcCols + (size_t)vtile * kTileCols) * kSkF, kSkVBytes, &full_v[vb]);
+        tma_bulk_g2s(Vs + vb * kSkVpTileFloats, vpb + ((size_t)ftile * w.vp_cols + (size_t)vtile * kTileCols) * kSkF, kSkVBytes, &full_v[vb]);
       }
     }
     return;
@@ -702,14 +708,19 @@ __global__ void __launch_bounds__(kSkinTcThreads, 1) lbs_skin_tc_kernel(SmplDev 
   SKIN_CLOCK_INIT();
   mbar_wait(full_w, 0);
   for (int i = i0, it = 0; i < i1; ++i, ++it) {
-    const int vtile = i / nft, ftile = i - vtile * nft, vb = it & 1;
-    int gv[2], ci[2];
+    const int vtile = vt0 + i / nft, ftile = i - (vtile - vt0) * nft, vb = it & 1;
+    // the output array of the tile (nullptr: stores nothing), its stride between frames and the row of each accumulator row of this
+    // thread (-1: none)
+    const bool sup = vtile >= kNVTiles;
+    float* const out = sup ? w.vcompact : vertices;
+    const int fstride = sup ? m.S * 3 : kV * 3;
+    int orow[2];
     const float* vrow[2];
 #pragma unroll
     for (int h = 0; h < 2; ++h) {
       const int vl = g * 64 + (warp & 3) * 16 + (lane >> 2) + 8 * h;   // accumulator rows of this thread
-      gv[h] = vtile * kVTile + vl;
-      ci[h] = m.compact_of_vertex[min(gv[h], kVPad - 1)];
+      const int v = (vtile - (sup ? kNVTiles : 0)) * kVTile + vl;      // support slot or mesh vertex
+      orow[h] = out && v < (sup ? m.S : kV) ? v * 3 : -1;
       vrow[h] = Vs + vb * kSkVpTileFloats + (size_t)vl * 3 * kSkF;
     }
     SKIN_CLOCK(4);
@@ -740,8 +751,7 @@ __global__ void __launch_bounds__(kSkinTcThreads, 1) lbs_skin_tc_kernel(SmplDev 
     SKIN_CLOCK(2);
     // Epilogue, straight-line: per frame pair x, y, z of frames 2 p and 2 p + 1 are loaded once and lane-dependent selects stand in for
     // branches, and a row is stored after all its outputs are computed, so the compiler can overlap the frame pairs; per output the same
-    // arithmetic as fmaf(t0, x, t1 * y) + fmaf(t0, z, t1) (t1 * 1.0f is exact).  Most rows store nothing: the optimiser keeps only
-    // the support vertices.
+    // arithmetic as fmaf(t0, x, t1 * y) + fmaf(t0, z, t1) (t1 * 1.0f is exact).  In the optimiser the mesh rows store nothing.
 #pragma unroll
     for (int h = 0; h < 2; ++h) {
       const float2* const vr = reinterpret_cast<const float2*>(vrow[h]);   // [coordinate][10 frame pairs]
@@ -761,18 +771,14 @@ __global__ void __launch_bounds__(kSkinTcThreads, 1) lbs_skin_tc_kernel(SmplDev 
         o0[p] = odd ? part[2] : part[0];
         o1[p] = part[1];
       }
-      const bool v_ok = gv[h] < kV;
-      if (v_ok && (vertices || ci[h] >= 0)) {
+      if (orow[h] >= 0) {
 #pragma unroll
         for (int p = 0; p < kSkF / 2; ++p)
 #pragma unroll
           for (int k = 0; k < 2; ++k) {
             if (k == 1 && odd) continue;                               // even lanes store j = 0, 1; odd lanes j = 2
             const int fl = ftile * kSkF + 2 * p + sf[k];               // local frame-person index
-            if (fl < n) {
-              if (vertices) vertices[((size_t)fl * kV + gv[h]) * 3 + srow[k]] = k ? o1[p] : o0[p];
-              if (ci[h] >= 0) w.vcompact[((size_t)fl * m.S + ci[h]) * 3 + srow[k]] = k ? o1[p] : o0[p];
-            }
+            if (fl < n) out[(size_t)fl * fstride + orow[h] + srow[k]] = k ? o1[p] : o0[p];
           }
       }
     }
@@ -876,7 +882,7 @@ static int lbs_set_attrs() {
   return GLAMR_OK;
 }
 // SMs of the device: the persistent LBS GEMM kernels launch at most one CTA per SM
-static int device_sms() {
+int smpl_device_sms() {
   static int sms = 0;
   if (sms <= 0) {
     int dev = 0;
@@ -888,22 +894,26 @@ static int device_sms() {
 static int launch_blend_gemm(const SmplDev& m, int n, const SmplWorkspace& w, cudaStream_t s, bool pdl) {
   const int mtiles = (n + kTcM - 1) / kTcM;
   const int half_last = (n - (mtiles - 1) * kTcM <= kTcM / 2) ? 1 : 0;
-  const dim3 grid(min(device_sms(), kTcNTiles * mtiles));
+  const int ntn = w.vp_tiled ? m.tc_ntiles : kTcNTiles;     // the support columns feed the tensor-core skinning only
+  const dim3 grid(min(smpl_device_sms(), ntn * mtiles));
   if (pdl) {
-    GLAMR_CUDA_TRY(launch_pdl(4, lbs_blend_tc_kernel, grid, dim3(kTcThreads), kTcSmemBytes, s, m, w, 0, mtiles, half_last));
+    GLAMR_CUDA_TRY(launch_pdl(4, lbs_blend_tc_kernel, grid, dim3(kTcThreads), kTcSmemBytes, s, m, w, 0, mtiles, half_last, ntn));
     return GLAMR_OK;
   }
-  lbs_blend_tc_kernel<<<grid, kTcThreads, kTcSmemBytes, s>>>(m, w, 0, mtiles, half_last);
+  lbs_blend_tc_kernel<<<grid, kTcThreads, kTcSmemBytes, s>>>(m, w, 0, mtiles, half_last, ntn);
   GLAMR_LAUNCH_CHECK();
   return GLAMR_OK;
 }
-static int launch_skin_tc(const SmplDev& m, int n, const SmplWorkspace& w, float* vertices, cudaStream_t s, bool pdl) {
-  const dim3 grid(min(device_sms(), kNVTiles * ((n + kSkF - 1) / kSkF)));
+// vertex tiles [vt0, vt1) on at most max_ctas CTAs
+static int launch_skin_tc(const SmplDev& m, int n, const SmplWorkspace& w, float* vertices, cudaStream_t s, bool pdl, int vt0, int vt1,
+                          int max_ctas) {
+  if (vt1 <= vt0) return GLAMR_OK;
+  const dim3 grid(max(1, min(max_ctas, (vt1 - vt0) * ((n + kSkF - 1) / kSkF))));
   if (pdl) {
-    GLAMR_CUDA_TRY(launch_pdl(4, lbs_skin_tc_kernel, grid, dim3(kSkinTcThreads), kSkinTcSmemBytes, s, m, n, w, vertices));
+    GLAMR_CUDA_TRY(launch_pdl(4, lbs_skin_tc_kernel, grid, dim3(kSkinTcThreads), kSkinTcSmemBytes, s, m, n, w, vertices, vt0, vt1));
     return GLAMR_OK;
   }
-  lbs_skin_tc_kernel<<<grid, kSkinTcThreads, kSkinTcSmemBytes, s>>>(m, n, w, vertices);
+  lbs_skin_tc_kernel<<<grid, kSkinTcThreads, kSkinTcSmemBytes, s>>>(m, n, w, vertices, vt0, vt1);
   GLAMR_LAUNCH_CHECK();
   return GLAMR_OK;
 }
@@ -922,11 +932,11 @@ int launch_blend(const SmplDev& m, int n, const float* body_pose, const float* b
   return GLAMR_OK;
 }
 // skinning of local frame-persons [0, n) from the workspace's v_posed and A
-int launch_skin(const SmplDev& m, int n, const SmplWorkspace& w, float* vertices, cudaStream_t s) {
+int launch_skin(const SmplDev& m, int n, const SmplWorkspace& w, float* vertices, cudaStream_t s, int vt0, int vt1, int max_ctas) {
   if (n <= 0) return GLAMR_OK;
   int rc;
   if ((rc = lbs_set_attrs())) return rc;
-  if (w.vp_tiled) return launch_skin_tc(m, n, w, vertices, s, false);
+  if (w.vp_tiled) return launch_skin_tc(m, n, w, vertices, s, false, vt0, vt1, max_ctas);
   dim3 grid(kNVTiles, (n + kFramesPerCta - 1) / kFramesPerCta);
   if (m.K == 4) lbs_skin_kernel<4><<<grid, kLbsThreads, kSkinSmemBytes, s>>>(m, 0, n, w, vertices);
   else lbs_skin_kernel<0><<<grid, kLbsThreads, kSkinSmemBytes, s>>>(m, 0, n, w, vertices);
@@ -957,7 +967,8 @@ int launch_lbs(const SmplDev& m, int n_begin, int n_end, const float* betas, con
   if (path >= 1 && m.tcB && w.tcA && n_begin == 0) {
     int rc;
     if ((rc = launch_blend_gemm(m, n_end, w, s, pdl))) return rc;
-    if (w.vp_tiled) return launch_skin_tc(m, n_end, w, vertices, s, pdl);
+    // mesh and support tiles in one launch: the joints come from vcompact
+    if (w.vp_tiled) return launch_skin_tc(m, n_end, w, vertices, s, pdl, 0, m.sk_tiles, smpl_device_sms());
     if (pdl) {
       if (m.K == 4) GLAMR_CUDA_TRY(launch_pdl(4, lbs_skin_kernel<4>, grid, dim3(kLbsThreads), kSkinSmemBytes, s, m, n_begin, n_end, w, vertices));
       else GLAMR_CUDA_TRY(launch_pdl(4, lbs_skin_kernel<0>, grid, dim3(kLbsThreads), kSkinSmemBytes, s, m, n_begin, n_end, w, vertices));
@@ -1061,6 +1072,32 @@ extern "C" int glamr_smpl_create(glamr_smpl_t** out, const float* v_template, co
   }
   d.n_extra = n_extra; d.n_picks = n_picks; d.n_map = n_map;
   int rc = GLAMR_OK;
+  std::vector<int32_t> sup;                  // support vertex of each slot
+  {  // support list (first, the LBS images below copy its vertices) + CSR of the extra regressor
+    std::vector<int32_t> cov(kVPad, -1);
+    auto touch = [&](int v) { if (cov[v] < 0) { cov[v] = (int32_t)sup.size(); sup.push_back(v); } };
+    for (int k = 0; k < n_picks; ++k) touch(pick_vertex_ids[k]);
+    std::vector<int32_t> ptr(n_extra + 1, 0), ci;
+    std::vector<float> rw;
+    for (int r = 0; r < n_extra; ++r) {
+      for (int v = 0; v < kV; ++v) {
+        const float wv = J_regressor_extra[(size_t)r * kV + v];
+        if (wv != 0.0f) { touch(v); ci.push_back(cov[v]); rw.push_back(wv); }
+      }
+      ptr[r + 1] = (int32_t)ci.size();
+    }
+    if (ci.empty()) { ci.push_back(0); rw.push_back(0.0f); }
+    if (sup.empty()) touch(0);
+    d.S = (int)sup.size();
+    std::vector<int32_t> pci(n_picks > 0 ? n_picks : 1, 0), jm(joint_map, joint_map + n_map);
+    for (int k = 0; k < n_picks; ++k) pci[k] = cov[pick_vertex_ids[k]];
+    if ((rc = upload(h, cov, &d.compact_of_vertex))) goto fail;
+    if ((rc = upload(h, ptr, &d.reg_ptr))) goto fail;
+    if ((rc = upload(h, ci, &d.reg_ci))) goto fail;
+    if ((rc = upload(h, rw, &d.reg_w))) goto fail;
+    if ((rc = upload(h, pci, &d.pick_ci))) goto fail;
+    if ((rc = upload(h, jm, &d.joint_map))) goto fail;
+  }
   {  // posedirs -> [tile][k][384]
     std::vector<float> t((size_t)kNVTiles * kPF * kTileCols, 0.0f);
     for (int tile = 0; tile < kNVTiles; ++tile)
@@ -1094,11 +1131,16 @@ extern "C" int glamr_smpl_create(glamr_smpl_t** out, const float* v_template, co
     if (amax > 0.0f && std::isfinite(amax)) std::frexp(amax, &ex);            // amax in [2^(ex-1), 2^ex)
     const int e_B = amax > 0.0f && std::isfinite(amax) ? 15 - ex : 0;
     d.tcB_unscale = std::ldexp(1.0f, -e_B);
-    std::vector<__half> img((size_t)kTcNTiles * kTcChunks * kTcBStageHalves, __float2half_rn(0.0f));
-    for (int col = 0; col < kV * 3; ++col) {
+    // columns past the mesh's 20736: the support vertices' columns again (slot s, coordinate c at 20736 + 3 s + c), so the GEMM blends
+    // them a second time where the support tiles of the skinning read them; copies leave max |basis| and e_B as they are
+    d.tc_ntiles = smpl_vp_cols(d.S) / kTcN;
+    std::vector<__half> img((size_t)d.tc_ntiles * kTcChunks * kTcBStageHalves, __float2half_rn(0.0f));
+    for (int col = 0; col < kTcCols + 3 * d.S; ++col) {
+      if (col >= kV * 3 && col < kTcCols) continue;
+      const int src = col < kTcCols ? col : sup[(col - kTcCols) / 3] * 3 + (col - kTcCols) % 3;
       const int tile = col / kTcN, r = col % kTcN;
       for (int k = 0; k < kTcFeat; ++k) {
-        const float v = std::ldexp(basis(col, k), e_B);
+        const float v = std::ldexp(basis(src, k), e_B);
         const __half hi = __float2half_rn(v), lo = __float2half_rn(v - __half2float(hi));
         __half* q = &img[((size_t)tile * kTcChunks + (k >> 4)) * kTcBStageHalves + ((((k >> 3) & 1) * kTcN + r) * 8) + (k & 7)];
         q[0] = hi;
@@ -1106,13 +1148,17 @@ extern "C" int glamr_smpl_create(glamr_smpl_t** out, const float* v_template, co
       }
     }
     if ((rc = upload(h, img, &d.tcB))) goto fail;
-    // dense skinning weights W[v][24] as the A operand of the tensor-core skinning: per 128-vertex tile [hi | lo][joint group][vertex][4]
-    std::vector<float> wimg((size_t)kNVTiles * kSkWImageFloats, 0.0f);
-    for (int v = 0; v < kV; ++v)
+    // dense skinning weights W[v][24] as the A operand of the tensor-core skinning: per 128-vertex tile [hi | lo][joint group][vertex][4];
+    // row kVPad + s (support tile s / 128) holds the weights of support vertex s
+    d.sk_tiles = kNVTiles + smpl_sup_tiles(d.S);
+    std::vector<float> wimg((size_t)d.sk_tiles * kSkWImageFloats, 0.0f);
+    for (int row = 0; row < kVPad + d.S; ++row)
       for (int j = 0; j < kNJ; ++j) {
+        if (row >= kV && row < kVPad) break;
+        const int v = row < kVPad ? row : sup[row - kVPad];
         const float x = lbs_weights[(size_t)v * kNJ + j];
         const float hi = tf32_rna(x), lo = tf32_rna(x - hi);
-        float* q = &wimg[(size_t)(v / kVTile) * kSkWImageFloats + ((size_t)(j >> 2) * kVTile + v % kVTile) * 4 + (j & 3)];
+        float* q = &wimg[(size_t)(row / kVTile) * kSkWImageFloats + ((size_t)(j >> 2) * kVTile + row % kVTile) * 4 + (j & 3)];
         q[0] = hi;
         q[kSkWHalf] = lo;
       }
@@ -1163,31 +1209,6 @@ extern "C" int glamr_smpl_create(glamr_smpl_t** out, const float* v_template, co
     }
     if ((rc = upload(h, sw, &d.skin_w))) goto fail;
     if ((rc = upload(h, sj, &d.skin_j))) goto fail;
-  }
-  {  // support list + CSR of the extra regressor
-    std::vector<int32_t> cov(kVPad, -1), sup;
-    auto touch = [&](int v) { if (cov[v] < 0) { cov[v] = (int32_t)sup.size(); sup.push_back(v); } };
-    for (int k = 0; k < n_picks; ++k) touch(pick_vertex_ids[k]);
-    std::vector<int32_t> ptr(n_extra + 1, 0), ci;
-    std::vector<float> rw;
-    for (int r = 0; r < n_extra; ++r) {
-      for (int v = 0; v < kV; ++v) {
-        const float wv = J_regressor_extra[(size_t)r * kV + v];
-        if (wv != 0.0f) { touch(v); ci.push_back(cov[v]); rw.push_back(wv); }
-      }
-      ptr[r + 1] = (int32_t)ci.size();
-    }
-    if (ci.empty()) { ci.push_back(0); rw.push_back(0.0f); }
-    if (sup.empty()) touch(0);
-    d.S = (int)sup.size();
-    std::vector<int32_t> pci(n_picks > 0 ? n_picks : 1, 0), jm(joint_map, joint_map + n_map);
-    for (int k = 0; k < n_picks; ++k) pci[k] = cov[pick_vertex_ids[k]];
-    if ((rc = upload(h, cov, &d.compact_of_vertex))) goto fail;
-    if ((rc = upload(h, ptr, &d.reg_ptr))) goto fail;
-    if ((rc = upload(h, ci, &d.reg_ci))) goto fail;
-    if ((rc = upload(h, rw, &d.reg_w))) goto fail;
-    if ((rc = upload(h, pci, &d.pick_ci))) goto fail;
-    if ((rc = upload(h, jm, &d.joint_map))) goto fail;
   }
   *out = h;
   return GLAMR_OK;

@@ -9,12 +9,16 @@ struct SmplDev {
   // dense constants
   const float* pd_tiles;     // [54][207][384]  posedirs, vertex-tile major: one contiguous 13,824 B block per
                              //                 (tile, 9-row chunk) so a CTA streams its slab with 1-D bulk TMA
-  const __half* tcB;         // [81 col tiles][14 K chunks][hi | lo][2 K groups][256 cols][8]  the blend basis (posedirs | shapedirs |
+  const __half* tcB;         // [tc_ntiles col tiles][14 K chunks][hi | lo][2 K groups][256 cols][8]  the blend basis (posedirs | shapedirs |
                              //                 v_template) scaled by 2^e_B, pre-split into fp16 hi / lo and pre-tiled as the wgmma K-major
-                             //                 core-matrix image: one contiguous 16 KB block per (tile, chunk) = one bulk copy per stage
+                             //                 core-matrix image: one contiguous 16 KB block per (tile, chunk) = one bulk copy per stage;
+                             //                 the 81 mesh tiles are followed by copies of the support vertices' columns (smpl_vp_cols)
   float tcB_unscale;         // 2^-e_B
-  const float* skW;          // [54 vertex tiles][hi | lo][6 joint groups][128 vertices][4]  dense skinning weights W[v][24], tf32 hi / lo,
-                             //                 wgmma K-major image: one contiguous 24 KB block per vertex tile (lbs_skin_tc_kernel)
+  int tc_ntiles;             // column tiles of tcB: smpl_vp_cols(S) / 256
+  const float* skW;          // [sk_tiles][hi | lo][6 joint groups][128 vertices][4]  dense skinning weights W[v][24], tf32 hi / lo,
+                             //                 wgmma K-major image: one contiguous 24 KB block per vertex tile (lbs_skin_tc_kernel);
+                             //                 the 54 mesh tiles are followed by the support tiles (slot s = support vertex s)
+  int sk_tiles;              // vertex tiles of skW: kNVTiles + smpl_sup_tiles(S)
   const float* v_template;   // [6912][3]  (padded with zeros)
   const float* shapedirs;    // [6912][30] ([v][c][l] as in the model file)
   const float* j_template;   // [24][3]    J_regressor @ v_template
@@ -46,7 +50,7 @@ struct SmplWorkspace {
   __half* tcA;      // [n/128][14][hi | lo][2][128][8]  blend features (pose feature | betas | 1 | 0-pad), row f scaled by 2^e_f, fp16
                     //              hi / lo, wgmma image per (128-frame tile, K chunk): 8 KB contiguous = one bulk copy per stage
   float* tcUnscale; // [mpad]  2^-e_f of each feature row
-  float* vpT;       // [20736][mpad]  blended vertices v_posed, TRANSPOSED (column-major over frames) so that the skinning kernel's
+  float* vpT;       // [vp_cols][mpad]  blended vertices v_posed, TRANSPOSED (column-major over frames) so that the skinning kernel's
                     //              lanes = frames read 128 contiguous bytes per vertex coordinate
   int mpad;         // frames padded to a multiple of 128
   float* skB;       // [ceil(mpad/20)][hi | lo][6 joint groups][20 frames x 12][4]  the relative joint transforms as the B operand of the
@@ -54,9 +58,17 @@ struct SmplWorkspace {
   float* vpT2;      // always NULL, see vp_buffer()
   const double* flip_src;
   int flip_add;
-  int vp_tiled;     // 1: v_posed is stored frame-tiled for lbs_skin_tc_kernel: [ceil(mpad/20)][20736 cols][20 frames] (the 128 vertices x
+  int vp_tiled;     // 1: v_posed is stored frame-tiled for lbs_skin_tc_kernel: [ceil(mpad/20)][vp_cols][20 frames] (the 128 vertices x
                     //    20 frames of a skinning tile are one contiguous 30,720 B block = one bulk copy); 0: vpT as described above
+  int vp_cols;      // columns of v_posed: the 20736 of the mesh, then the support vertices' copies (smpl_vp_cols)
 };
+
+// The support vertices (the S vertices the optimiser reads, compacted) are skinned as vertex tiles of their own after the 54 mesh
+// tiles: support tile t holds support slots 128 t .. 128 t + 127.  Their blend-basis columns are copied after the 20736 mesh columns
+// (slot s, coordinate c at column 20736 + 3 s + c), rounded up to whole 256-column GEMM tiles and at least as far as the last support
+// tile's 384-column v_posed block reaches, so that support tile t reads its block at column 20736 + 384 t just like a mesh tile.
+inline int smpl_sup_tiles(int S) { return (S + kVTile - 1) / kVTile; }
+inline int smpl_vp_cols(int S) { return (kTcCols + smpl_sup_tiles(S) * kTileCols + kTcN - 1) / kTcN * kTcN; }
 
 // FK only (glamr_smpl_fk24): the kinematic-chain scratch without the blend operands (they are carved last)
 inline size_t smpl_workspace_floats_fk(int n, int S) {
@@ -67,7 +79,7 @@ inline size_t smpl_workspace_floats(int n, int S) {
   const size_t n32 = ((size_t)n + 31) / 32 * 32;   // the pose feature is tile-major over whole 32-frame tiles
   const size_t n128 = ((size_t)n + kTcM - 1) / kTcM * kTcM;
   return (size_t)n * (kNJ * 3 + (size_t)S * 3 + 3) + n32 * (kPFPad + kNJ * 12) + 64 + 64 +
-         (n128 / kTcM) * kTcChunks * kTcAStageHalves / 2 + n128 + (size_t)kTcCols * ((n128 + kSkF - 1) / kSkF * kSkF) +
+         (n128 / kTcM) * kTcChunks * kTcAStageHalves / 2 + n128 + (size_t)smpl_vp_cols(S) * ((n128 + kSkF - 1) / kSkF * kSkF) +
          ((n128 + kSkF - 1) / kSkF) * kSkBImageFloats + 64;
 }
 int lbs_path();                              // 2 tensor-core blend + tensor-core skinning, 1 tensor-core blend + SIMT skinning, 0 one-kernel FP32 SIMT path
@@ -84,8 +96,9 @@ inline SmplWorkspace smpl_carve_workspace(void* base, int n, int S) {
   w.tcA = reinterpret_cast<__half*>(p); p += (size_t)(w.mpad / kTcM) * kTcChunks * kTcAStageHalves / 2;
   w.tcUnscale = p; p += w.mpad;
   w.skB = p; p += (size_t)((w.mpad + kSkF - 1) / kSkF) * kSkBImageFloats;
-  w.vpT = p;                                   // [20736][mpad] or, frame-tiled, [ceil(mpad/20)][20736][20]
+  w.vpT = p;                                   // [vp_cols][mpad] or, frame-tiled, [ceil(mpad/20)][vp_cols][20]
   w.vp_tiled = lbs_path() == 2 ? 1 : 0;
+  w.vp_cols = smpl_vp_cols(S);
   w.vpT2 = nullptr; w.flip_src = nullptr; w.flip_add = 0;
   return w;
 }
@@ -256,7 +269,10 @@ int launch_lbs(const SmplDev& m, int n_begin, int n_end, const float* betas, con
 // tensor-core path in two halves (the optimiser pipelines them: the blend depends on body pose / betas only)
 int launch_blend(const SmplDev& m, int n, const float* body_pose, const float* betas, const SmplWorkspace& w, cudaStream_t s,
                  bool features = true, bool gemm = true);
-int launch_skin(const SmplDev& m, int n, const SmplWorkspace& w, float* vertices, cudaStream_t s);
+// skinning of the vertex tiles [vt0, vt1) (tensor-core path; mesh tiles < kNVTiles <= support tiles < m.sk_tiles) on at most max_ctas
+// CTAs; the SIMT skinning (vp_tiled == 0) always skins the whole mesh
+int launch_skin(const SmplDev& m, int n, const SmplWorkspace& w, float* vertices, cudaStream_t s, int vt0, int vt1, int max_ctas);
+int smpl_device_sms();                       // SMs of the current device
 int lbs_kernel_count(const SmplDev& m);      // kernels one launch_lbs call launches
 int launch_joints_finalize(const SmplDev& m, int n, int orig_joints, const float* root_trans, const float* root_scale,
                            const SmplWorkspace& w, float* joints, cudaStream_t s);

@@ -282,15 +282,18 @@ int glamr_opt_losses(glamr_opt_t* st, const float* reduce_buf, float* loss_terms
  * multi-GPU loop of global_recon_model.py:558-569): the pipelined side-stream work is joined by that apply call, not at the end of this one */
 int glamr_opt_backward_for_apply(glamr_opt_t* st, const float* theta, float* reduce_buf, void* stream);
 int glamr_opt_kernel_timing(glamr_opt_t* st, int enable);
-/* the last timed evaluation split into the critical-path kernel (skinning; whole LBS kernel on the SIMT path) and the side-stream blend */
+/* the last timed evaluation's LBS split into the critical-path kernel (the support vertices' skinning on the tensor-core path, the
+ * whole skinning with tcblend, the whole LBS kernel on the SIMT path) and the side stream's part (mesh skinning + blend on the
+ * tensor-core path, the blend with tcblend, 0 on the SIMT path) */
 int glamr_opt_last_lbs_parts_ms(glamr_opt_t* st, float* critical_ms, float* blend_ms);
 /* mean ms of the blend (feature kernel + tcgen05 GEMM) of this rank's frame-persons launched ALONE `reps` times (synchronises;
  * GLAMR_EUNSUPPORTED on the SIMT path or before the first evaluation) */
 int glamr_opt_time_blend(glamr_opt_t* st, int reps, float* ms);
 int glamr_opt_last_lbs_ms(glamr_opt_t* st, float* ms);
 /* enable == 2: also record an event after every launch; durations (ms) between consecutive marks of the last
- * backward (+ apply) sequence: memset, traj_fwd, cam_fwd, pose_prep, lbs, joints, residuals, cam_bwd[, scatter], traj_bwd,
- * reduce[, losses, adam, advance] */
+ * backward (+ apply) sequence on the caller's stream: traj_fwd, cam_fwd, pose_prep, skinning (the support vertices' on the
+ * tensor-core path), residuals[, cam_bwd + scatter], traj_bwd, apply; on the tensor-core path two more follow, measured on the side
+ * stream: the mesh skinning and the blend after it (features + GEMM) */
 int glamr_opt_kernel_times(glamr_opt_t* st, float* ms, int* n);
 
 enum glamr_read {

@@ -21,6 +21,9 @@ lib = m._lib
 def it():      # the library's single-GPU iteration (backward kernels, then apply_kernel), eager so that events can sit between launches
     L.check(lib.glamr_opt_iterate(m._opt, L.ptr(m._theta), L.ptr(m._reduce), float(specs['opt_lr']), L.ptr(hist), L.NUM_TERMS + 1, 1, 0, L.stream_ptr()), 'iterate')
 for _ in range(5): it()
+# the caller's stream: traj_fwd, cam_fwd, pose_prep, skinning, residuals[, cam_bwd + scatter], traj_bwd, apply
+ms_labels = ['traj_fwd', 'cam_fwd', 'pose_prep', 'skin', 'residuals'] + (['cam_bwd'] if m._pb.cam_mode == L.CAM_FROM_PERSONS else []) + \
+    ['traj_bwd', 'apply']
 L.check(lib.glamr_opt_kernel_timing(m._opt, 2), 't')
 acc = None
 for _ in range(50):
@@ -29,4 +32,7 @@ for _ in range(50):
     L.check(lib.glamr_opt_kernel_times(m._opt, ms, ctypes.byref(n)), 'times')
     v = np.array(ms[:n.value]); acc = v if acc is None else acc + v
 acc = acc / 50 * 1000
-print(f'P={P} T={T} {cfgid}:{stage}  per-segment us:', np.round(acc, 1).tolist(), 'sum', round(float(acc.sum()), 1))
+side = 2 if n.value > len(ms_labels) else 0     # the tensor-core path appends the side stream's mesh skinning and blend
+main = acc[:len(acc) - side]
+print(f'P={P} T={T} {cfgid}:{stage}  per-segment us:', np.round(main, 1).tolist(), 'sum', round(float(main.sum()), 1),
+      '| side stream (mesh skinning, blend):', np.round(acc[len(main):], 1).tolist())
