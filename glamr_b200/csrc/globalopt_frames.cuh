@@ -241,6 +241,15 @@ GLAMR_HD void mat34_mul(const float* A, const float* B, float* o) {
     }
   }
 }
+// person2cam @ make_transform(person2cam_res_rot, person2cam_res_trans, '6d') of one person at frame s (:484-488).  At the
+// initial residuals (identity 6d, zero translation) every product is with 1 or 0, so the result is person2cam bit for bit.
+GLAMR_HD void person2cam_with_residual(const OptCtx& c, const glamr_person_t& ps, int s, float* P2C) {
+  float R[9];
+  rot6d_to_rotmat(c.theta + ps.off_p2c_rot + 6 * s, R);
+  const float* tr = c.theta + ps.off_p2c_trans + 3 * s;
+  const float E[12] = {R[0], R[1], R[2], tr[0], R[3], R[4], R[5], tr[1], R[6], R[7], R[8], tr[2]};
+  mat34_mul(ps.person2cam + (size_t)s * 12, E, P2C);
+}
 // mean over visible persons of person_transform_world @ person2cam at source frame s  (:482-492)
 GLAMR_HD void mean_cam_inv(const OptCtx& c, int s, float* M) {
 #pragma unroll
@@ -250,7 +259,13 @@ GLAMR_HD void mean_cam_inv(const OptCtx& c, int s, float* M) {
     if (ps.vis[s] == 0.0f) continue;
     float Tw[12], C[12];
     person_world_transform(c, p, s, Tw);
-    mat34_mul(Tw, ps.person2cam + (size_t)s * 12, C);
+    if (c.pb.has_person2cam) {
+      float P2C[12];
+      person2cam_with_residual(c, ps, s, P2C);
+      mat34_mul(Tw, P2C, C);
+    } else {
+      mat34_mul(Tw, ps.person2cam + (size_t)s * 12, C);
+    }
 #pragma unroll
     for (int k = 0; k < 12; ++k) M[k] += C[k];
   }
@@ -838,7 +853,8 @@ GLAMR_HD void camera_backward(const OptCtx& c, int t, TermAcc& acc) {
   }
 }
 // mode 3 only, after camera_backward of all frames: frame s gathers dL/d(mean) of every frame filled from it and
-// pushes it into dL/d(person_transform_world) of its visible persons.
+// pushes it into dL/d(person_transform_world) of its visible persons and, with has_person2cam, into their person2cam
+// residuals at frame s (a person invisible at s gets none: the reference multiplies its term by vis_frames).
 GLAMR_HD void camera_scatter_to_persons(const OptCtx& c, int s) {
   const glamr_problem_t& pb = c.pb;
   const int T = pb.T;
@@ -858,15 +874,34 @@ GLAMR_HD void camera_scatter_to_persons(const OptCtx& c, int s) {
     if (ps.vis[s] == 0.0f) continue;
     // M = Tw @ P2C: R_M = Rw Rp, t_M = Rw tp + tw  ->  dRw = G_R Rp^T + G_t tp^T, dtw = G_t
     const float* P2C = ps.person2cam + (size_t)s * 12;
-    float Rp[9], gRw[9], g[3];
-    mat34_R(P2C, Rp);
+    const size_t n = (size_t)p * T + s;
+    float Rp[9], gRw[9], g[3], tp[3];
+    if (pb.has_person2cam) {
+      float P2Cr[12];
+      person2cam_with_residual(c, ps, s, P2Cr);
+      mat34_R(P2Cr, Rp);
+      tp[0] = P2Cr[3]; tp[1] = P2Cr[7]; tp[2] = P2Cr[11];
+      // P2C' = P2C @ [Rr | tr]: with Q = Tw @ P2C,  dRr = R_Q^T G_R,  dtr = R_Q^T G_t
+      float Rw[9], Rp0[9], RQ[9], gRr[9], g6[6], gtr[3];
+      aa_to_rotmat(c.sc.orient_world + n * 3, Rw);
+      mat34_R(P2C, Rp0);
+      mat3_mul(Rw, Rp0, RQ);
+      mat3_tmul(RQ, G, gRr);
+      mat3_tvec(RQ, G + 9, gtr);
+      rot6d_to_rotmat_vjp(c.theta + ps.off_p2c_rot + 6 * s, gRr, g6);
+#pragma unroll
+      for (int k = 0; k < 6; ++k) c.sc.grad[ps.off_p2c_rot + 6 * s + k] = g6[k];
+#pragma unroll
+      for (int k = 0; k < 3; ++k) c.sc.grad[ps.off_p2c_trans + 3 * s + k] = gtr[k];
+    } else {
+      mat34_R(P2C, Rp);
+      tp[0] = P2C[3]; tp[1] = P2C[7]; tp[2] = P2C[11];
+    }
     mat3_mult(G, Rp, gRw);
-    const float tp[3] = {P2C[3], P2C[7], P2C[11]};
 #pragma unroll
     for (int a = 0; a < 3; ++a)
 #pragma unroll
       for (int b = 0; b < 3; ++b) gRw[a * 3 + b] += G[9 + a] * tp[b];
-    const size_t n = (size_t)p * T + s;
     aa_to_rotmat_vjp(c.sc.orient_world + n * 3, gRw, g);
 #pragma unroll
     for (int k = 0; k < 3; ++k) { c.sc.g_orient[n * 3 + k] += g[k]; c.sc.g_trans[n * 3 + k] += G[9 + k]; }

@@ -19,11 +19,12 @@ from . import lib as L
 
 
 class VariableLayout:
-    def __init__(self, T, n_empty, trans_res_rows, lens, heading_dim=1, world_dxy=False):
+    def __init__(self, T, n_empty, trans_res_rows, lens, heading_dim=1, world_dxy=False, person2cam=False):
         """heading_dim 2: heading_type 'vec' (traj_local_heading [2], traj_local_dheading [L-1,2]); world_dxy: every person also
-        gets a world_dxy [T,2] block (only when a stage can create it, so other problems keep their layout)"""
+        gets a world_dxy [T,2] block (only when a stage can create it, so other problems keep their layout); person2cam: every
+        person also gets person2cam_res_rot [T,6] and person2cam_res_trans [T,3] (only when init_data creates them)"""
         self.T, self.n_empty, self.trans_res_rows, self.lens = T, n_empty, trans_res_rows, list(lens)
-        self.heading_dim, self.world_dxy = heading_dim, bool(world_dxy)
+        self.heading_dim, self.world_dxy, self.person2cam = heading_dim, bool(world_dxy), bool(person2cam)
         hd = heading_dim
         off = 0
 
@@ -39,7 +40,8 @@ class VariableLayout:
         for Ln in self.lens:
             self.persons.append(dict(xy=take(2), heading=take(hd), dxy=take(2 * (Ln - 1)), dheading=take(hd * (Ln - 1)), z=take(Ln),
                                      rot=take(6 * Ln), world_dheading=take(T), orient_res=take(3 * T), trans_res=take(3 * T),
-                                     world_dxy=take(2 * T if self.world_dxy else 0)))
+                                     world_dxy=take(2 * T if self.world_dxy else 0),
+                                     p2c_rot=take(6 * T if self.person2cam else 0), p2c_trans=take(3 * T if self.person2cam else 0)))
         self.n_params = off
 
     def views(self, theta, p=None):
@@ -61,6 +63,9 @@ class VariableLayout:
                'root_trans_world_res': v('trans_res', 3 * T, T, 3)}
         if self.world_dxy:
             out['world_dxy'] = v('world_dxy', 2 * T, T, 2)
+        if self.person2cam:
+            out['person2cam_res_rot'] = v('p2c_rot', 6 * T, T, 6)
+            out['person2cam_res_trans'] = v('p2c_trans', 3 * T, T, 3)
         return out
 
 
@@ -74,8 +79,8 @@ class StageCompiler:
     def __init__(self, data, layout, flags, device, aa_to_rot6d, num_joints=26, aa_to_quat=None):
         """flags: dict with flag_fixed_cam, flag_opt_cam, flag_opt_cam_from_person_pose, flag_cam_inv_trans_res_all,
         flag_opt_vis_local_rot, cam_fix_frames and optionally flag_opt_traj / traj_source (when absent they are read off
-        `data`: a predicted trajectory leaves traj_local_pred, flag_opt_traj leaves the world_res variables) and heading_vec
-        (heading_type 'vec'; default: the layout's heading size).
+        `data`: a predicted trajectory leaves traj_local_pred, flag_opt_traj leaves the world_res variables), heading_vec
+        (heading_type 'vec'; default: the layout's heading size) and flag_opt_person2cam_rot / _trans (default false).
         aa_to_rot6d: callable (device math lives in the CUDA library)."""
         self.data, self.layout, self.flags, self.device, self.J = data, layout, flags, device, num_joints
         self.pids = list(data['person_data'].keys())
@@ -202,6 +207,9 @@ class StageCompiler:
     def compile(self, theta, opt_variables, loss_cfg, stage, n_begin=0, n_end=None, owner=True):
         data, lay, fl, dev, P, T, J = self.data, self.layout, self.flags, self.device, self.P, self.T, self.J
         n_end = P * T if n_end is None else n_end
+        if 'person2cam_res_trans_reg' in loss_cfg:           # loss_func.py:244-245
+            raise ValueError("residual 'person2cam_res_trans_reg' reads data['person2cam_res_trans'], a key the reference never creates "
+                             "(the residuals live per person), so the reference fails with KeyError; it has no defined meaning to implement")
         for name in loss_cfg:
             if name not in L.TERM_INDEX:
                 raise NotImplementedError(f"residual '{name}' has no CUDA implementation (no CPU fallback)")
@@ -241,6 +249,18 @@ class StageCompiler:
                              "no world_dheading: otherwise the reference adds world_dxy in place to a base it never re-creates, and "
                              "its second backward fails (autograd graph already freed)")
         pb.has_world_dxy, pb.world_dxy_alias = int(has_dxy), int(alias)
+        # person2cam residuals (:173-175,484-488,616-619): created by init_data with flag_opt_traj, then composed into every
+        # camera-from-persons forward; Adam moves them only in stages that list them
+        p2c_flags = {'person2cam_rot': fl.get('flag_opt_person2cam_rot', False), 'person2cam_trans': fl.get('flag_opt_person2cam_trans', False)}
+        if any(p2c_flags.values()) and not self.opt_traj:
+            listed = [k for k, f in p2c_flags.items() if f and k in opt_variables]
+            if listed:
+                raise ValueError(f"optimisation variable '{listed[0]}' needs flag_opt_traj: the person2cam residuals are created only with "
+                                 "it, so the reference's get_parameter fails with KeyError")
+            if mode == L.CAM_FROM_PERSONS:
+                raise ValueError('flag_opt_person2cam_rot / _trans need flag_opt_traj when the camera comes from the persons: the '
+                                 "residuals are created only with flag_opt_traj, so the reference's forward fails with KeyError")
+        pb.has_person2cam = int(lay.person2cam)
         # combinations the reference fails on (KeyError / None.items() in get_parameter or loss_func.py): fail clearly here
         if not self.has_local:
             for key in opt_variables:
@@ -276,6 +296,7 @@ class StageCompiler:
             ps.off_xy, ps.off_heading, ps.off_dxy, ps.off_dheading = o['xy'], o['heading'], o['dxy'], o['dheading']
             ps.off_z, ps.off_rot, ps.off_world_dheading = o['z'], o['rot'], o['world_dheading']
             ps.off_orient_res, ps.off_trans_res, ps.off_world_dxy = o['orient_res'], o['trans_res'], o['world_dxy']
+            ps.off_p2c_rot, ps.off_p2c_trans = o['p2c_rot'], o['p2c_trans']
             for name in ['traj_local_pred', 'orient_base_init', 'trans_base_init', 'cam_K', 'kp_target', 'orient_cam_6d',
                          'orient_cam_q', 'trans_cam', 'person2cam', 'dheading_mask', 'rot_mask', 'vis', 'world_dxy_base']:
                 setattr(ps, name, None if c[name] is None else c[name].data_ptr())
@@ -371,8 +392,12 @@ class StageCompiler:
                     on(o['world_dheading'], T)
                 if key == 'world_dxy' and self.opt_traj:          # without flag_opt_traj the forward never reads it (:451)
                     on(o['world_dxy'], 2 * T)
-                if key in ('person2cam_rot', 'person2cam_trans'):
-                    raise NotImplementedError(f"optimisation variable '{key}' is not implemented in the CUDA path")
+                # with the flag and flag_opt_traj (get_parameter, :616-619); a stage whose forward never reads them ('cam' listed, or
+                # 'init') gives them a zero gradient, which leaves them unchanged like torch's Adam skipping a grad of None
+                if key == 'person2cam_rot' and p2c_flags[key] and lay.person2cam:
+                    on(o['p2c_rot'], 6 * T)
+                if key == 'person2cam_trans' and p2c_flags[key] and lay.person2cam:
+                    on(o['p2c_trans'], 3 * T)
         active = active.to(dev)
         keep.append(active)
         pb.active = active.data_ptr()
@@ -390,8 +415,11 @@ def make_layout(data, flags):
     heading_vec = flags.get('heading_vec')
     if heading_vec is None:              # read off the variables init_data created (:191-196)
         heading_vec = any('traj_local_heading' in d and torch.as_tensor(d['traj_local_heading']).numel() == 2 for d in persons.values())
+    # init_data created them (:173-175); with both flags off the reference neither reads nor optimises them
+    person2cam = ((flags.get('flag_opt_person2cam_rot', False) or flags.get('flag_opt_person2cam_trans', False))
+                  and any('person2cam_res_rot' in d for d in persons.values()))
     return VariableLayout(T, n_empty, rows, [int(d['exist_len']) for d in persons.values()],
-                          heading_dim=2 if heading_vec else 1, world_dxy=world_dxy)
+                          heading_dim=2 if heading_vec else 1, world_dxy=world_dxy, person2cam=person2cam)
 
 
 def bind_variables(data, layout, theta):
@@ -404,7 +432,8 @@ def bind_variables(data, layout, theta):
     for p, d in enumerate(data['person_data'].values()):
         pv = layout.views(theta, p)
         for name in ['traj_local_xy', 'traj_local_heading', 'traj_local_dxy', 'traj_local_dheading', 'traj_local_z',
-                     'traj_local_rot', 'smpl_orient_world_res', 'root_trans_world_res', 'world_dheading', 'world_dxy']:
+                     'traj_local_rot', 'smpl_orient_world_res', 'root_trans_world_res', 'world_dheading', 'world_dxy',
+                     'person2cam_res_rot', 'person2cam_res_trans']:
             # world_dheading exists once a stage has requested it (global_recon_model.py:624-627); with continue_opt it
             # arrives already optimised and forward() keeps composing with it (:459-465)
             if name in d:

@@ -180,6 +180,8 @@ class GlobalReconOptimizer:
         self.flag_opt_cam = g('flag_opt_cam', True)
         self.flag_fixed_cam = g('flag_fixed_cam', False)
         self.flag_opt_vis_local_rot = g('flag_opt_vis_local_rot', False)
+        self.flag_opt_person2cam_rot = g('flag_opt_person2cam_rot', False)
+        self.flag_opt_person2cam_trans = g('flag_opt_person2cam_trans', False)
         self.flag_cam_inv_trans_res_all = g('flag_cam_inv_trans_res_all', True)
         self.flag_filter_pose = g('flag_filter_pose', True)
         self.flag_make_invis_with_keypoint = g('flag_make_invis_with_keypoint', False)
@@ -191,8 +193,7 @@ class GlobalReconOptimizer:
         self.flag_traj_from_cam = g('flag_traj_from_cam', False)
         self.traj_interp_method = g('traj_interp_method', 'linear_interp')
         self.opt_stage_specs = self.cfg.opt_stage_specs
-        for flag in ['flag_opt_motion_latent', 'flag_opt_traj_latent', 'flag_use_pen_loss',
-                     'flag_opt_person2cam_rot', 'flag_opt_person2cam_trans']:
+        for flag in ['flag_opt_motion_latent', 'flag_opt_traj_latent', 'flag_use_pen_loss']:
             if g(flag, False):
                 raise NotImplementedError(f'{flag} is not implemented in the CUDA path (SURVEY.md §8(f)-4); no CPU fallback')
         if g('absolute_heading', False):
@@ -234,7 +235,8 @@ class GlobalReconOptimizer:
     def _flags(self):
         return {k: getattr(self, k) for k in ['flag_fixed_cam', 'flag_opt_cam', 'flag_opt_cam_from_person_pose',
                                               'flag_cam_inv_trans_res_all', 'flag_opt_vis_local_rot', 'cam_fix_frames',
-                                              'flag_opt_traj', 'traj_source', 'heading_vec', 'world_dxy']}
+                                              'flag_opt_traj', 'traj_source', 'heading_vec', 'world_dxy', 'flag_opt_person2cam_rot',
+                                              'flag_opt_person2cam_trans']}
 
     # ------------------------------------------------------------------------------------------------ init_data
     def _person_from_estimate(self, est, gt_entry):
@@ -504,6 +506,9 @@ class GlobalReconOptimizer:
         if self.flag_opt_traj:                                     # :171-205
             last = d
             for d in persons.values():
+                if self.flag_opt_person2cam_rot or self.flag_opt_person2cam_trans:        # identity 6d, zero translation (:173-175)
+                    d['person2cam_res_rot'] = torch.tensor([1., 0., 0., 0., 1., 0.], device=dev).repeat(num_fr, 1)
+                    d['person2cam_res_trans'] = torch.zeros(num_fr, 3, device=dev)
                 d['smpl_orient_world_res'] = torch.zeros_like(last['smpl_orient_world'])
                 d['root_trans_world_res'] = torch.zeros_like(last['root_trans_world'])
             rel = {}

@@ -173,6 +173,8 @@ typedef struct glamr_person {
   int32_t off_xy, off_heading, off_dxy, off_dheading, off_z, off_rot;     /* offsets into theta (floats)        */
   int32_t off_world_dheading, off_orient_res, off_trans_res;              /* [T], [T,3], [T,3]                  */
   int32_t off_world_dxy;           /* [T,2] world_dxy (read only with has_world_dxy)                              */
+  int32_t off_p2c_rot, off_p2c_trans; /* [T,6] person2cam_res_rot, [T,3] person2cam_res_trans (read only with
+                                    * has_person2cam)                                                               */
   const float* traj_local_pred;    /* [len,11]                                                                    */
   const float* orient_base_init;   /* [T,3] smpl_orient_world_base outside the exist range                        */
   const float* trans_base_init;    /* [T,3]                                                                       */
@@ -216,6 +218,8 @@ typedef struct glamr_problem {
                                     * the predicted heading VECTOR, whose angle enters the scan; 0 = 'scalar' (angle)   */
   int32_t has_world_dxy;           /* world_dxy [T,2] is added to root_trans_world x / y (:467-468)                */
   int32_t world_dxy_alias;         /* that add also lands in the base (see glamr_person_t.world_dxy_base)          */
+  int32_t has_person2cam;          /* flag_opt_person2cam_rot / _trans (:484-488): mode 3 composes each person's person2cam with
+                                    * [rot6d(person2cam_res_rot) | person2cam_res_trans] before the mean; 0 = person2cam as is */
   float cam_up_first_weight;
   float rel_trans_weight;
   float term_weight[GLAMR_NUM_TERMS];   /* YAML weight, 0 if the term is absent                                  */
