@@ -44,6 +44,21 @@ GLAMR_HD void svd3(const double K[9], double U[9], double s[3], double Vm[9]) {
     for (int i = 0; i < 3; ++i) { Vm[i * 3 + j] = V[i * 3 + k]; U[i * 3 + j] = s[k] > 1e-300 ? A[i * 3 + k] / s[k] : 0.0; }
   }
   for (int j = 0; j < 3; ++j) s[j] = ss[j];
+  if (s[1] <= 1e-12 * fmax(s[0], 1e-300)) {
+    // rank <= 1 (collinear points): the second column of A is rounding noise, and normalising it gives a U column that need
+    // not be orthogonal to the first, which would leak into R a.  Take the unit vector orthogonal to U[:,0] built from the
+    // axis least aligned with it.
+    int k = 0;
+    for (int i = 1; i < 3; ++i)
+      if (fabs(U[i * 3]) < fabs(U[k * 3])) k = i;
+    double e[3] = {0, 0, 0};
+    e[k] = 1.0;
+    const double d = U[k * 3];
+    double nrm = 0.0;
+    for (int i = 0; i < 3; ++i) { e[i] -= d * U[i * 3]; nrm += e[i] * e[i]; }
+    nrm = sqrt(nrm);
+    for (int i = 0; i < 3; ++i) U[i * 3 + 1] = e[i] / nrm;
+  }
   if (s[2] <= 1e-12 * fmax(s[0], 1e-300)) {   // rank deficient: complete U with the cross product of the first two columns
     U[2] = U[3] * U[7] - U[6] * U[4];
     U[5] = U[6] * U[1] - U[0] * U[7];

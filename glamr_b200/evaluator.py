@@ -159,7 +159,11 @@ class Evaluator:
         self.reset()
 
     def _set_regressor(self, reg):
-        """dense [rows, V] -> CSR on the device (the H36M regressor is ~99.9 % zeros)"""
+        """dense [rows, V] -> CSR on the device (the H36M regressor is ~99.9 % zeros).  V must be the body model's vertex count: the
+        kernel takes it as the per-frame vertex stride, so any other width would read other frames' vertices or past the end."""
+        nv = self.smpl.num_verts
+        if reg.ndim != 2 or reg.shape[0] <= 0 or reg.shape[1] != nv:
+            raise L.GlamrError(f'h36m_regressor must be [rows, {nv}] (one column per vertex of the body model); got {list(reg.shape)}')
         rows, V = reg.shape
         ptr, ci, w = [0], [], []
         for r in range(rows):
@@ -179,6 +183,8 @@ class Evaluator:
     def regress_h36m(self, vertices):
         """torch.matmul(self.J_regressor, vertices) (:263) -> [n, 17, 3]"""
         rows, V, ptr, ci, w = self._reg
+        if vertices.dim() != 3 or vertices.shape[1:] != (V, 3):
+            raise L.GlamrError(f'regress_h36m: vertices must be [n, {V}, 3] to match the regressor; got {list(vertices.shape)}')
         v = vertices.contiguous().float()
         out = torch.empty((v.shape[0], rows, 3), device=self.device)
         with torch.cuda.device(self.device):

@@ -60,6 +60,8 @@ def load_smpl_assets(model_dir=SMPL_MODEL_DIR, extra_path=JOINT_REGRESSOR_TRAIN_
 class SMPL:
     """``SMPL(model_path_or_assets, pose_type='body26fk', device=...)``"""
 
+    num_verts = 6890                              # the SMPL mesh: forward returns vertices [n, num_verts, 3]
+
     def __init__(self, model_path=SMPL_MODEL_DIR, *args, pose_type='body26fk', device='cuda', joint_map=None, **kwargs):
         self.device = L.require_cuda(device)
         assets = model_path if isinstance(model_path, dict) else load_smpl_assets(model_path)
@@ -125,7 +127,7 @@ class SMPL:
         go, rt, rs = self._prep(global_orient, n, 3), self._prep(root_trans, n, 3), self._prep(root_scale, n, 0)
         nj = 24 if orig_joints else self.num_joints
         joints = torch.empty((n, nj, 3), dtype=torch.float32, device=self.device)
-        verts = torch.empty((n, 6890, 3), dtype=torch.float32, device=self.device) if return_verts else None
+        verts = torch.empty((n, self.num_verts, 3), dtype=torch.float32, device=self.device) if return_verts else None
         ws = self._workspace(n)
         with torch.cuda.device(self.device):
             L.check(self._lib.glamr_smpl_forward(self._h, n, L.ptr(go), L.ptr(bp), L.ptr(be), L.ptr(rt), L.ptr(rs), int(orig_joints),

@@ -21,7 +21,7 @@ def quat_apply(q, v):
 
 def world2heading(orient_q, trans):
     """traj_pred/utils/traj_utils.py:97-107 with apply_base_orient_after=True"""
-    base = torch.tensor(BASE, dtype=orient_q.dtype)
+    base = torch.tensor(BASE, dtype=orient_q.dtype, device=orient_q.device)
     nobase = rt.quat_mul(orient_q, rt.quat_conj(base).expand_as(orient_q))
     inv_h = rt.quat_conj(rt.get_heading_q(nobase[0])).expand_as(nobase)
     oh = rt.quat_mul(inv_h, nobase)
@@ -31,14 +31,16 @@ def world2heading(orient_q, trans):
 
 
 def similarity_align(S1, S2):
-    """lib/utils/torch_transform.py:282-345 for [n, J, 3] inputs"""
+    """lib/utils/torch_transform.py:282-345 for [n, J, 3] inputs, aligned frame by frame.  The reference transposes its inputs
+    only when the batch size is neither 2 nor 3 (torch_transform.py:298-302, a test of S1.shape[0]), so for n in {2, 3} it aligns
+    across frames; this restatement, like the product, keeps the per-frame alignment at every n."""
     S1, S2 = S1.permute(0, 2, 1), S2.permute(0, 2, 1)
     mu1, mu2 = S1.mean(dim=-1, keepdim=True), S2.mean(dim=-1, keepdim=True)
     X1, X2 = S1 - mu1, S2 - mu2
     var1 = (X1 ** 2).sum(dim=1).sum(dim=1)
     K = X1.bmm(X2.permute(0, 2, 1))
     U, s, V = torch.svd(K)
-    Z = torch.eye(3).unsqueeze(0).repeat(U.shape[0], 1, 1)
+    Z = torch.eye(3, dtype=S1.dtype, device=S1.device).unsqueeze(0).repeat(U.shape[0], 1, 1)
     Z[:, -1, -1] *= torch.sign(torch.det(U.bmm(V.permute(0, 2, 1))))
     R = V.bmm(Z.bmm(U.permute(0, 2, 1)))
     scale = torch.stack([torch.trace(x) for x in R.bmm(K)]) / var1
@@ -47,10 +49,17 @@ def similarity_align(S1, S2):
 
 
 class OracleEvaluator:
-    def __init__(self, smpl_assets, h36m_regressor, dataset='', align_freq=250):
-        self.smpl = OracleSMPL(smpl_assets)
-        self.J = torch.tensor(np.asarray(h36m_regressor, np.float32))
+    def __init__(self, smpl_assets, h36m_regressor, dataset='', align_freq=250, dtype=torch.float32, device='cpu'):
+        """dtype, device: where and in what precision everything is computed; the inputs are converted to them (the float32
+        constants and inputs are read as float32 first, so a float64 oracle sees the same values as the float32 one)"""
+        self.dtype, self.device = dtype, torch.device(device)
+        self.smpl = OracleSMPL(smpl_assets, device=self.device, dtype=dtype)
+        self.J = torch.tensor(np.asarray(h36m_regressor, np.float32), device=self.device).to(dtype)
         self.dataset, self.align_freq = dataset, align_freq
+
+    def _w(self, x):
+        """an input in the working dtype on the working device"""
+        return torch.as_tensor(x).to(self.device, self.dtype)
 
     def aligned(self, d):
         """:202-216"""
@@ -74,20 +83,20 @@ class OracleEvaluator:
             if 'exist_frames' in pd:
                 ex = pd['exist_frames']
                 for d in (pd, data['gt'][idx]):
-                    for k in ['smpl_orient_world', 'root_trans_world', 'smpl_pose', 'smpl_beta', 'pose', 'root_trans', 'visible_orig']:
+                    for k in ['smpl_orient_world', 'root_trans_world', 'smpl_pose', 'smpl_beta', 'pose', 'root_trans', 'scale', 'visible_orig']:
                         if k in d and d[k] is not None:        # every key containing a use_keys substring (:221-236), 'visible_orig' included
                             d[k] = d[k][ex]
         for idx, gd in data['gt'].items():
             vis = data['person_data'][idx]['visible_orig']
             gd['vis_frames'], gd['invis_frames'] = vis == 1, vis == 0
-            gd['smpl_orient_world'], gd['root_trans_world'] = gd['pose'][:, :3].float(), gd['root_trans'].float()
+            gd['smpl_orient_world'], gd['root_trans_world'] = self._w(gd['pose'][:, :3]), self._w(gd['root_trans'])
             if self.dataset == '3DPW':
                 oq = rt.aa_to_quat(gd['smpl_orient_world'])
-                quat = rt.aa_to_quat(torch.tensor([[np.pi * 0.5, 0, 0]])).expand_as(oq)
+                quat = rt.aa_to_quat(torch.tensor([[np.pi * 0.5, 0, 0]], dtype=self.dtype, device=self.device)).expand_as(oq)
                 gd['smpl_orient_world'] = rt.quat_to_aa(rt.quat_mul(quat, oq))
                 gd['root_trans_world'] = quat_apply(quat, gd['root_trans_world'])
             n = gd['pose'].shape[0]
-            body, betas = gd['pose'][:, 3:].float(), gd['shape'].float().reshape(1, -1).repeat(n, 1)
+            body, betas = self._w(gd['pose'][:, 3:]), self._w(gd['shape']).reshape(1, -1).repeat(n, 1)
             verts, j15 = self._eval(gd['smpl_orient_world'], body, betas, gd['root_trans_world'])
             pelvis = (j15[:, [3]] + j15[:, [4]]) * 0.5
             gd['eval_joints_world'], gd['eval_verts_world'] = j15[:, 1:] - pelvis, verts - pelvis
@@ -97,6 +106,9 @@ class OracleEvaluator:
         for idx, pd in data['person_data'].items():
             vis = pd['visible_orig']
             pd['vis_frames'], pd['invis_frames'] = vis == 1, vis == 0
+            for k in ('smpl_orient_world', 'smpl_pose', 'smpl_beta', 'root_trans_world', 'scale'):
+                if pd.get(k) is not None:
+                    pd[k] = self._w(pd[k])
             verts, j15 = self._eval(pd['smpl_orient_world'], pd['smpl_pose'], pd['smpl_beta'], pd['root_trans_world'], pd.get('scale'))
             pelvis = (j15[:, [3]] + j15[:, [4]]) * 0.5
             pd['eval_joints_world'], pd['eval_verts_world'] = j15[:, 1:] - pelvis, verts - pelvis
