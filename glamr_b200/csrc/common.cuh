@@ -58,6 +58,11 @@ constexpr int kTcNTiles = (kV * 3 + kTcN - 1) / kTcN;   // 81
 constexpr int kTcCols = kTcNTiles * kTcN;    // 20736
 constexpr int kTcAStageHalves = 2 * (kTcChunkK / 8) * kTcM * 8;   // hi | lo images of a [128 x 16] K-major core-matrix tile: 4096 halves
 constexpr int kTcBStageHalves = 2 * (kTcChunkK / 8) * kTcN * 8;   // 8192 halves
+// the blend epilogue stages a warpgroup's 64 frames x 32 columns at a time in shared memory, [column][frame] with a pitch of 84 floats:
+// 2 x 84 = 8 (mod 32) banks between the fragment's column pairs keeps its scalar writes conflict free, and 21 = 5 (mod 8) 16-byte units
+// per column puts the 4-frame pieces of a whole 20-frame group (5 per column) in consecutive bank quads, as they run in v_posed
+constexpr int kTcOutCols = 32;
+constexpr int kTcOutPitch = 84;
 // tensor-core skinning (lbs_skin_tc_kernel): T[vertex][frame x 12] = W[vertex][24 joints] . A[24 joints][frame x 12]
 constexpr int kSkF = 20;                     // frames per CTA tile
 constexpr int kSkN = kSkF * 12;              // 240 accumulator columns (wgmma N): the 3x4 blended transform of each frame

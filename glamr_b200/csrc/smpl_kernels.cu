@@ -327,8 +327,11 @@ __global__ void __launch_bounds__(128) blend_features_kernel(int n, const float*
 // of B) with no SIMT work on the operand path.  Tile = 128 frames x 256 basis columns, K in 14 steps of 16; warp 8 = TMA producer,
 // warpgroups 0 and 1 = consumers (64 frames each, m64n256k16, the accumulator in 128 registers per thread), which release a stage once
 // the wgmma group that read it has retired and finally multiply each row by its exact unscale factor 2^-(e_f + e_B) and store the
-// accumulator TRANSPOSED ([column][frame]) so that lbs_skin_kernel (lanes = frames) reads contiguous bytes per vertex coordinate.  8 stages x 24 KB = 192 KB of shared memory per CTA: with 4 stages the blend alone runs as fast, but the iteration of
-// 4 x 300 frame-persons, where the blend shares the GPU with the residual and backward kernels, is ~5 % slower.
+// accumulator TRANSPOSED ([column][frame]) so that lbs_skin_kernel (lanes = frames) reads contiguous bytes per vertex coordinate; the
+// store goes through a shared-memory staging chunk per warpgroup, so that it leaves as 16-byte pieces of whole frame runs instead of
+// scalars that half-fill their sectors.  8 stages x 24 KB = 192 KB of shared memory per CTA (+ 21 KB of staging): with 4 stages the
+// blend alone runs as fast, but the iteration of 4 x 300 frame-persons, where the blend shares the GPU with the residual and backward
+// kernels, is ~5 % slower.
 // Persistent: the grid has one CTA per SM (the register file holds one), and CTA b runs tiles b, b + grid, ...  The stage ring runs on
 // across tiles, so the producer fetches the next tile's first stages while the consumers store the current accumulator.  Tiles are
 // numbered column-tile major (frame tile fastest): the CTAs that read one 448 KB basis column tile run at the same time, and the
@@ -338,7 +341,8 @@ constexpr int kTcStages = 8;
 constexpr int kTcThreads = 288;           // warpgroups 0-1 consume, warp 8 produces
 constexpr uint32_t kTcABytes = kTcAStageHalves * sizeof(__half);     // 8,192
 constexpr uint32_t kTcBBytes = kTcBStageHalves * sizeof(__half);     // 16,384
-constexpr size_t kTcSmemBytes = (size_t)kTcStages * (kTcABytes + kTcBBytes) + 128;
+constexpr size_t kTcRingBytes = (size_t)kTcStages * (kTcABytes + kTcBBytes) + 128;   // stages, then the full / empty barriers
+constexpr size_t kTcSmemBytes = kTcRingBytes + 2 * (size_t)kTcOutCols * kTcOutPitch * sizeof(float);   // + a staging chunk per warpgroup
 
 // Phase clock of the consumer warpgroups (tools/blend_phases_exp.py), experiment build only: each consumer thread adds the clock64
 // cycles since its previous stamp to a phase; lane 0 of the first warp of each warpgroup adds the sums of its CTA at the end of a launch.
@@ -365,6 +369,13 @@ extern "C" int glamr_exp_blend_phases(long long* out) {    // the per-CTA sums o
 #define BLEND_CLOCK_TILE() do { } while (0)
 #define BLEND_CLOCK_STORE() do { } while (0)
 #endif
+
+// bar.sync of the 128 threads of consumer warpgroup g on named barrier 1 + g (0 is __syncthreads); immediate ids, so that ptxas
+// reserves 3 barriers rather than all 16
+__device__ __forceinline__ void warpgroup_sync(int g) {
+  if (g == 0) asm volatile("bar.sync 1, 128;" ::: "memory");
+  else asm volatile("bar.sync 2, 128;" ::: "memory");
+}
 
 // mtile0 / mtiles: the 128-frame tiles [mtile0, mtile0 + mtiles) of this launch (the host launches them all, from mtile0 = 0);
 // half_last: the last of them holds at most 64 frames; ntn: the 256-column tiles (the mesh's 81, plus the support columns when the
@@ -458,24 +469,59 @@ __global__ void __launch_bounds__(kTcThreads, 1) lbs_blend_tc_kernel(SmplDev m, 
     else mainloop(acc, [](float (&d)[kTcN / 2], uint64_t da, uint64_t db, uint32_t acc_in) { wgmma_m64n256k16_f16(d, da, db, acc_in); });
     __syncwarp();
     if (lane == 0) mbar_arrive(&empty[(q - 1) % kTcStages]);                     // the tile's last stage: the producer moves on
-    // ---- epilogue: d[4 i + 2 h + e] = D[16 (warp % 4) + lane / 4 + 8 h][8 i + 2 (lane % 4) + e]
-    // v_posed^T [column][frame], or frame-tiled [frame / 20][column][frame % 20] for the tensor-core skinning; a store instruction
-    // writes 8 consecutive frames (32 bytes) of 4 columns
-    const int row0 = mtile * kTcM + (half ? 0 : g * 64) + (warp & 3) * 16 + (lane >> 2);
+    // ---- epilogue: d[4 i + 2 h + e] = D[16 (warp % 4) + lane / 4 + 8 h][8 i + 2 (lane % 4) + e], times the row's unscale factor.
+    // The warpgroup stages kTcOutCols columns at a time in shared memory ([column][frame]) and stores them as 16-byte pieces of 4
+    // consecutive frames: it starts at a multiple of 64 frames, so every piece lies inside one 20-frame group and is 16-byte aligned in
+    // both layouts.  v_posed^T [column][mpad]: a column's 64 frames are one 256-byte run, piece p of the chunk is frame piece p % 16 of
+    // column p / 16.  Frame-tiled [frame / 20][column][frame % 20] (tensor-core skinning): the chunk's pieces run group by group, and
+    // inside a group column by column over the group's frames the warpgroup holds, so that a group the warpgroup holds whole goes out
+    // as one contiguous run of kTcOutCols x 80 bytes.
+    const int f0 = mtile * kTcM + (half ? 0 : g * 64);                            // the warpgroup's first frame
     const int col0 = ntile * kTcN + (half ? g * 128 : 0);
     const int ncols = half ? kTcN / 2 : kTcN;
+    const int rl = (warp & 3) * 16 + (lane >> 2);                                 // the fragment's row for h = 0
+    float unscale[2];
 #pragma unroll
-    for (int h = 0; h < 2; ++h) {
-      const int frame = row0 + 8 * h;                                             // < w.mpad by construction
-      const float unscale = w.tcUnscale[frame] * m.tcB_unscale;                   // 2^-(e_f + e_B): exact
-      float* out = (w.vp_tiled ? vpb + ((size_t)(frame / kSkF) * w.vp_cols + (size_t)col0) * kSkF + frame % kSkF
-                               : vpb + (size_t)col0 * w.mpad + frame) + (size_t)(2 * (lane & 3)) * cstride;
+    for (int h = 0; h < 2; ++h) unscale[h] = w.tcUnscale[f0 + rl + 8 * h] * m.tcB_unscale;   // 2^-(e_f + e_B): exact
+    // the pieces this thread stores in every chunk: their offsets in the staging chunk and in v_posed at the chunk's first column
+    constexpr int kPieces = kTcOutCols * 16 / 128;
+    int soff[kPieces];
+    size_t goff[kPieces];
 #pragma unroll
-      for (int i = 0; i < kTcN / 8; ++i) {
-        if (8 * i < ncols) {
-          out[(size_t)(8 * i) * cstride] = acc[4 * i + 2 * h] * unscale;
-          out[(size_t)(8 * i + 1) * cstride] = acc[4 * i + 2 * h + 1] * unscale;
-        }
+    for (int j = 0; j < kPieces; ++j) {
+      const int p = (tid & 127) + 128 * j;
+      int fq, c;                                                                  // frame piece 0..15 of the warpgroup, column of the chunk
+      if (w.vp_tiled) {
+        const int q0 = f0 / 4, grp = (q0 + p / kTcOutCols) / 5;                   // the 20-frame group whose run holds p
+        const int qa = max(5 * grp - q0, 0), qn = min(5 * grp + 5 - q0, 16) - qa; // the warpgroup's pieces qa .. qa + qn - 1 of it
+        const int pg = p - kTcOutCols * qa;
+        c = pg / qn;
+        fq = qa + pg - c * qn;
+      } else {
+        fq = p & 15;
+        c = p >> 4;
+      }
+      const int f = f0 + 4 * fq;
+      soff[j] = c * kTcOutPitch + 4 * fq;
+      goff[j] = w.vp_tiled ? ((size_t)(f / kSkF) * w.vp_cols + (size_t)(col0 + c)) * kSkF + f % kSkF : (size_t)(col0 + c) * w.mpad + f;
+    }
+    float* const stage = reinterpret_cast<float*>(tc_raw + kTcRingBytes) + g * kTcOutCols * kTcOutPitch;
+#pragma unroll
+    for (int k = 0; k < kTcN / kTcOutCols; ++k) {
+      if (kTcOutCols * k < ncols) {
+        warpgroup_sync(g);                                                    // the previous chunk has been read
+#pragma unroll
+        for (int i = 0; i < kTcOutCols / 8; ++i)
+#pragma unroll
+          for (int h = 0; h < 2; ++h)
+#pragma unroll
+            for (int e = 0; e < 2; ++e)
+              stage[(8 * i + 2 * (lane & 3) + e) * kTcOutPitch + rl + 8 * h] = acc[4 * (k * kTcOutCols / 8 + i) + 2 * h + e] * unscale[h];
+        warpgroup_sync(g);
+        float* const out = vpb + (size_t)(k * kTcOutCols) * cstride;
+#pragma unroll
+        for (int j = 0; j < kPieces; ++j)
+          *reinterpret_cast<float4*>(out + goff[j]) = *reinterpret_cast<const float4*>(stage + soff[j]);
       }
     }
     BLEND_CLOCK(2);
