@@ -23,9 +23,9 @@ struct OptScratch {
   float* trans_base;    // [N][3]
   float* orient_world;  // [N][3]
   float* trans_world;   // [N][3]
-  float* cam;           // [T][12] world->cam (3x4 row-major)
-  float* cam_inv;       // [T][12]
-  float* cam_d6;        // [T][6]  6d of cam_inv rotation incl. residual (mode 3)
+  float* cam;           // [G*T][12] world->cam (3x4 row-major), one block of T rows per seed group
+  float* cam_inv;       // [G*T][12]
+  float* cam_d6;        // [G*T][6]  6d of cam_inv rotation incl. residual (mode 3)
   float* joints_world;  // [N][J][3]
   float* kp_pred;       // [N][J][2]
   float* orient_ciw;    // [N][3]  smpl_orient_cam_in_world
@@ -33,7 +33,7 @@ struct OptScratch {
   float* g_orient;      // [N][3]  dL/d smpl_orient_world
   float* g_trans;       // [N][3]  dL/d root_trans_world
   float* g_cam;         // [N][12] per frame-person dL/d cam (R 9, t 3)
-  float* g_cam_fix;     // [T][12] per-frame dL/d (cam_rot_6d, cam_trans) [9 used] in fixed-camera mode; mode 3: dL/d(mean cam_inv)
+  float* g_cam_fix;     // [G*T][12] per-frame dL/d (cam_rot_6d, cam_trans) [9 used] in fixed-camera mode; mode 3: dL/d(mean cam_inv)
   float* g_xy;          // [N][2]  backward scan buffer
   float* g_head;        // [N]
   float* grad;          // [n_params]
@@ -52,6 +52,18 @@ struct TermAcc {
     for (int k = 0; k < GLAMR_NUM_TERMS; ++k) v[k] = 0.0;
   }
 };
+
+// Seed groups (include/glamr_b200.h, glamr_problem_t.G): group g owns persons [g*Q, (g+1)*Q), Q = P/G, the camera rows
+// [g*T, (g+1)*T) of every per-frame table and scratch array, and theta [g*group_params, ...).  A camera frame is addressed by its
+// row gt = g*T + t; with one group gt = t.
+GLAMR_HD int num_groups(const glamr_problem_t& pb) { return pb.G > 1 ? pb.G : 1; }
+GLAMR_HD int group_persons(const glamr_problem_t& pb) { return pb.P / num_groups(pb); }
+GLAMR_HD int group_theta(const glamr_problem_t& pb, int g) { return g > 0 ? g * pb.group_params : 0; }
+// group of person p (persons are stored group by group; glamr_person_t.group records the same).  Computed from the index, so the
+// camera address of a frame-person does not wait on a load of its person record
+GLAMR_HD int person_group(const glamr_problem_t& pb, int p) { return pb.G > 1 ? p / group_persons(pb) : 0; }
+// camera row of frame t seen by person p
+GLAMR_HD size_t cam_row(const OptCtx& c, int p, int t) { return (size_t)person_group(c.pb, p) * c.pb.T + t; }
 
 GLAMR_HD void mat34_inverse(const float* M, float* I) {
   // lib/utils/torch_transform.py:274-279  [R^T | -R^T t]
@@ -250,11 +262,12 @@ GLAMR_HD void person2cam_with_residual(const OptCtx& c, const glamr_person_t& ps
   const float E[12] = {R[0], R[1], R[2], tr[0], R[3], R[4], R[5], tr[1], R[6], R[7], R[8], tr[2]};
   mat34_mul(ps.person2cam + (size_t)s * 12, E, P2C);
 }
-// mean over visible persons of person_transform_world @ person2cam at source frame s  (:482-492)
-GLAMR_HD void mean_cam_inv(const OptCtx& c, int s, float* M) {
+// mean over the visible persons of group g of person_transform_world @ person2cam at source frame s  (:482-492)
+GLAMR_HD void mean_cam_inv(const OptCtx& c, int g, int s, float* M) {
 #pragma unroll
   for (int k = 0; k < 12; ++k) M[k] = 0.0f;
-  for (int p = 0; p < c.pb.P; ++p) {
+  const int Q = group_persons(c.pb);
+  for (int p = g * Q; p < (g + 1) * Q; ++p) {
     const glamr_person_t& ps = c.pb.persons[p];
     if (ps.vis[s] == 0.0f) continue;
     float Tw[12], C[12];
@@ -269,46 +282,48 @@ GLAMR_HD void mean_cam_inv(const OptCtx& c, int s, float* M) {
 #pragma unroll
     for (int k = 0; k < 12; ++k) M[k] += C[k];
   }
-  const float inv = c.pb.inv_num_persons[s];
+  const float inv = c.pb.inv_num_persons[(size_t)g * c.pb.T + s];
 #pragma unroll
   for (int k = 0; k < 12; ++k) M[k] *= inv;
 }
-GLAMR_HD void cam_forward(const OptCtx& c, int t) {
+// camera of row gt = g*T + t (frame t of group g)
+GLAMR_HD void cam_forward(const OptCtx& c, int gt) {
   float cam[12], inv[12];
   const int mode = c.pb.cam_mode;
+  const int g = gt / c.pb.T, t = gt - g * c.pb.T, og = group_theta(c.pb, g);
   if (mode == GLAMR_CAM_CONST) {
 #pragma unroll
-    for (int k = 0; k < 12; ++k) cam[k] = c.pb.cam_pose_const[(size_t)t * 12 + k];
+    for (int k = 0; k < 12; ++k) cam[k] = c.pb.cam_pose_const[(size_t)gt * 12 + k];
     mat34_inverse(cam, inv);
   } else if (mode == GLAMR_CAM_PER_FRAME || mode == GLAMR_CAM_FIXED) {
     const int r = (mode == GLAMR_CAM_FIXED) ? 0 : t;
     float R[9];
-    rot6d_to_rotmat(c.theta + c.pb.off_cam_rot + 6 * r, R);
-    const float* tc = c.theta + c.pb.off_cam_trans + 3 * r;
+    rot6d_to_rotmat(c.theta + og + c.pb.off_cam_rot + 6 * r, R);
+    const float* tc = c.theta + og + c.pb.off_cam_trans + 3 * r;
     cam[0] = R[0]; cam[1] = R[1]; cam[2] = R[2]; cam[3] = tc[0];
     cam[4] = R[3]; cam[5] = R[4]; cam[6] = R[5]; cam[7] = tc[1];
     cam[8] = R[6]; cam[9] = R[7]; cam[10] = R[8]; cam[11] = tc[2];
     mat34_inverse(cam, inv);
   } else {
     float M[12], R[9], d6[6];
-    mean_cam_inv(c, c.pb.fill_src[t], M);
+    mean_cam_inv(c, g, c.pb.fill_src[gt], M);
     mat34_R(M, R);
     rotmat_to_rot6d(R, d6);
-    const int e = c.pb.empty_index[t];
+    const int e = c.pb.empty_index[gt];
     if (e >= 0) {
 #pragma unroll
-      for (int k = 0; k < 6; ++k) d6[k] += c.theta[c.pb.off_cam_rot + 6 * e + k];
+      for (int k = 0; k < 6; ++k) d6[k] += c.theta[og + c.pb.off_cam_rot + 6 * e + k];
     }
 #pragma unroll
-    for (int k = 0; k < 6; ++k) c.sc.cam_d6[(size_t)t * 6 + k] = d6[k];
+    for (int k = 0; k < 6; ++k) c.sc.cam_d6[(size_t)gt * 6 + k] = d6[k];
     rot6d_to_rotmat(d6, R);
     float tt[3] = {M[3], M[7], M[11]};
     if (c.pb.trans_res_all) {
 #pragma unroll
-      for (int k = 0; k < 3; ++k) tt[k] += c.theta[c.pb.off_cam_trans + 3 * t + k];
+      for (int k = 0; k < 3; ++k) tt[k] += c.theta[og + c.pb.off_cam_trans + 3 * t + k];
     } else if (e >= 0) {
 #pragma unroll
-      for (int k = 0; k < 3; ++k) tt[k] += c.theta[c.pb.off_cam_trans + 3 * e + k];
+      for (int k = 0; k < 3; ++k) tt[k] += c.theta[og + c.pb.off_cam_trans + 3 * e + k];
     }
     inv[0] = R[0]; inv[1] = R[1]; inv[2] = R[2]; inv[3] = tt[0];
     inv[4] = R[3]; inv[5] = R[4]; inv[6] = R[5]; inv[7] = tt[1];
@@ -317,8 +332,8 @@ GLAMR_HD void cam_forward(const OptCtx& c, int t) {
   }
 #pragma unroll
   for (int k = 0; k < 12; ++k) {
-    c.sc.cam[(size_t)t * 12 + k] = cam[k];
-    c.sc.cam_inv[(size_t)t * 12 + k] = inv[k];
+    c.sc.cam[(size_t)gt * 12 + k] = cam[k];
+    c.sc.cam_inv[(size_t)gt * 12 + k] = inv[k];
   }
 }
 
@@ -415,9 +430,10 @@ GLAMR_HD void frame_rest(const OptCtx& c, int p, int t, const KpGrad& kg, TermAc
   const size_t n = (size_t)p * T + t;
   const float* ow = c.sc.orient_world + n * 3;
   const float* tw = c.sc.trans_world + n * 3;
+  const float* cam = c.sc.cam + cam_row(c, p, t) * 12;
   float Rc[9], tc[3];
-  mat34_R(c.sc.cam + (size_t)t * 12, Rc);
-  tc[0] = c.sc.cam[(size_t)t * 12 + 3]; tc[1] = c.sc.cam[(size_t)t * 12 + 7]; tc[2] = c.sc.cam[(size_t)t * 12 + 11];
+  mat34_R(cam, Rc);
+  tc[0] = cam[3]; tc[1] = cam[7]; tc[2] = cam[11];
   float g_ow[3] = {0, 0, 0}, g_tw[3], g_Rc[9], g_tc[3];
 #pragma unroll
   for (int k = 0; k < 3; ++k) { g_tw[k] = kg.g_tw[k]; g_tc[k] = kg.g_tc[k]; }
@@ -586,23 +602,25 @@ GLAMR_HD void frame_rest(const OptCtx& c, int p, int t, const KpGrad& kg, TermAc
   }
 
   GLAMR_STAMP(7);
-  // ---- relative transforms between persons (loss_func.py:248-271): W_ij = inv(T_i) T_j against C_ij
+  // ---- relative transforms between the persons of one group (loss_func.py:248-271): W_ij = inv(T_i) T_j against C_ij.  i, j are
+  // indices inside the group; the group's pair tables start at rel_target / rel_w / rel_wt + its block
   if (pb.rel_target && pb.term_enabled[GLAMR_T_REL_TRANSFORM]) {
     const float gsr = c.gs[GLAMR_T_REL_TRANSFORM];
     const float twt = pb.rel_trans_weight;
-    const int i = p;
-    for (int j = 0; j < pb.P; ++j) {
+    const int Q = group_persons(pb), g = person_group(pb, p), i = p - g * Q;
+    const size_t pairs0 = (size_t)g * Q * Q;
+    for (int j = 0; j < Q; ++j) {
       if (j == i) continue;
-      const size_t nj = (size_t)j * T + t;
-      const float w_ij = pb.rel_w[((size_t)i * pb.P + j) * T + t], wt_ij = pb.rel_wt[((size_t)i * pb.P + j) * T + t];
-      const float w_ji = pb.rel_w[((size_t)j * pb.P + i) * T + t], wt_ji = pb.rel_wt[((size_t)j * pb.P + i) * T + t];
+      const size_t nj = ((size_t)g * Q + j) * T + t;
+      const float w_ij = pb.rel_w[(pairs0 + (size_t)i * Q + j) * T + t], wt_ij = pb.rel_wt[(pairs0 + (size_t)i * Q + j) * T + t];
+      const float w_ji = pb.rel_w[(pairs0 + (size_t)j * Q + i) * T + t], wt_ji = pb.rel_wt[(pairs0 + (size_t)j * Q + i) * T + t];
       if (w_ij == 0.0f && wt_ij == 0.0f && w_ji == 0.0f && wt_ji == 0.0f) continue;
       float Rj[9];
       aa_to_rotmat(c.sc.orient_world + nj * 3, Rj);
       const float* tj = c.sc.trans_world + nj * 3;
       const float dt[3] = {tj[0] - tw[0], tj[1] - tw[1], tj[2] - tw[2]};
       {  // pair (i,j): R_W = Ri^T Rj, t_W = Ri^T (tj - ti); this thread owns its loss value and dL/dT_i
-        const float* C = pb.rel_target + (((size_t)i * pb.P + j) * T + t) * 12;
+        const float* C = pb.rel_target + ((pairs0 + (size_t)i * Q + j) * T + t) * 12;
         float RW[9], tW[3], gRW[9] = {0, 0, 0, 0, 0, 0, 0, 0, 0}, gtW[3];
         mat3_tmul(Rw, Rj, RW);
         mat3_tvec(Rw, dt, tW);
@@ -635,7 +653,7 @@ GLAMR_HD void frame_rest(const OptCtx& c, int p, int t, const KpGrad& kg, TermAc
       }
       if (gsr != 0.0f && (w_ji != 0.0f || wt_ji != 0.0f)) {
         // pair (j,i): R_W' = Rj^T Ri, t_W' = Rj^T (ti - tj); only dL/dT_i here (thread (j,t) adds the value)
-        const float* C = pb.rel_target + (((size_t)j * pb.P + i) * T + t) * 12;
+        const float* C = pb.rel_target + ((pairs0 + (size_t)j * Q + i) * T + t) * 12;
         float RW[9], tW[3], gRW[9] = {0, 0, 0, 0, 0, 0, 0, 0, 0}, gtW[3];
         const float mdt[3] = {-dt[0], -dt[1], -dt[2]};
         mat3_tmul(Rj, Rw, RW);
@@ -674,9 +692,10 @@ GLAMR_HD void frame_rest(const OptCtx& c, int p, int t, const KpGrad& kg, TermAc
 // Sequential form (host harness): all joints of (p,t), then the rest.
 GLAMR_HD void frame_residuals(const OptCtx& c, int p, int t, TermAcc& acc) {
   const size_t n = (size_t)p * c.pb.T + t;
+  const float* cam = c.sc.cam + cam_row(c, p, t) * 12;
   float Rc[9], tc[3], Rs[9];
-  mat34_R(c.sc.cam + (size_t)t * 12, Rc);
-  tc[0] = c.sc.cam[(size_t)t * 12 + 3]; tc[1] = c.sc.cam[(size_t)t * 12 + 7]; tc[2] = c.sc.cam[(size_t)t * 12 + 11];
+  mat34_R(cam, Rc);
+  tc[0] = cam[3]; tc[1] = cam[7]; tc[2] = cam[11];
   rodrigues_smplx(c.sc.orient_world + n * 3, Rs);
   KpGrad kg;
   kg.clear();
@@ -686,20 +705,22 @@ GLAMR_HD void frame_residuals(const OptCtx& c, int p, int t, TermAcc& acc) {
 }
 
 // ------------------------------------------------------------------------------------------------ camera backward
-// Per frame t: sum dL/dcam over this rank's persons, add the camera-only terms (loss_func.py:60-114,199-201,240)
-// and push the gradient into the camera variables (or, mode 3, into the residual variables and back into the
+// Per camera row gt = g*T + t: sum dL/dcam over this rank's persons of group g, add the camera-only terms (loss_func.py:60-114,
+// 199-201,240) and push the gradient into the group's camera variables (or, mode 3, into the residual variables and back into the
 // persons' world transforms).
-GLAMR_HD void camera_backward(const OptCtx& c, int t, TermAcc& acc) {
+GLAMR_HD void camera_backward(const OptCtx& c, int gt, TermAcc& acc) {
   const glamr_problem_t& pb = c.pb;
   const int T = pb.T;
+  const int grp = gt / T, t = gt - grp * T, Q = group_persons(pb);
+  const int off_rot = group_theta(pb, grp) + pb.off_cam_rot, off_trans = group_theta(pb, grp) + pb.off_cam_trans;
   float G[12] = {0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0};   // dL/dRc (9) , dL/dtc (3)
-  for (int p = 0; p < pb.P; ++p) {          // frame-persons of other ranks hold zeros (frame_residuals_kernel)
+  for (int p = grp * Q; p < (grp + 1) * Q; ++p) {          // frame-persons of other ranks hold zeros (frame_residuals_kernel)
     const float* g = c.sc.g_cam + ((size_t)p * T + t) * 12;
 #pragma unroll
     for (int k = 0; k < 12; ++k) G[k] += g[k];
   }
-  const float* cam = c.sc.cam + (size_t)t * 12;
-  const float* inv = c.sc.cam_inv + (size_t)t * 12;
+  const float* cam = c.sc.cam + (size_t)gt * 12;
+  const float* inv = c.sc.cam_inv + (size_t)gt * 12;
   float gRi[9] = {0, 0, 0, 0, 0, 0, 0, 0, 0}, gti[3] = {0, 0, 0};   // w.r.t. cam_inv
   if (pb.owner) {
     if (pb.term_enabled[GLAMR_T_CAM_INV_ROT_SMOOTH] && T > 1) {
@@ -771,13 +792,13 @@ GLAMR_HD void camera_backward(const OptCtx& c, int t, TermAcc& acc) {
     G[9] -= r[0]; G[10] -= r[1]; G[11] -= r[2];
     const int row = (mode == GLAMR_CAM_FIXED) ? 0 : t;
     float g6[6];
-    rot6d_to_rotmat_vjp(c.theta + pb.off_cam_rot + 6 * row, G, g6);
+    rot6d_to_rotmat_vjp(c.theta + off_rot + 6 * row, G, g6);
     float gtr[3] = {G[9], G[10], G[11]};
     if (pb.owner && mode == GLAMR_CAM_PER_FRAME) {
       // smoothness directly on the camera variables (loss_func.py:60-73)
       if (pb.term_enabled[GLAMR_T_CAM_ROT_SMOOTH] && T > 1) {
         const float gs = c.gs[GLAMR_T_CAM_ROT_SMOOTH];
-        const float* x = c.theta + pb.off_cam_rot + 6 * t;
+        const float* x = c.theta + off_rot + 6 * t;
         float ss = 0.0f;
 #pragma unroll
         for (int k = 0; k < 6; ++k) {
@@ -788,7 +809,7 @@ GLAMR_HD void camera_backward(const OptCtx& c, int t, TermAcc& acc) {
       }
       if (pb.term_enabled[GLAMR_T_CAM_TRANS_SMOOTH] && T > 1) {
         const float gs = c.gs[GLAMR_T_CAM_TRANS_SMOOTH];
-        const float* x = c.theta + pb.off_cam_trans + 3 * t;
+        const float* x = c.theta + off_trans + 3 * t;
         float ss = 0.0f;
 #pragma unroll
         for (int k = 0; k < 3; ++k) {
@@ -800,14 +821,14 @@ GLAMR_HD void camera_backward(const OptCtx& c, int t, TermAcc& acc) {
     }
     if (mode == GLAMR_CAM_PER_FRAME) {
 #pragma unroll
-      for (int k = 0; k < 6; ++k) c.sc.grad[pb.off_cam_rot + 6 * t + k] = g6[k];
+      for (int k = 0; k < 6; ++k) c.sc.grad[off_rot + 6 * t + k] = g6[k];
 #pragma unroll
-      for (int k = 0; k < 3; ++k) c.sc.grad[pb.off_cam_trans + 3 * t + k] = gtr[k];
+      for (int k = 0; k < 3; ++k) c.sc.grad[off_trans + 3 * t + k] = gtr[k];
     } else {
 #pragma unroll
-      for (int k = 0; k < 6; ++k) c.sc.g_cam_fix[(size_t)t * 12 + k] = g6[k];
+      for (int k = 0; k < 6; ++k) c.sc.g_cam_fix[(size_t)gt * 12 + k] = g6[k];
 #pragma unroll
-      for (int k = 0; k < 3; ++k) c.sc.g_cam_fix[(size_t)t * 12 + 6 + k] = gtr[k];
+      for (int k = 0; k < 3; ++k) c.sc.g_cam_fix[(size_t)gt * 12 + 6 + k] = gtr[k];
     }
   } else if (mode == GLAMR_CAM_FROM_PERSONS) {
     // cam = inverse(cam_inv): Rc = Ri^T, tc = -Ri^T ti  ->  dRi += G_R^T - ti G_t^T ,  dti += -Ri G_t
@@ -823,11 +844,11 @@ GLAMR_HD void camera_backward(const OptCtx& c, int t, TermAcc& acc) {
     mat3_vec(Ri, Gt, r);
     gti[0] -= r[0]; gti[1] -= r[1]; gti[2] -= r[2];
     float g6[6];
-    rot6d_to_rotmat_vjp(c.sc.cam_d6 + (size_t)t * 6, gRi, g6);
-    const int e = pb.empty_index[t];
+    rot6d_to_rotmat_vjp(c.sc.cam_d6 + (size_t)gt * 6, gRi, g6);
+    const int e = pb.empty_index[gt];
     if (e >= 0) {
 #pragma unroll
-      for (int k = 0; k < 6; ++k) c.sc.grad[pb.off_cam_rot + 6 * e + k] = g6[k];
+      for (int k = 0; k < 6; ++k) c.sc.grad[off_rot + 6 * e + k] = g6[k];
     }
     // cam_inv_trans_residual_reg (loss_func.py:199-201,:240): sum (30 x)^2 / rows, owner only
     const int trow = pb.trans_res_all ? t : e;
@@ -837,39 +858,41 @@ GLAMR_HD void camera_backward(const OptCtx& c, int t, TermAcc& acc) {
         const float gs = c.gs[GLAMR_T_CAM_INV_TRANS_RES_REG];
         float ss = 0.0f;
 #pragma unroll
-        for (int k = 0; k < 3; ++k) { const float x = c.theta[pb.off_cam_trans + 3 * trow + k]; ss += x * x; gr[k] += 2.0f * kFps2 * gs * x; }
+        for (int k = 0; k < 3; ++k) { const float x = c.theta[off_trans + 3 * trow + k]; ss += x * x; gr[k] += 2.0f * kFps2 * gs * x; }
         acc.v[GLAMR_T_CAM_INV_TRANS_RES_REG] += (double)(kFps2 * ss);
       }
 #pragma unroll
-      for (int k = 0; k < 3; ++k) c.sc.grad[pb.off_cam_trans + 3 * trow + k] = gr[k];
+      for (int k = 0; k < 3; ++k) c.sc.grad[off_trans + 3 * trow + k] = gr[k];
     }
     // stash dL/d(mean cam_inv) of this frame in g_cam_fix for the scatter to the source frame
     float gR[9];
     rotmat_to_rot6d_vjp(g6, gR);
 #pragma unroll
-    for (int k = 0; k < 9; ++k) c.sc.g_cam_fix[(size_t)t * 12 + k] = gR[k];
+    for (int k = 0; k < 9; ++k) c.sc.g_cam_fix[(size_t)gt * 12 + k] = gR[k];
 #pragma unroll
-    for (int k = 0; k < 3; ++k) c.sc.g_cam_fix[(size_t)t * 12 + 9 + k] = gti[k];
+    for (int k = 0; k < 3; ++k) c.sc.g_cam_fix[(size_t)gt * 12 + 9 + k] = gti[k];
   }
 }
-// mode 3 only, after camera_backward of all frames: frame s gathers dL/d(mean) of every frame filled from it and
-// pushes it into dL/d(person_transform_world) of its visible persons and, with has_person2cam, into their person2cam
-// residuals at frame s (a person invisible at s gets none: the reference multiplies its term by vis_frames).
-GLAMR_HD void camera_scatter_to_persons(const OptCtx& c, int s) {
+// mode 3 only, after camera_backward of all frames: frame s (camera row gs = g*T + s) gathers dL/d(mean) of every frame of its
+// group filled from it and pushes it into dL/d(person_transform_world) of the group's persons visible at s and, with has_person2cam,
+// into their person2cam residuals at frame s (a person invisible at s gets none: the reference multiplies its term by vis_frames).
+GLAMR_HD void camera_scatter_to_persons(const OptCtx& c, int gs) {
   const glamr_problem_t& pb = c.pb;
   const int T = pb.T;
-  if (pb.fill_src[s] != s || pb.inv_num_persons[s] == 0.0f) return;
+  const int grp = gs / T, s = gs - grp * T, Q = group_persons(pb);
+  const int32_t* fill = pb.fill_src + (size_t)grp * T;
+  if (fill[s] != s || pb.inv_num_persons[gs] == 0.0f) return;
   float G[12] = {0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0};
   for (int t = 0; t < T; ++t) {
-    if (pb.fill_src[t] != s) continue;
-    const float* g = c.sc.g_cam_fix + (size_t)t * 12;
+    if (fill[t] != s) continue;
+    const float* g = c.sc.g_cam_fix + ((size_t)grp * T + t) * 12;
 #pragma unroll
     for (int k = 0; k < 12; ++k) G[k] += g[k];
   }
-  const float inv_n = pb.inv_num_persons[s];
+  const float inv_n = pb.inv_num_persons[gs];
 #pragma unroll
   for (int k = 0; k < 12; ++k) G[k] *= inv_n;
-  for (int p = 0; p < pb.P; ++p) {
+  for (int p = grp * Q; p < (grp + 1) * Q; ++p) {
     const glamr_person_t& ps = pb.persons[p];
     if (ps.vis[s] == 0.0f) continue;
     // M = Tw @ P2C: R_M = Rw Rp, t_M = Rw tp + tw  ->  dRw = G_R Rp^T + G_t tp^T, dtw = G_t

@@ -20,6 +20,18 @@ namespace glamr {
 
 constexpr int kFrameThreads = 128;
 
+// Partial-sum slots of the loss terms, per seed group (include/glamr_b200.h, glamr_problem_t.G): every group has its own block of
+// `per_group` slots, [res residual CTAs | Q persons | cam camera CTAs of traj_cam_backward_kernel | cam3 CTAs of
+// camera_backward_kernel], and each group's CTAs cover that group's frame-persons / frames exactly as the CTAs of the one-group
+// problem do, so that every group's term sums see the same elements in the same order as its one-group run.
+struct SlotLayout {
+  int res;          // residual CTAs per group: ceil(Q*T / 4)
+  int persons;      // Q = P / G
+  int cam;          // camera CTAs of kScanThreads frames per group (traj_cam_forward / traj_cam_backward)
+  int cam3;         // camera CTAs of kFrameThreads frames per group (camera_backward_kernel, mode 3)
+  int per_group;    // res + persons + cam + cam3
+};
+
 __device__ void block_reduce_terms(const TermAcc& acc, double* out /*[NUM_TERMS]*/, double* smem /*[warps][NUM_TERMS]*/) {
   const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5, nw = blockDim.x >> 5;
 #pragma unroll
@@ -51,16 +63,18 @@ __device__ bool grid_last_block(unsigned int* ticket) {
   return last;
 }
 
-// blocks [0,P): trajectory codec of one person; blocks [P, P+cam_blocks): camera of 256 frames each (modes 0-2)
-__global__ void __launch_bounds__(kScanThreads) traj_cam_forward_kernel(OptCtx c, int with_cam) {
+// blocks [0,P): trajectory codec of one person; blocks [P, P+G*cam_blocks): camera of 256 frames of one group each (modes 0-2)
+__global__ void __launch_bounds__(kScanThreads) traj_cam_forward_kernel(OptCtx c, int with_cam, int cam_blocks) {
   __shared__ float sm[kScanThreads / 32 + 1];
   pdl_launch_dependents();
   pdl_wait();
   // [grad | term sums] of this iteration start from zero (the previous iteration's apply has consumed them)
-  for (int i = blockIdx.x * kScanThreads + threadIdx.x; i < c.pb.n_params + GLAMR_NUM_TERMS; i += gridDim.x * kScanThreads) c.sc.grad[i] = 0.0f;
+  const int n_reduce = c.pb.n_params + num_groups(c.pb) * GLAMR_NUM_TERMS;
+  for (int i = blockIdx.x * kScanThreads + threadIdx.x; i < n_reduce; i += gridDim.x * kScanThreads) c.sc.grad[i] = 0.0f;
   if ((int)blockIdx.x >= c.pb.P) {
-    const int t = (blockIdx.x - c.pb.P) * kScanThreads + threadIdx.x;
-    if (with_cam && t < c.pb.T) cam_forward(c, t);
+    const int b = blockIdx.x - c.pb.P, g = b / cam_blocks;
+    const int t = (b - g * cam_blocks) * kScanThreads + threadIdx.x;
+    if (with_cam && t < c.pb.T) cam_forward(c, g * c.pb.T + t);
     return;
   }
   const int p = blockIdx.x;
@@ -84,32 +98,37 @@ __global__ void __launch_bounds__(kScanThreads) traj_cam_forward_kernel(OptCtx c
 __global__ void __launch_bounds__(kFrameThreads) cam_forward_kernel(OptCtx c) {
   pdl_launch_dependents();
   pdl_wait();
-  const int t = blockIdx.x * blockDim.x + threadIdx.x;
-  if (t < c.pb.T) cam_forward(c, t);
+  const int gt = blockIdx.x * blockDim.x + threadIdx.x;
+  if (gt < num_groups(c.pb) * c.pb.T) cam_forward(c, gt);
 }
 
 // One warp per frame-person: lanes = joints for the SMPL joint assembly (lib/models/smpl.py:299-315, fused here) and the
-// reprojection terms, warp-shuffle sums, then lane 0 finishes the per-frame terms.  4 frame-persons per CTA.
-__global__ void __launch_bounds__(kFrameThreads) frame_residuals_kernel(OptCtx c, SmplDev m, SmplWorkspace wo, int n_begin, double* partial) {
+// reprojection terms, warp-shuffle sums, then lane 0 finishes the per-frame terms.  4 frame-persons of one seed group per CTA:
+// sl.res CTAs per group (the last one of a group may run idle warps), so a group's partial sums match its one-group run.
+__global__ void __launch_bounds__(kFrameThreads) frame_residuals_kernel(OptCtx c, SmplDev m, SmplWorkspace wo, int n_begin, double* partial,
+                                                                        SlotLayout sl) {
   __shared__ double sm[(kFrameThreads / 32) * GLAMR_NUM_TERMS];
   pdl_launch_dependents();
   pdl_wait();
   const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
-  const int n = blockIdx.x * (kFrameThreads / 32) + wid;
-  const int N = c.pb.P * c.pb.T, J = c.pb.J;
+  const int g = blockIdx.x / sl.res, lb = blockIdx.x - g * sl.res;
+  const int Ng = sl.persons * c.pb.T, J = c.pb.J;
+  const int ng = lb * (kFrameThreads / 32) + wid;           // frame-person inside the group
+  const int n = g * Ng + ng;
   GLAMR_STAMP(0);
   TermAcc acc;
   acc.clear();
-  if (n < N) {
+  if (ng < Ng) {
     const int p = n / c.pb.T, t = n - p * c.pb.T;
     if (n >= c.pb.n_begin && n < c.pb.n_end) {
       const int nl = n - n_begin;
       const float* tw = c.sc.trans_world + (size_t)n * 3;
       const float sc = c.pb.scale_all ? c.pb.scale_all[n] : 1.0f;
+      const float* cam = c.sc.cam + cam_row(c, p, t) * 12;
       float root[3], Rc[9], tc[3], Rs[9];
       raw_joint(m, wo, nl, m.joint_map[0], root);
-      mat34_R(c.sc.cam + (size_t)t * 12, Rc);
-      tc[0] = c.sc.cam[(size_t)t * 12 + 3]; tc[1] = c.sc.cam[(size_t)t * 12 + 7]; tc[2] = c.sc.cam[(size_t)t * 12 + 11];
+      mat34_R(cam, Rc);
+      tc[0] = cam[3]; tc[1] = cam[7]; tc[2] = cam[11];
       rodrigues_smplx(c.sc.orient_world + (size_t)n * 3, Rs);
       KpGrad kg;
       kg.clear();
@@ -145,7 +164,7 @@ __global__ void __launch_bounds__(kFrameThreads) frame_residuals_kernel(OptCtx c
   if (threadIdx.x < GLAMR_NUM_TERMS) {
     double s = 0.0;
     for (int w = 0; w < kFrameThreads / 32; ++w) s += sm[w * GLAMR_NUM_TERMS + threadIdx.x];
-    partial[(size_t)blockIdx.x * GLAMR_NUM_TERMS + threadIdx.x] = s;
+    partial[((size_t)g * sl.per_group + lb) * GLAMR_NUM_TERMS + threadIdx.x] = s;
   }
   GLAMR_STAMP(11);
 }
@@ -158,22 +177,24 @@ extern "C" int glamr_exp_frame_stamps(long long* out32) {     // experiment buil
 }
 #endif
 
-__global__ void __launch_bounds__(kFrameThreads) camera_backward_kernel(OptCtx c, double* partial) {
+// sl.cam3 CTAs of kFrameThreads frames per seed group
+__global__ void __launch_bounds__(kFrameThreads) camera_backward_kernel(OptCtx c, double* partial, SlotLayout sl) {
   __shared__ double sm[(kFrameThreads / 32) * GLAMR_NUM_TERMS];
   pdl_launch_dependents();
   pdl_wait();
-  const int t = blockIdx.x * blockDim.x + threadIdx.x;
+  const int g = blockIdx.x / sl.cam3, lb = blockIdx.x - g * sl.cam3;
+  const int t = lb * blockDim.x + threadIdx.x;
   TermAcc acc;
   acc.clear();
-  if (t < c.pb.T) camera_backward(c, t, acc);
-  block_reduce_terms(acc, partial + (size_t)blockIdx.x * GLAMR_NUM_TERMS, sm);
+  if (t < c.pb.T) camera_backward(c, g * c.pb.T + t, acc);
+  block_reduce_terms(acc, partial + ((size_t)g * sl.per_group + sl.res + sl.persons + sl.cam + lb) * GLAMR_NUM_TERMS, sm);
 }
 
 __global__ void __launch_bounds__(kFrameThreads) camera_scatter_kernel(OptCtx c) {
   pdl_launch_dependents();
   pdl_wait();
-  const int s = blockIdx.x * blockDim.x + threadIdx.x;
-  if (s < c.pb.T) camera_scatter_to_persons(c, s);
+  const int gs = blockIdx.x * blockDim.x + threadIdx.x;
+  if (gs < num_groups(c.pb) * c.pb.T) camera_scatter_to_persons(c, gs);
 }
 
 // ---- cross-GPU reduction over NVLink peer memory (one process per GPU, buffers exchanged as CUDA IPC handles) --------
@@ -220,48 +241,60 @@ __device__ __forceinline__ float peer_take(const PeerCtx& pc, uint32_t e, int sr
   return __uint_as_float((uint32_t)w);
 }
 
-// loss partials -> un-normalised term sums (reduce_buf tail); fixed camera: sum the per-frame gradients over T
-__device__ void reduce_tail(const OptCtx& c, const double* partial, int n_slots, float* reduce_buf, double* sm /*[8*16]*/) {
+// loss partials -> un-normalised term sums of every group (reduce_buf tail: the first n_slots slots of each group's block, in slot
+// order); fixed camera: each group's per-frame gradients summed over its T frames
+__device__ void reduce_tail(const OptCtx& c, const double* partial, int n_slots, int per_group, float* reduce_buf, double* sm /*[8*16]*/) {
   const int tid = threadIdx.x, lane = tid & 31, wid = tid >> 5;
-  if (tid < GLAMR_NUM_TERMS) {
+  const int G = num_groups(c.pb);
+  for (int i = tid; i < G * GLAMR_NUM_TERMS; i += blockDim.x) {
+    const int g = i / GLAMR_NUM_TERMS, k0 = i - g * GLAMR_NUM_TERMS;
+    const double* pg = partial + (size_t)g * per_group * GLAMR_NUM_TERMS;
     double s = 0.0;
-    for (int k = 0; k < n_slots; ++k) s += partial[(size_t)k * GLAMR_NUM_TERMS + tid];
-    reduce_buf[c.pb.n_params + tid] = (float)s;
+    for (int k = 0; k < n_slots; ++k) s += pg[(size_t)k * GLAMR_NUM_TERMS + k0];
+    reduce_buf[c.pb.n_params + i] = (float)s;
   }
   if (c.pb.cam_mode == GLAMR_CAM_FIXED) {
-    double a[9];
-    for (int k = 0; k < 9; ++k) a[k] = 0.0;
-    for (int t = tid; t < c.pb.T; t += blockDim.x)
-      for (int k = 0; k < 9; ++k) a[k] += (double)c.sc.g_cam_fix[(size_t)t * 12 + k];
-    for (int k = 0; k < 9; ++k) {
-      const double s = warp_sum(a[k]);
-      if (lane == 0) sm[wid * 16 + k] = s;
-    }
-    __syncthreads();
-    if (tid < 9) {
-      double s = 0.0;
-      for (int w = 0; w < (int)(blockDim.x >> 5); ++w) s += sm[w * 16 + tid];
-      const int off = (tid < 6) ? c.pb.off_cam_rot + tid : c.pb.off_cam_trans + (tid - 6);
-      reduce_buf[off] = (float)s;
+    for (int g = 0; g < G; ++g) {
+      const float* gcf = c.sc.g_cam_fix + (size_t)g * c.pb.T * 12;
+      double a[9];
+      for (int k = 0; k < 9; ++k) a[k] = 0.0;
+      for (int t = tid; t < c.pb.T; t += blockDim.x)
+        for (int k = 0; k < 9; ++k) a[k] += (double)gcf[(size_t)t * 12 + k];
+      for (int k = 0; k < 9; ++k) {
+        const double s = warp_sum(a[k]);
+        if (lane == 0) sm[wid * 16 + k] = s;
+      }
+      __syncthreads();
+      if (tid < 9) {
+        double s = 0.0;
+        for (int w = 0; w < (int)(blockDim.x >> 5); ++w) s += sm[w * 16 + tid];
+        const int off = group_theta(c.pb, g) + ((tid < 6) ? c.pb.off_cam_rot + tid : c.pb.off_cam_trans + (tid - 6));
+        reduce_buf[off] = (float)s;
+      }
+      __syncthreads();          // sm is rewritten by the next group
     }
   }
 }
 
-// blocks [0,P): reverse trajectory codec of one person; blocks [P, P+cam_blocks): camera backward of 256 frames (modes
-// 0-2; mode 3 runs camera_backward/scatter kernels first).  The last CTA to finish folds all partial sums.
-__global__ void __launch_bounds__(kScanThreads, 1) traj_cam_backward_kernel(OptCtx c, int with_cam, double* partial_traj, const double* partial_all,
-                                                                         int n_slots, float* reduce_buf, unsigned int* ticket, PeerCtx pc) {
+// blocks [0,P): reverse trajectory codec of one person; blocks [P, P+G*sl.cam): camera backward of 256 frames of one group
+// (modes 0-2; mode 3 runs camera_backward/scatter kernels first).  The last CTA to finish folds all partial sums.
+__global__ void __launch_bounds__(kScanThreads, 1) traj_cam_backward_kernel(OptCtx c, int with_cam, double* partial, int n_slots, SlotLayout sl,
+                                                                         float* reduce_buf, unsigned int* ticket, PeerCtx pc) {
   __shared__ float sm[kScanThreads / 32 + 1];
   __shared__ double smd[(kScanThreads / 32) * GLAMR_NUM_TERMS];
   pdl_launch_dependents();
   pdl_wait();
   TermAcc acc;
   acc.clear();
+  size_t slot;
   if ((int)blockIdx.x >= c.pb.P) {
-    const int t = (blockIdx.x - c.pb.P) * kScanThreads + threadIdx.x;
-    if (with_cam && t < c.pb.T) camera_backward(c, t, acc);
+    const int b = blockIdx.x - c.pb.P, g = b / sl.cam, lb = b - g * sl.cam;
+    const int t = lb * kScanThreads + threadIdx.x;
+    if (with_cam && t < c.pb.T) camera_backward(c, g * c.pb.T + t, acc);
+    slot = (size_t)g * sl.per_group + sl.res + sl.persons + lb;
   } else {
-    const int p = blockIdx.x;
+    const int p = blockIdx.x, g = p / sl.persons;
+    slot = (size_t)g * sl.per_group + sl.res + (p - g * sl.persons);
     const glamr_person_t& ps = c.pb.persons[p];
     const int len = ps.len, T = c.pb.T;
     const size_t n0 = (size_t)p * T + ps.start;
@@ -281,9 +314,9 @@ __global__ void __launch_bounds__(kScanThreads, 1) traj_cam_backward_kernel(OptC
     }
     for (int i = threadIdx.x; i < len; i += kScanThreads) traj_back_post(c, p, i, acc);
   }
-  block_reduce_terms(acc, partial_traj + (size_t)blockIdx.x * GLAMR_NUM_TERMS, smd);
+  block_reduce_terms(acc, partial + slot * GLAMR_NUM_TERMS, smd);
   if (grid_last_block(ticket)) {
-    reduce_tail(c, partial_all, n_slots, reduce_buf, smd);
+    reduce_tail(c, partial, n_slots, sl.per_group, reduce_buf, smd);
   }
 }
 
@@ -323,8 +356,10 @@ __device__ void write_losses(const OptCtx& c, const float* term_sums /*[NUM_TERM
   loss_terms[GLAMR_NUM_TERMS] = (float)total;
 }
 
+// thread g: the loss terms of seed group g
 __global__ void __launch_bounds__(32) losses_kernel(OptCtx c, const float* __restrict__ reduce_buf, float* __restrict__ loss_terms) {
-  if (threadIdx.x == 0) write_losses(c, reduce_buf + c.pb.n_params, loss_terms);
+  for (int g = threadIdx.x; g < num_groups(c.pb); g += blockDim.x)
+    write_losses(c, reduce_buf + c.pb.n_params + g * GLAMR_NUM_TERMS, loss_terms + g * (GLAMR_NUM_TERMS + 1));
 }
 
 // loss terms (block 0) + torch.optim.Adam step; the last CTA to finish advances the step count / beta powers.
@@ -340,7 +375,7 @@ __global__ void __launch_bounds__(256) apply_kernel(OptCtx c, float* __restrict_
     // with the iteration number in the same 8-byte word, into slot (epoch & 1), source row `rank`, of every rank's buffer.  All
     // pushes of a rank are issued before any of its threads starts polling, so ranks never wait on each other circularly.
     const size_t row = peer_row(pc, epoch, pc.rank);
-    const int count = c.pb.n_params + GLAMR_NUM_TERMS;
+    const int count = c.pb.n_params + num_groups(c.pb) * GLAMR_NUM_TERMS;
     for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < count; i += gridDim.x * blockDim.x) {
       const unsigned long long w = ((unsigned long long)epoch << 32) | (unsigned long long)__float_as_uint(reduce_buf[i]);
       for (int r = 0; r < pc.world; ++r) st_peer_u64(pc.bufs[r] + row + i, w);
@@ -353,10 +388,10 @@ __global__ void __launch_bounds__(256) apply_kernel(OptCtx c, float* __restrict_
     for (int r = 0; r < pc.world; ++r) g += peer_take(pc, epoch, r, i);
     return g;
   };
-  if (blockIdx.x == 0 && threadIdx.x == 0 && loss_terms) {
+  for (int g = threadIdx.x; blockIdx.x == 0 && g < num_groups(c.pb) && loss_terms; g += blockDim.x) {   // the loss terms of seed group g
     float sums[GLAMR_NUM_TERMS];
-    for (int k = 0; k < GLAMR_NUM_TERMS; ++k) sums[k] = grad_at(c.pb.n_params + k);
-    write_losses(c, sums, loss_terms + (hist_stride > 0 ? (size_t)step * hist_stride : 0));
+    for (int k = 0; k < GLAMR_NUM_TERMS; ++k) sums[k] = grad_at(c.pb.n_params + g * GLAMR_NUM_TERMS + k);
+    write_losses(c, sums, loss_terms + (hist_stride > 0 ? (size_t)step * hist_stride : 0) + g * (GLAMR_NUM_TERMS + 1));
   }
   const float bc2s = (float)sqrt(1.0 - b2);
   const float step_size = (float)(lr / (1.0 - b1));
@@ -390,7 +425,7 @@ struct glamr_opt {
   SmplWorkspace ws;
   AdamState adam;
   double* partial;
-  int n_slots, slots_res, slots_cam, cam_blocks;   // partial-sum slots: residual CTAs | P + cam_blocks (traj/cam kernel) | slots_cam (mode 3)
+  SlotLayout sl;                                   // partial-sum slots of one seed group; G blocks of sl.per_group
   unsigned int* tickets;                           // [0] backward tail, [1] apply, [3] peer all-reduce ([2] unused)
   void* arena;
   size_t arena_bytes;
@@ -436,30 +471,43 @@ static OptCtx make_ctx(const glamr_opt* st, const float* theta, float* grad) {
   return c;
 }
 
+// seed groups: P splits into G equal groups; with several groups every frame-person lives on this rank, and theta holds G
+// equal blocks
+static bool groups_valid(const glamr_problem_t* pb) {
+  const int G = num_groups(*pb);
+  if (pb->P % G != 0) return false;
+  if (G == 1) return true;
+  return pb->n_begin == 0 && pb->n_end == pb->P * pb->T && pb->owner && pb->group_params > 0 &&
+         (long long)pb->group_params * G == (long long)pb->n_params;
+}
+
 extern "C" int glamr_opt_create(glamr_opt_t** out, const glamr_smpl_t* smpl, const glamr_problem_t* pb) {
   if (!out || !smpl || !pb || pb->P <= 0 || pb->T <= 0 || pb->J <= 0 || pb->n_params <= 0) return GLAMR_EINVAL;
   if (pb->J != smpl->dev.n_map) return GLAMR_EINVAL;
   if (pb->traj_source != GLAMR_TRAJ_PREDICTED && pb->traj_source != GLAMR_TRAJ_BASE) return GLAMR_EINVAL;
+  if (!groups_valid(pb)) return GLAMR_EINVAL;
   glamr_opt* st = (glamr_opt*)calloc(1, sizeof(glamr_opt));
   if (!st) return GLAMR_EINVAL;
   st->smpl = smpl->dev;
   st->pb = *pb;
   compute_gs(st);
-  const size_t N = (size_t)pb->P * pb->T, T = pb->T, J = pb->J;
-  st->slots_res = (int)((N + kFrameThreads / 32 - 1) / (kFrameThreads / 32));
-  st->slots_cam = (int)((T + kFrameThreads - 1) / kFrameThreads);
-  st->cam_blocks = (int)((T + kScanThreads - 1) / kScanThreads);
-  st->n_slots = st->slots_res + pb->P + st->cam_blocks + st->slots_cam;
+  const size_t N = (size_t)pb->P * pb->T, T = pb->T, J = pb->J, G = num_groups(*pb);
+  const size_t GT = G * T;                 // camera rows of all groups
+  st->sl.persons = pb->P / (int)G;
+  st->sl.res = (int)(((size_t)st->sl.persons * T + kFrameThreads / 32 - 1) / (kFrameThreads / 32));
+  st->sl.cam3 = (int)((T + kFrameThreads - 1) / kFrameThreads);
+  st->sl.cam = (int)((T + kScanThreads - 1) / kScanThreads);
+  st->sl.per_group = st->sl.res + st->sl.persons + st->sl.cam + st->sl.cam3;
   // one arena for all scratch (floats), doubles first for alignment
   size_t floats = 0;
   auto take = [&](size_t nfl) { size_t o = floats; floats += (nfl + 63) & ~(size_t)63; return o; };
-  const size_t o_partial = take((size_t)st->n_slots * GLAMR_NUM_TERMS * 2);
+  const size_t o_partial = take(G * st->sl.per_group * GLAMR_NUM_TERMS * 2);
   const size_t o_beta = take(8);
   const size_t o_ticket = take(4);
   const size_t o_heading = take(N), o_xy = take(2 * N), o_tl = take(11 * N), o_ob = take(3 * N), o_tb = take(3 * N),
-               o_ow = take(3 * N), o_tw = take(3 * N), o_cam = take(12 * T), o_caminv = take(12 * T), o_camd6 = take(6 * T),
+               o_ow = take(3 * N), o_tw = take(3 * N), o_cam = take(12 * GT), o_caminv = take(12 * GT), o_camd6 = take(6 * GT),
                o_jw = take(N * J * 3), o_kp = take(N * J * 2), o_ociw = take(3 * N), o_tciw = take(3 * N), o_go = take(3 * N),
-               o_gt = take(3 * N), o_gcam = take(12 * N), o_gcf = take(12 * T), o_gxy = take(2 * N), o_gh = take(N),
+               o_gt = take(3 * N), o_gcam = take(12 * N), o_gcf = take(12 * GT), o_gxy = take(2 * N), o_gh = take(N),
                o_m = take(pb->n_params), o_v = take(pb->n_params);
   const size_t o_ws = take(smpl_workspace_floats((int)N, smpl->dev.S));
   {
@@ -604,6 +652,7 @@ static int join_pending(glamr_opt_t* st, cudaStream_t s);
 extern "C" int glamr_opt_set_problem(glamr_opt_t* st, const glamr_problem_t* pb, int reset_adam, void* stream) {
   if (!st || !pb) return GLAMR_EINVAL;
   if (pb->P != st->pb.P || pb->T != st->pb.T || pb->J != st->pb.J || pb->n_params != st->pb.n_params) return GLAMR_EINVAL;
+  if (num_groups(*pb) != num_groups(st->pb) || !groups_valid(pb)) return GLAMR_EINVAL;
   if (pb->traj_source != GLAMR_TRAJ_PREDICTED && pb->traj_source != GLAMR_TRAJ_BASE) return GLAMR_EINVAL;
   {
     const int rc = join_pending(st, (cudaStream_t)stream);
@@ -634,7 +683,9 @@ extern "C" int glamr_opt_set_problem(glamr_opt_t* st, const glamr_problem_t* pb,
   return GLAMR_OK;
 }
 
-extern "C" size_t glamr_opt_reduce_count(const glamr_opt_t* st) { return st ? (size_t)st->pb.n_params + GLAMR_NUM_TERMS : 0; }
+extern "C" size_t glamr_opt_reduce_count(const glamr_opt_t* st) {
+  return st ? (size_t)st->pb.n_params + (size_t)num_groups(st->pb) * GLAMR_NUM_TERMS : 0;
+}
 
 // the tensor-core skinning runs in two launches, the support tiles on the iteration's critical path and the mesh tiles on the side stream
 static bool skin_split(const glamr_opt_t* st) { return lbs_path() >= 1 && st->smpl.tcB != nullptr && st->ws.vp_tiled; }
@@ -740,10 +791,13 @@ static int backward_impl(glamr_opt_t* st, const float* theta, float* reduce_buf,
       if (rc) return rc;
     }
   }
-  GLAMR_CUDA_TRY(launch_pdl(1, traj_cam_forward_kernel, dim3(pb.P + st->cam_blocks), dim3(kScanThreads), 0, s, c, from_persons ? 0 : 1));   // also zeroes reduce_buf
+  const SlotLayout sl = st->sl;
+  const int G = num_groups(pb);
+  const int cam_rows_ctas = (G * pb.T + kFrameThreads - 1) / kFrameThreads;      // one thread per camera row of every group
+  GLAMR_CUDA_TRY(launch_pdl(1, traj_cam_forward_kernel, dim3(pb.P + G * sl.cam), dim3(kScanThreads), 0, s, c, from_persons ? 0 : 1, sl.cam));   // also zeroes reduce_buf
   GLAMR_MARK();
   if (from_persons) {          // the camera is the mean of the persons' world transforms: needs traj_forward of all persons
-    GLAMR_CUDA_TRY(launch_pdl(1, cam_forward_kernel, dim3(st->slots_cam), dim3(kFrameThreads), 0, s, c));
+    GLAMR_CUDA_TRY(launch_pdl(1, cam_forward_kernel, dim3(cam_rows_ctas), dim3(kFrameThreads), 0, s, c));
   }
   GLAMR_MARK();
   if (n_end > n_begin) {
@@ -784,21 +838,18 @@ static int backward_impl(glamr_opt_t* st, const float* theta, float* reduce_buf,
     }
     GLAMR_MARK();
   }
-  double* part_res = st->partial;
-  double* part_traj = st->partial + (size_t)st->slots_res * GLAMR_NUM_TERMS;
-  double* part_cam3 = part_traj + (size_t)(pb.P + st->cam_blocks) * GLAMR_NUM_TERMS;
   if (!(exp_skip & 4))
-    GLAMR_CUDA_TRY(launch_pdl(8, frame_residuals_kernel, dim3(st->slots_res), dim3(kFrameThreads), 0, s, c, st->smpl, wo, n_begin, part_res));
+    GLAMR_CUDA_TRY(launch_pdl(8, frame_residuals_kernel, dim3(G * sl.res), dim3(kFrameThreads), 0, s, c, st->smpl, wo, n_begin, st->partial, sl));
   GLAMR_MARK();
   if (from_persons) {
-    GLAMR_CUDA_TRY(launch_pdl(16, camera_backward_kernel, dim3(st->slots_cam), dim3(kFrameThreads), 0, s, c, part_cam3));
-    GLAMR_CUDA_TRY(launch_pdl(16, camera_scatter_kernel, dim3(st->slots_cam), dim3(kFrameThreads), 0, s, c));
+    GLAMR_CUDA_TRY(launch_pdl(16, camera_backward_kernel, dim3(G * sl.cam3), dim3(kFrameThreads), 0, s, c, st->partial, sl));
+    GLAMR_CUDA_TRY(launch_pdl(16, camera_scatter_kernel, dim3(cam_rows_ctas), dim3(kFrameThreads), 0, s, c));
     GLAMR_MARK();
   }
-  const int n_slots = st->slots_res + pb.P + st->cam_blocks + (from_persons ? st->slots_cam : 0);
+  const int n_slots = sl.res + sl.persons + sl.cam + (from_persons ? sl.cam3 : 0);      // slots of each group that hold partial sums
   if (!(exp_skip & 8))
-    GLAMR_CUDA_TRY(launch_pdl(16, traj_cam_backward_kernel, dim3(pb.P + st->cam_blocks), dim3(kScanThreads), 0, s, c, from_persons ? 0 : 1, part_traj,
-                              (const double*)st->partial, n_slots, reduce_buf, st->tickets, pc));
+    GLAMR_CUDA_TRY(launch_pdl(16, traj_cam_backward_kernel, dim3(pb.P + G * sl.cam), dim3(kScanThreads), 0, s, c, from_persons ? 0 : 1, st->partial,
+                              n_slots, sl, reduce_buf, st->tickets, pc));
   GLAMR_MARK();
   if (forked) {
     if (defer_join) st->join_pending = 1;
@@ -877,7 +928,7 @@ extern "C" int glamr_peer_free(void* dev_ptr) {
 }
 extern "C" size_t glamr_opt_peer_bytes(const glamr_opt_t* st) {
   if (!st) return 0;
-  const size_t slot = ((size_t)st->pb.n_params + GLAMR_NUM_TERMS + 63) & ~(size_t)63;
+  const size_t slot = (glamr_opt_reduce_count(st) + 63) & ~(size_t)63;
   return kPeerHeaderWords * sizeof(uint32_t) + 2 * (size_t)GLAMR_MAX_PEERS * slot * sizeof(unsigned long long);
 }
 extern "C" int glamr_opt_set_peers(glamr_opt_t* st, int rank, int world, void* const* bufs) {
@@ -887,7 +938,7 @@ extern "C" int glamr_opt_set_peers(glamr_opt_t* st, int rank, int world, void* c
   if (world <= 1) return GLAMR_OK;
   st->peer.rank = rank;
   st->peer.world = world;
-  st->peer.slot_elems = ((size_t)st->pb.n_params + GLAMR_NUM_TERMS + 63) & ~(size_t)63;
+  st->peer.slot_elems = (glamr_opt_reduce_count(st) + 63) & ~(size_t)63;
   for (int r = 0; r < world; ++r) {
     if (!bufs[r]) return GLAMR_EINVAL;
     st->peer.bufs[r] = (unsigned long long*)bufs[r];
@@ -948,7 +999,7 @@ extern "C" int glamr_opt_iterate(glamr_opt_t* st, float* theta, float* reduce_bu
 
 extern "C" int glamr_opt_read(glamr_opt_t* st, int what, const float** ptr, size_t* count) {
   if (!st || !ptr || !count) return GLAMR_EINVAL;
-  const size_t N = (size_t)st->pb.P * st->pb.T, T = st->pb.T, J = st->pb.J;
+  const size_t N = (size_t)st->pb.P * st->pb.T, T = (size_t)num_groups(st->pb) * st->pb.T, J = st->pb.J;   // T: camera rows of all groups
   switch (what) {
     case GLAMR_R_ORIENT_WORLD: *ptr = st->sc.orient_world; *count = 3 * N; break;
     case GLAMR_R_TRANS_WORLD: *ptr = st->sc.trans_world; *count = 3 * N; break;

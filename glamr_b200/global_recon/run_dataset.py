@@ -9,6 +9,10 @@ Pose estimation (HybrIK), visualisation and evaluation are out of scope (SURVEY.
 Independent sequences are replicas (SURVEY.md §8e, BASELINE config 5): under ``torchrun`` rank r takes sequences
 r, r + world, ... on its own GPU; there is no collective on the data path.
 
+``--batch_seeds`` optimises the seeds of a sequence together, one ``optimize_seeds`` call per sequence instead of one
+``optimize`` call per seed: same files, same contents; each seed's recorded time is the call's time divided by the number of
+seeds it ran.
+
     python -m glamr_b200.global_recon.run_dataset --cfg glamr_3dpw --synthetic 32 --frames 300 --out_dir out/sweep
     python -m torch.distributed.run --nproc-per-node 8 --master-addr 127.0.0.1 -m glamr_b200.global_recon.run_dataset ...
 """
@@ -97,7 +101,36 @@ def run(args, make_model=None, make_in_dict=None):
     seeds = [int(x) for x in str(args.seeds).split(',')]
     done = []
     mine = shard(list_sequences(args), rank, world)
+    def load(seq_name):
+        if make_in_dict is not None:
+            return make_in_dict(seq_name)
+        gt_file = os.path.join(args.gt_pose_root, f'{seq_name}.pkl') if args.gt_pose_root else None
+        return load_in_dict(find_pose_file(args.pose_root, seq_name), seq_name, gt_file)
+
     for i, seq_name in enumerate(mine):
+        if args.batch_seeds:
+            todo = []
+            for seed in seeds:
+                out_file = out_file_of(args.out_dir, seq_name, seed)
+                if args.cached and os.path.exists(out_file):
+                    done.append((seq_name, seed, out_file, 0.0))
+                else:
+                    todo.append((seed, out_file))
+            if not todo:
+                continue
+            in_dict = load(seq_name)
+            t0 = time.perf_counter()
+            outs = model.optimize_seeds(in_dict, [seed for seed, _ in todo])       # sets the RNGs of every seed itself
+            dt = (time.perf_counter() - t0) / len(todo)
+            for (seed, out_file), out_dict in zip(todo, outs):
+                os.makedirs(os.path.dirname(out_file), exist_ok=True)
+                with open(out_file, 'wb') as f:
+                    pickle.dump(out_dict, f)
+                done.append((seq_name, seed, out_file, dt))
+                if not args.quiet:
+                    print(f'[rank {rank}] {i + 1}/{len(mine)} seed {seed} {seq_name}: {dt * 1e3:.1f} ms (batch of {len(todo)}) -> {out_file}',
+                          flush=True)
+            continue
         for seed in seeds:
             out_file = out_file_of(args.out_dir, seq_name, seed)
             if args.cached and os.path.exists(out_file):
@@ -110,11 +143,7 @@ def run(args, make_model=None, make_in_dict=None):
                 torch.manual_seed(seed)
             except ImportError:
                 pass
-            if make_in_dict is not None:
-                in_dict = make_in_dict(seq_name)
-            else:
-                gt_file = os.path.join(args.gt_pose_root, f'{seq_name}.pkl') if args.gt_pose_root else None
-                in_dict = load_in_dict(find_pose_file(args.pose_root, seq_name), seq_name, gt_file)
+            in_dict = load(seq_name)
             t0 = time.perf_counter()
             out_dict = model.optimize(in_dict)
             dt = time.perf_counter() - t0
@@ -141,6 +170,7 @@ def parse(argv=None):
     ap.add_argument('--persons', type=int, default=1)
     ap.add_argument('--gaps', action='store_true', help='synthetic sequences with occlusion gaps')
     ap.add_argument('--real_assets', action='store_true', help='with --synthetic: still load SMPL files / checkpoints from disk')
+    ap.add_argument('--batch_seeds', action='store_true', help='optimise all seeds of a sequence in one optimize_seeds call')
     ap.add_argument('--quiet', action='store_true')
     return ap.parse_args(argv)
 

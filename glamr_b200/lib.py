@@ -44,7 +44,7 @@ _vp = ctypes.c_void_p
 
 class Person(ctypes.Structure):
     _fields_ = [(n, ctypes.c_int32) for n in
-                ['start', 'len', 'off_xy', 'off_heading', 'off_dxy', 'off_dheading', 'off_z', 'off_rot',
+                ['start', 'len', 'group', 'off_xy', 'off_heading', 'off_dxy', 'off_dheading', 'off_z', 'off_rot',
                  'off_world_dheading', 'off_orient_res', 'off_trans_res', 'off_world_dxy', 'off_p2c_rot', 'off_p2c_trans']] + \
                [(n, _vp) for n in
                 ['traj_local_pred', 'orient_base_init', 'trans_base_init', 'cam_K', 'kp_target', 'orient_cam_6d',
@@ -56,7 +56,7 @@ class Problem(ctypes.Structure):
     _fields_ = [(n, ctypes.c_int32) for n in
                 ['P', 'T', 'J', 'cam_mode', 'off_cam_rot', 'off_cam_trans', 'use_world_res', 'has_world_dheading',
                  'trans_res_all', 'cam_up_first_only', 'n_params', 'n_begin', 'n_end', 'owner', 'cam_traj_rot_quat', 'traj_rot_smooth_quat',
-                 'traj_source', 'heading_vec', 'has_world_dxy', 'world_dxy_alias', 'has_person2cam']] + \
+                 'traj_source', 'heading_vec', 'has_world_dxy', 'world_dxy_alias', 'has_person2cam', 'G', 'group_params']] + \
                [('cam_up_first_weight', ctypes.c_float), ('rel_trans_weight', ctypes.c_float),
                 ('term_weight', ctypes.c_float * NUM_TERMS), ('term_norm', ctypes.c_float * NUM_TERMS),
                 ('term_enabled', ctypes.c_int32 * NUM_TERMS), ('term_monitor', ctypes.c_int32 * NUM_TERMS)] + \

@@ -7,6 +7,11 @@
 * ``StageCompiler`` turns ``loss_cfg`` (global_recon/models/loss_func.py semantics: min_conf, first_frame_only,
   first_frame_weight, visibility masks, normalisers) into per-frame weight arrays and scalar term tables.
 
+Seed groups: ``make_layout`` / ``bind_variables`` / ``begin_stage_variables`` / ``StageCompiler`` also take a list of G data
+dicts, the seeds of one sequence (same persons, frames, visibility and loss normalisers, each with its own initial state).  theta
+then holds group 0's blocks, group 1's, and so on; the G*Q persons are simply more persons, each with its group index
+(include/glamr_b200.h, glamr_problem_t.G).  One dict is one group, with exactly the layout it always had.
+
 Pure tensor bookkeeping, device agnostic (tests build it on the CPU for the host harness); nothing here computes
 on the optimisation path.
 """
@@ -19,10 +24,12 @@ from . import lib as L
 
 
 class VariableLayout:
-    def __init__(self, T, n_empty, trans_res_rows, lens, heading_dim=1, world_dxy=False, person2cam=False):
+    def __init__(self, T, n_empty, trans_res_rows, lens, heading_dim=1, world_dxy=False, person2cam=False, groups=1):
         """heading_dim 2: heading_type 'vec' (traj_local_heading [2], traj_local_dheading [L-1,2]); world_dxy: every person also
         gets a world_dxy [T,2] block (only when a stage can create it, so other problems keep their layout); person2cam: every
-        person also gets person2cam_res_rot [T,6] and person2cam_res_trans [T,3] (only when init_data creates them)"""
+        person also gets person2cam_res_rot [T,6] and person2cam_res_trans [T,3] (only when init_data creates them).
+        groups G: `lens` are the Q persons of one group; theta holds G copies of the one-group layout, group g's at
+        g * group_params, and `persons` / `lens` list the G*Q persons group by group."""
         self.T, self.n_empty, self.trans_res_rows, self.lens = T, n_empty, trans_res_rows, list(lens)
         self.heading_dim, self.world_dxy, self.person2cam = heading_dim, bool(world_dxy), bool(person2cam)
         hd = heading_dim
@@ -42,13 +49,20 @@ class VariableLayout:
                                      rot=take(6 * Ln), world_dheading=take(T), orient_res=take(3 * T), trans_res=take(3 * T),
                                      world_dxy=take(2 * T if self.world_dxy else 0),
                                      p2c_rot=take(6 * T if self.person2cam else 0), p2c_trans=take(3 * T if self.person2cam else 0)))
-        self.n_params = off
+        self.G, self.Q, self.group_params = int(groups), len(self.lens), off
+        one = list(self.persons)
+        for g in range(1, self.G):
+            self.persons += [{k: o + g * off for k, o in d.items()} for d in one]
+        self.lens = self.lens * self.G
+        self.n_params = self.G * off
 
-    def views(self, theta, p=None):
-        """name -> view of theta with the reference's tensor shape"""
+    def views(self, theta, p=None, group=0):
+        """name -> view of theta with the reference's tensor shape: the camera variables of `group` (p None), else those of
+        person p (counted over all groups)"""
         T = self.T
         if p is None:
-            v = lambda o, n, *shape: theta[o:o + n].view(*shape)
+            g0 = group * self.group_params
+            v = lambda o, n, *shape: theta[g0 + o:g0 + o + n].view(*shape)
             return {'cam_rot_6d': v(self.cam_rot, 6 * T, T, 6), 'cam_trans': v(self.cam_trans, 3 * T, T, 3),
                     'cam_rot_6d_fix': v(self.cam_rot_fix, 6, 1, 6), 'cam_trans_fix': v(self.cam_trans_fix, 3, 1, 3),
                     'cam_inv_rot_residual': v(self.cam_inv_rot_res, 6 * self.n_empty, self.n_empty, 6),
@@ -73,20 +87,32 @@ def _f32(x, device):
     return torch.as_tensor(x).to(device=device, dtype=torch.float32).contiguous()
 
 
+def _groups(data):
+    """one data dict, or the list of the seed groups' data dicts -> list"""
+    return list(data) if isinstance(data, (list, tuple)) else [data]
+
+
 class StageCompiler:
     """Holds the per-person constant tensors and builds a ``Problem`` for every stage."""
 
     def __init__(self, data, layout, flags, device, aa_to_rot6d, num_joints=26, aa_to_quat=None):
-        """flags: dict with flag_fixed_cam, flag_opt_cam, flag_opt_cam_from_person_pose, flag_cam_inv_trans_res_all,
+        """data: one data dict, or the list of the seed groups' data dicts (see the module docstring).
+        flags: dict with flag_fixed_cam, flag_opt_cam, flag_opt_cam_from_person_pose, flag_cam_inv_trans_res_all,
         flag_opt_vis_local_rot, cam_fix_frames and optionally flag_opt_traj / traj_source (when absent they are read off
         `data`: a predicted trajectory leaves traj_local_pred, flag_opt_traj leaves the world_res variables), heading_vec
         (heading_type 'vec'; default: the layout's heading size) and flag_opt_person2cam_rot / _trans (default false).
         aa_to_rot6d: callable (device math lives in the CUDA library)."""
+        self.datas = _groups(data)
+        data = self.datas[0]
         self.data, self.layout, self.flags, self.device, self.J = data, layout, flags, device, num_joints
         self.pids = list(data['person_data'].keys())
-        self.P, self.T = len(self.pids), data['seq_len']
+        self.G, self.Q, self.T = len(self.datas), len(self.pids), data['seq_len']
+        self.P = self.G * self.Q                     # persons of all groups, group by group
         T, dev = self.T, device
-        persons = [data['person_data'][pid] for pid in self.pids]
+        persons = [d for dd in self.datas for d in dd['person_data'].values()]
+        if any(len(dd['person_data']) != self.Q or dd['seq_len'] != T for dd in self.datas):
+            raise ValueError('seed groups need the same persons and frame count')
+        self.persons = persons
         self.traj_source = flags.get('traj_source', L.TRAJ_PREDICTED if all('traj_local_pred' in d for d in persons) else L.TRAJ_BASE)
         self.opt_traj = flags.get('flag_opt_traj', all('smpl_orient_world_res' in d for d in persons))
         self.has_local = all('traj_local_xy' in d for d in persons)        # created with flag_opt_traj and flag_pred_traj (:185-199)
@@ -94,8 +120,7 @@ class StageCompiler:
         self.keep = []                               # tensors whose storage the structs point into
         self.const = []
         pose_all, beta_all, scale_all = [], [], []
-        for pid in self.pids:
-            d = data['person_data'][pid]
+        for d in persons:
             start, Ln = int(d['fr_start']), int(d['exist_len'])
             mask = torch.ones(max(Ln - 1, 0))
             for (s, e) in flags['cam_fix_frames']:
@@ -127,33 +152,35 @@ class StageCompiler:
         self.scale_all = None if scale_all[0] is None else torch.stack(scale_all).contiguous()
         # host copies of what the per-stage weight tables are built from (visibility, keypoint scores, persons per frame):
         # ONE device->host copy here instead of several per person and stage
-        P_, J_ = self.P, self.J
-        packed = torch.cat([torch.stack([torch.as_tensor(data['person_data'][pid]['vis_frames']).to(dev).double() for pid in self.pids]).reshape(-1),
-                            torch.stack([torch.as_tensor(data['person_data'][pid]['kp_2d_score']).to(dev).double() for pid in self.pids]).reshape(-1),
-                            torch.as_tensor(data['fr_num_persons']).to(dev).double().reshape(-1)]).cpu()
+        P_, J_, G_, Q_ = self.P, self.J, self.G, self.Q
+        packed = torch.cat([torch.stack([torch.as_tensor(d['vis_frames']).to(dev).double() for d in persons]).reshape(-1),
+                            torch.stack([torch.as_tensor(d['kp_2d_score']).to(dev).double() for d in persons]).reshape(-1),
+                            torch.stack([torch.as_tensor(dd['fr_num_persons']).to(dev).double().reshape(-1) for dd in self.datas]).reshape(-1)]).cpu()
         self.host_vis = packed[:P_ * T].reshape(P_, T) > 0.5
         self.host_score = packed[P_ * T:P_ * T + P_ * T * J_].reshape(P_, T, J_)
-        # camera-from-persons bookkeeping (global_recon_model.py:489-506)
-        npers = packed[P_ * T + P_ * T * J_:].to(torch.int64)
-        has = npers > 0
-        first = int(torch.where(has)[0][0])
-        src, empty_idx, last, ne = [], [], first, 0
-        for t in range(T):
-            if npers[t] > 0:
-                last = t
-                empty_idx.append(-1)
-            else:
-                empty_idx.append(ne)
-                ne += 1
-            src.append(last)
+        # camera-from-persons bookkeeping (global_recon_model.py:489-506), one [T] block per group
+        src, empty_idx, inv_num = [], [], []
+        for npers in packed[P_ * T + P_ * T * J_:].to(torch.int64).reshape(G_, T):
+            has = npers > 0
+            last, ne = int(torch.where(has)[0][0]), 0
+            for t in range(T):
+                if npers[t] > 0:
+                    last = t
+                    empty_idx.append(-1)
+                else:
+                    empty_idx.append(ne)
+                    ne += 1
+                src.append(last)
+            inv_num.append(torch.where(has, 1.0 / npers.clamp(min=1).float(), torch.zeros(T)))
         self.fill_src = torch.tensor(src, dtype=torch.int32, device=dev)
         self.empty_index = torch.tensor(empty_idx, dtype=torch.int32, device=dev)
-        self.inv_num = _f32(torch.where(has, 1.0 / npers.clamp(min=1).float(), torch.zeros(T)), dev)
-        rel = data.get('rel_transform_cam')
-        if rel:
-            tgt = torch.zeros(self.P * self.P, T, 12, device=dev)
-            for (i, j), C in rel.items():
-                tgt[i * self.P + j] = torch.as_tensor(C).detach().to(dev).float()[:, :3, :].reshape(T, 12)
+        self.inv_num = _f32(torch.cat(inv_num), dev)
+        # rel_transform targets: pairs (i, j) inside each group, one [Q*Q] block per group
+        if data.get('rel_transform_cam'):
+            tgt = torch.zeros(G_ * Q_ * Q_, T, 12, device=dev)
+            for g, dd in enumerate(self.datas):
+                for (i, j), C in dd['rel_transform_cam'].items():
+                    tgt[(g * Q_ + i) * Q_ + j] = torch.as_tensor(C).detach().to(dev).float()[:, :3, :].reshape(T, 12)
             self.rel_target = tgt.contiguous()
         else:
             self.rel_target = None
@@ -206,6 +233,7 @@ class StageCompiler:
 
     def compile(self, theta, opt_variables, loss_cfg, stage, n_begin=0, n_end=None, owner=True):
         data, lay, fl, dev, P, T, J = self.data, self.layout, self.flags, self.device, self.P, self.T, self.J
+        G, Q, persons_all = self.G, self.Q, self.persons
         n_end = P * T if n_end is None else n_end
         if 'person2cam_res_trans_reg' in loss_cfg:           # loss_func.py:244-245
             raise ValueError("residual 'person2cam_res_trans_reg' reads data['person2cam_res_trans'], a key the reference never creates "
@@ -215,6 +243,7 @@ class StageCompiler:
                 raise NotImplementedError(f"residual '{name}' has no CUDA implementation (no CPU fallback)")
         pb = L.Problem()
         pb.P, pb.T, pb.J, pb.n_params = P, T, J, lay.n_params
+        pb.G, pb.group_params = G, lay.group_params
         pb.n_begin, pb.n_end, pb.owner = n_begin, n_end, int(owner)
         keep = []
         # ---- camera mode (global_recon_model.py:473-508)
@@ -231,18 +260,18 @@ class StageCompiler:
             pb.off_cam_rot, pb.off_cam_trans = lay.cam_rot, lay.cam_trans
         else:
             pb.off_cam_rot, pb.off_cam_trans = lay.cam_inv_rot_res, lay.cam_inv_trans_res
-        cam_const = _f32(data['cam_pose'], dev)[:, :3, :].reshape(T, 12).contiguous().clone()
+        cam_const = torch.cat([_f32(dd['cam_pose'], dev)[:, :3, :].reshape(T, 12) for dd in self.datas]).contiguous().clone()
         keep.append(cam_const)
         pb.cam_pose_const = cam_const.data_ptr()
         pb.trans_res_all = int(fl['flag_cam_inv_trans_res_all'])
         # ---- trajectory source; the world variables enter the forward only with flag_opt_traj (:451-468)
         pb.traj_source = self.traj_source
         pb.use_world_res = int(self.opt_traj and 'world_res' in opt_variables)
-        pb.has_world_dheading = int(self.opt_traj and any('world_dheading' in data['person_data'][pid] for pid in self.pids))
+        pb.has_world_dheading = int(self.opt_traj and any('world_dheading' in d for d in persons_all))
         pb.heading_vec = int(self.heading_vec)
         # world_dxy, once created, is added in place to root_trans_world (:467-468); that tensor IS the base unless world_res
         # alone composes the pose, and then the add lands in the base too
-        has_dxy = self.opt_traj and any('world_dxy' in data['person_data'][pid] for pid in self.pids)
+        has_dxy = self.opt_traj and any('world_dxy' in d for d in persons_all)
         alias = has_dxy and (pb.has_world_dheading or not pb.use_world_res)
         if alias and self.traj_source == L.TRAJ_BASE:
             raise ValueError("world_dxy with a trajectory that does not come from the predictor needs world_res in opt_variables and "
@@ -280,19 +309,22 @@ class StageCompiler:
         pb.scale_all = None if self.scale_all is None else self.scale_all.data_ptr()
         # ---- persons
         persons = (L.Person * P)()
-        norms = {}
+        group_norms = [{} for _ in range(G)]                 # normalisers of each group's persons: the groups must agree
         host_w = torch.zeros(P, 2 * T * J + 2 * T, dtype=torch.float32)        # [kp_w | kp_dist_mask | ctr_w | ctt_w] per person
         for p in range(P):
             kp_w, kp_dm, ctr_w, ctt_w, nrm = self._person_weights(p, loss_cfg)
             host_w[p] = torch.cat([kp_w.reshape(-1), kp_dm.reshape(-1), ctr_w, ctt_w]).float()
             for k, v in nrm.items():
-                norms[k] = norms.get(k, 0) + v
+                group_norms[p // Q][k] = group_norms[p // Q].get(k, 0) + v
+        if any(n != group_norms[0] for n in group_norms[1:]):
+            raise ValueError('seed groups need the same loss normalisers (visibility and keypoint scores of one sequence)')
+        norms = group_norms[0]
         dev_w = host_w.to(dev)                                                   # one upload for all persons
         keep.append(dev_w)
-        for p, pid in enumerate(self.pids):
-            d, c, o = data['person_data'][pid], self.const[p], lay.persons[p]
+        for p in range(P):
+            c, o = self.const[p], lay.persons[p]
             ps = persons[p]
-            ps.start, ps.len = c['start'], c['len']
+            ps.start, ps.len, ps.group = c['start'], c['len'], p // Q
             ps.off_xy, ps.off_heading, ps.off_dxy, ps.off_dheading = o['xy'], o['heading'], o['dxy'], o['dheading']
             ps.off_z, ps.off_rot, ps.off_world_dheading = o['z'], o['rot'], o['world_dheading']
             ps.off_orient_res, ps.off_trans_res, ps.off_world_dxy = o['orient_res'], o['trans_res'], o['world_dxy']
@@ -310,22 +342,22 @@ class StageCompiler:
         if self.rel_target is not None and 'rel_transform' in loss_cfg:
             sp = loss_cfg['rel_transform']
             ffw = sp.get('first_frame_weight', 10)
-            rw, rwt = torch.zeros(P * P, T), torch.zeros(P * P, T)
-            n_rel = 0
-            for (i, j) in data['rel_transform_cam'].keys():
-                n_rel += T
-                both = self.host_vis[i] & self.host_vis[j]
-                if both.sum() == 0:
-                    continue
-                f0 = int(torch.where(both)[0][0])
-                wv = both.float()
-                wv[f0] = float(ffw) ** 2
-                rw[i * P + j] = wv
-                wt = wv.clone()
-                if sp.get('first_frame_trans_only', False):
-                    wt[:] = 0
-                    wt[f0] = float(ffw) ** 2
-                rwt[i * P + j] = wt
+            rw, rwt = torch.zeros(G * Q * Q, T), torch.zeros(G * Q * Q, T)
+            n_rel = T * len(data['rel_transform_cam'])
+            for g, dd in enumerate(self.datas):
+                for (i, j) in dd['rel_transform_cam'].keys():
+                    both = self.host_vis[g * Q + i] & self.host_vis[g * Q + j]
+                    if both.sum() == 0:
+                        continue
+                    f0 = int(torch.where(both)[0][0])
+                    wv = both.float()
+                    wv[f0] = float(ffw) ** 2
+                    rw[(g * Q + i) * Q + j] = wv
+                    wt = wv.clone()
+                    if sp.get('first_frame_trans_only', False):
+                        wt[:] = 0
+                        wt[f0] = float(ffw) ** 2
+                    rwt[(g * Q + i) * Q + j] = wt
             rw, rwt = rw.to(dev).contiguous(), rwt.to(dev).contiguous()
             keep += [rw, rwt]
             pb.rel_target, pb.rel_w, pb.rel_wt = self.rel_target.data_ptr(), rw.data_ptr(), rwt.data_ptr()
@@ -334,12 +366,12 @@ class StageCompiler:
         elif 'rel_transform' in loss_cfg:
             norms['rel_transform'] = 0
         # ---- scalar term tables
-        lens = lay.lens
+        lens = lay.lens[:Q]                                  # one group's persons
         norms.update({
-            'traj_rot_smoothness': P * (T - 1), 'traj_trans_smoothness': P * (T - 1),
+            'traj_rot_smoothness': Q * (T - 1), 'traj_trans_smoothness': Q * (T - 1),
             'local_traj_dxy_reg': sum(n - 1 for n in lens), 'local_traj_dheading_reg': sum(n - 1 for n in lens),
             'local_traj_dheading_reg_new': sum(n - 1 for n in lens), 'local_traj_rot_reg': sum(lens), 'local_traj_z_reg': sum(lens),
-            'traj_rot_res': P * T, 'traj_trans_res': P * T, 'cam_inv_trans_residual_reg': lay.trans_res_rows,
+            'traj_rot_res': Q * T, 'traj_trans_res': Q * T, 'cam_inv_trans_residual_reg': lay.trans_res_rows,
             'cam_inv_rot_smoothness': T - 1, 'cam_origin_smoothness': T - 1, 'cam_rot_smoothness': T - 1, 'cam_trans_smoothness': T - 1,
             'cam_depth_smoothness': 1,          # loss_func.py:102 sums over the T-1 frame pairs (the .mean() sees a 0-d tensor)
         })
@@ -366,19 +398,20 @@ class StageCompiler:
 
         def on(o, n):
             active[o:o + n] = 1
-        if 'cam' not in opt_variables:
-            on(lay.cam_inv_rot_res, 6 * lay.n_empty)
-            on(lay.cam_inv_trans_res, 3 * lay.trans_res_rows)
-        elif fl['flag_fixed_cam']:
-            on(lay.cam_rot_fix, 6)
-            on(lay.cam_trans_fix, 3)
-        else:
-            on(lay.cam_rot, 6 * T)
-            on(lay.cam_trans, 3 * T)
+        for g0 in range(0, lay.n_params, lay.group_params):        # each group's camera variables
+            if 'cam' not in opt_variables:
+                on(g0 + lay.cam_inv_rot_res, 6 * lay.n_empty)
+                on(g0 + lay.cam_inv_trans_res, 3 * lay.trans_res_rows)
+            elif fl['flag_fixed_cam']:
+                on(g0 + lay.cam_rot_fix, 6)
+                on(g0 + lay.cam_trans_fix, 3)
+            else:
+                on(g0 + lay.cam_rot, 6 * T)
+                on(g0 + lay.cam_trans, 3 * T)
         hd = lay.heading_dim
         sizes = lambda Ln: {'xy': 2, 'heading': hd, 'dxy': 2 * (Ln - 1), 'dheading': hd * (Ln - 1), 'z': Ln, 'rot': 6 * Ln}
         for p in range(P):
-            o, sz = lay.persons[p], sizes(lens[p])
+            o, sz = lay.persons[p], sizes(lay.lens[p])
             for key in opt_variables:
                 if key == 'world_res' and self.opt_traj:
                     on(o['orient_res'], 3 * T)
@@ -407,6 +440,20 @@ class StageCompiler:
 
 # ---------------------------------------------------------------------------------------------------- variables
 def make_layout(data, flags):
+    """layout of one data dict, or of the seed groups in a list of data dicts (which must agree on every block)"""
+    datas = _groups(data)
+    lays = [_one_group_layout(d, flags) for d in datas]
+    key = lambda l: (l.T, l.n_empty, l.trans_res_rows, l.lens, l.heading_dim, l.world_dxy, l.person2cam)
+    if any(key(l) != key(lays[0]) for l in lays[1:]):
+        raise ValueError('seed groups need the same variable layout (persons, exist ranges, frames without persons, variables)')
+    if len(datas) == 1:
+        return lays[0]
+    l0 = lays[0]
+    return VariableLayout(l0.T, l0.n_empty, l0.trans_res_rows, l0.lens, heading_dim=l0.heading_dim, world_dxy=l0.world_dxy,
+                          person2cam=l0.person2cam, groups=len(datas))
+
+
+def _one_group_layout(data, flags):
     persons = data['person_data']
     T = data['seq_len']
     n_empty = int((torch.as_tensor(data['fr_num_persons']) == 0).sum())
@@ -424,48 +471,49 @@ def make_layout(data, flags):
 
 def bind_variables(data, layout, theta):
     """Move every optimisation variable that already exists in `data` into the packed vector `theta` and replace the
-    dict entry by the view, so later reads (and the final tensor_to_numpy) see what the kernels update."""
-    gv = layout.views(theta)
-    for name in ['cam_inv_rot_residual', 'cam_inv_trans_residual']:
-        gv[name].copy_(torch.as_tensor(data[name]).to(theta))
-        data[name] = gv[name]
-    for p, d in enumerate(data['person_data'].values()):
-        pv = layout.views(theta, p)
-        for name in ['traj_local_xy', 'traj_local_heading', 'traj_local_dxy', 'traj_local_dheading', 'traj_local_z',
-                     'traj_local_rot', 'smpl_orient_world_res', 'root_trans_world_res', 'world_dheading', 'world_dxy',
-                     'person2cam_res_rot', 'person2cam_res_trans']:
-            # world_dheading exists once a stage has requested it (global_recon_model.py:624-627); with continue_opt it
-            # arrives already optimised and forward() keeps composing with it (:459-465)
-            if name in d:
-                pv[name].copy_(torch.as_tensor(d[name]).to(theta))
-                d[name] = pv[name]
+    dict entry by the view, so later reads (and the final tensor_to_numpy) see what the kernels update.  `data`: one dict or
+    the seed groups' list."""
+    for g, dd in enumerate(_groups(data)):
+        gv = layout.views(theta, group=g)
+        for name in ['cam_inv_rot_residual', 'cam_inv_trans_residual']:
+            gv[name].copy_(torch.as_tensor(dd[name]).to(theta))
+            dd[name] = gv[name]
+        for q, d in enumerate(dd['person_data'].values()):
+            pv = layout.views(theta, g * layout.Q + q)
+            for name in ['traj_local_xy', 'traj_local_heading', 'traj_local_dxy', 'traj_local_dheading', 'traj_local_z',
+                         'traj_local_rot', 'smpl_orient_world_res', 'root_trans_world_res', 'world_dheading', 'world_dxy',
+                         'person2cam_res_rot', 'person2cam_res_trans']:
+                # world_dheading exists once a stage has requested it (global_recon_model.py:624-627); with continue_opt it
+                # arrives already optimised and forward() keeps composing with it (:459-465)
+                if name in d:
+                    pv[name].copy_(torch.as_tensor(d[name]).to(theta))
+                    d[name] = pv[name]
 
 
 def begin_stage_variables(data, layout, theta, flags, opt_variables):
     """Side effects of GlobalReconOptimizer.get_parameter (global_recon_model.py:596-631): camera variables are
-    re-initialised from the current cam_pose, world_dheading / world_dxy are created (zeros) the first time they are requested."""
-    gv = layout.views(theta)
-    if 'cam' in opt_variables:
-        cam = torch.as_tensor(data['cam_pose']).to(theta)
-        d6 = torch.cat([cam[:, :3, 0], cam[:, :3, 1]], dim=-1)           # rotmat_to_rot6d: first two columns
-        if flags['flag_fixed_cam']:
-            gv['cam_rot_6d_fix'].copy_(d6[:1])
-            gv['cam_trans_fix'].copy_(cam[:1, :3, 3])
-            data['cam_rot_6d_fix'], data['cam_trans_fix'] = gv['cam_rot_6d_fix'], gv['cam_trans_fix']
-            data['cam_rot_6d'] = gv['cam_rot_6d_fix'].expand(layout.T, -1)
-            data['cam_trans'] = gv['cam_trans_fix'].expand(layout.T, -1)
-        else:
-            gv['cam_rot_6d'].copy_(d6)
-            gv['cam_trans'].copy_(cam[:, :3, 3])
-            data['cam_rot_6d'], data['cam_trans'] = gv['cam_rot_6d'], gv['cam_trans']
-    if 'world_dheading' in opt_variables:
-        for p, d in enumerate(data['person_data'].values()):
-            if 'world_dheading' not in d:
-                d['world_dheading'] = layout.views(theta, p)['world_dheading']
-    if 'world_dxy' in opt_variables:
-        if not layout.world_dxy:
-            raise ValueError("opt_variables lists 'world_dxy' but the variable layout has no world_dxy block "
-                             "(make_layout(..., flags={'world_dxy': True, ...}))")
-        for p, d in enumerate(data['person_data'].values()):
-            if 'world_dxy' not in d:
-                d['world_dxy'] = layout.views(theta, p)['world_dxy']
+    re-initialised from the current cam_pose, world_dheading / world_dxy are created (zeros) the first time they are requested.
+    `data`: one dict or the seed groups' list."""
+    if 'world_dxy' in opt_variables and not layout.world_dxy:
+        raise ValueError("opt_variables lists 'world_dxy' but the variable layout has no world_dxy block "
+                         "(make_layout(..., flags={'world_dxy': True, ...}))")
+    for g, data in enumerate(_groups(data)):
+        gv = layout.views(theta, group=g)
+        if 'cam' in opt_variables:
+            cam = torch.as_tensor(data['cam_pose']).to(theta)
+            d6 = torch.cat([cam[:, :3, 0], cam[:, :3, 1]], dim=-1)           # rotmat_to_rot6d: first two columns
+            if flags['flag_fixed_cam']:
+                gv['cam_rot_6d_fix'].copy_(d6[:1])
+                gv['cam_trans_fix'].copy_(cam[:1, :3, 3])
+                data['cam_rot_6d_fix'], data['cam_trans_fix'] = gv['cam_rot_6d_fix'], gv['cam_trans_fix']
+                data['cam_rot_6d'] = gv['cam_rot_6d_fix'].expand(layout.T, -1)
+                data['cam_trans'] = gv['cam_trans_fix'].expand(layout.T, -1)
+            else:
+                gv['cam_rot_6d'].copy_(d6)
+                gv['cam_trans'].copy_(cam[:, :3, 3])
+                data['cam_rot_6d'], data['cam_trans'] = gv['cam_rot_6d'], gv['cam_trans']
+        for q, d in enumerate(data['person_data'].values()):
+            if 'world_dheading' in opt_variables and 'world_dheading' not in d:
+                d['world_dheading'] = layout.views(theta, g * layout.Q + q)['world_dheading']
+            if 'world_dxy' in opt_variables and 'world_dxy' not in d:
+                d['world_dxy'] = layout.views(theta, g * layout.Q + q)['world_dxy']

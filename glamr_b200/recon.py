@@ -3,10 +3,13 @@
 
 Same constructor, ``optimize(in_dict, continue_opt=False) -> dict`` (numpy), ``init_data``, ``forward``,
 ``compute_loss``, ``optimize_main``; same YAML stage specs; same output keys / shapes / dtypes (SURVEY.md Appendix B).
+``optimize_seeds(in_dict, seeds) -> [dict]`` runs several seeds of one sequence as one problem (seed groups, see
+glamr_b200/problem.py): every seed's result is the one ``optimize`` gives for that seed.
 Host Python does what the reference does on the host (dict bookkeeping, SciPy rotation-vector conversion and linear
 gap interpolation, log lines); every formula of the per-iteration path -- trajectory codec, camera, SMPL, projection,
 residuals, analytic backward, Adam -- is a kernel of glamr_b200/csrc.  No autograd, no CPU fallback.
 """
+import copy
 import ctypes
 import time
 
@@ -555,16 +558,19 @@ class GlobalReconOptimizer:
     # ------------------------------------------------------------------------------------------------ device state
     def _attach(self, data):
         """Pack the optimisation variables into theta and build the constant tables.  The CUDA handle (scratch arena,
-        Adam moments, captured iteration graph) is kept across calls while (P, T, J, n_params) stay the same."""
+        Adam moments, captured iteration graph) is kept across calls while (P, T, J, n_params) stay the same.  `data`: one
+        data dict, or the list of the seed groups' data dicts (optimize_seeds)."""
         self._fresh_attach = True
         self._data = data
+        self._n_groups = len(data) if isinstance(data, list) else 1
         self._layout = PB.make_layout(data, self._flags)
         self._theta = torch.zeros(self._layout.n_params, device=self.device)
         PB.bind_variables(data, self._layout, self._theta)
         self._comp = PB.StageCompiler(data, self._layout, self._flags, self.device, G.angle_axis_to_rot6d, num_joints=self.smpl.num_joints,
                                       aa_to_quat=G.angle_axis_to_quaternion)
-        self._reduce = torch.zeros(self._layout.n_params + NUM_TERMS, device=self.device)
-        self._terms = torch.zeros(NUM_TERMS + 1, device=self.device)
+        # [grad | term sums of every group], and the loss terms of every group
+        self._reduce = torch.zeros(self._layout.n_params + self._n_groups * NUM_TERMS, device=self.device)
+        self._terms = torch.zeros(self._n_groups * (NUM_TERMS + 1), device=self.device)
         self._stage_key = None
         # multi-GPU: contiguous shards of the frame-persons n = p*T + t (SMPL + per-frame residuals are independent per
         # frame-person, so a person may straddle two ranks; P persons on P GPUs gives one person each)
@@ -683,8 +689,8 @@ class GlobalReconOptimizer:
         return _device_view(p.value, n.value, self.device).view(*shape).clone()
 
     def _scatter_outputs(self, data):
-        """copy what forward() stores into the data dict in the reference (:421-528)"""
-        P, T, J = self._comp.P, self._comp.T, self._comp.J
+        """copy what forward() stores into the data dict (each seed group's, for a list) in the reference (:421-528)"""
+        P, T, J, Q = self._comp.P, self._comp.T, self._comp.J, self._comp.Q
         ow, tw = self._read(L.R_ORIENT_WORLD, P, T, 3), self._read(L.R_TRANS_WORLD, P, T, 3)
         ob, tb = self._read(L.R_ORIENT_BASE, P, T, 3), self._read(L.R_TRANS_BASE, P, T, 3)
         kp = self._read(L.R_KP_PRED, P, T, J, 2)
@@ -705,17 +711,22 @@ class GlobalReconOptimizer:
                 outs.append(packed[:, o:o + w].reshape(x.shape))
                 o += w
             kp, ociw, tciw, jw = outs
-        data['cam_pose'] = G.from34(self._read(L.R_CAM_POSE, T, 12))
-        data['cam_pose_inv'] = G.from34(self._read(L.R_CAM_POSE_INV, T, 12))
-        for p, d in enumerate(data['person_data'].values()):
-            d['smpl_orient_world'], d['root_trans_world'] = ow[p], tw[p]
-            d['smpl_orient_world_base'], d['root_trans_world_base'] = ob[p], tb[p]
-            d['kp_2d_pred'] = kp[p]
-            d['smpl_orient_cam_in_world'], d['root_trans_cam_in_world'] = ociw[p], tciw[p]
-            if self.traj_source == L.TRAJ_PREDICTED:           # without the codec the reference has no traj_local
-                d['traj_local'] = tl[p][d['exist_frames']]
-            d['joints_world'] = jw[p]
-            d['person_transform_world'] = G.make_transform(ow[p], tw[p], 'axis_angle')
+        datas = data if isinstance(data, list) else [data]
+        ng = len(datas)
+        cam, cam_inv = self._read(L.R_CAM_POSE, ng, T, 12), self._read(L.R_CAM_POSE_INV, ng, T, 12)
+        for g, dg in enumerate(datas):
+            dg['cam_pose'] = G.from34(cam[g] if ng > 1 else cam.view(T, 12))
+            dg['cam_pose_inv'] = G.from34(cam_inv[g] if ng > 1 else cam_inv.view(T, 12))
+            for q, d in enumerate(dg['person_data'].values()):
+                p = g * Q + q
+                d['smpl_orient_world'], d['root_trans_world'] = ow[p], tw[p]
+                d['smpl_orient_world_base'], d['root_trans_world_base'] = ob[p], tb[p]
+                d['kp_2d_pred'] = kp[p]
+                d['smpl_orient_cam_in_world'], d['root_trans_cam_in_world'] = ociw[p], tciw[p]
+                if self.traj_source == L.TRAJ_PREDICTED:           # without the codec the reference has no traj_local
+                    d['traj_local'] = tl[p][d['exist_frames']]
+                d['joints_world'] = jw[p]
+                d['person_transform_world'] = G.make_transform(ow[p], tw[p], 'axis_angle')
 
     # ------------------------------------------------------------------------------------------------ reference API
     def forward(self, data, opt_variables, opt_meta):
@@ -738,18 +749,25 @@ class GlobalReconOptimizer:
         return terms[NUM_TERMS], wt, uw
 
     def optimize_main(self, data, opt_variables, opt_lr, opt_niters, loss_cfg, opt_meta):
-        """:547-570 -- opt_niters fused iterations (forward + residuals + backward [+ allreduce] + Adam)."""
+        """:547-570 -- opt_niters fused iterations (forward + residuals + backward [+ allreduce] + Adam).  `data` may be the
+        list of the seed groups' data dicts attached by optimize_seeds."""
         stage = opt_meta['stage']
         self._cur_vars, self._cur_stage, self._loss_cfg = opt_variables, stage, loss_cfg
         lib = self._lib
+        datas = data if isinstance(data, list) else [data]
+        ng = len(datas)
+        seq_names = [d['seq_name'] for d in datas]
+        if ng > 1:
+            seq_names = [f'{n} (seed group {g})' for g, n in enumerate(seq_names)]
+        stride = ng * (NUM_TERMS + 1)                            # one row of loss terms per group and iteration
         with torch.cuda.device(self.device):
             self._set_stage(data, opt_variables, loss_cfg, stage, reset_adam=True, begin=True)
-            hist = torch.zeros((max(opt_niters, 1), NUM_TERMS + 1), device=self.device)
+            hist = torch.zeros((max(opt_niters, 1), stride), device=self.device)
             stream = torch.cuda.current_stream()
 
             def one_iteration():
                 self._backward(for_apply=True)
-                L.check(lib.glamr_opt_apply(self._opt, L.ptr(self._theta), L.ptr(self._reduce), float(opt_lr), L.ptr(hist), NUM_TERMS + 1,
+                L.check(lib.glamr_opt_apply(self._opt, L.ptr(self._theta), L.ptr(self._reduce), float(opt_lr), L.ptr(hist), stride,
                                             L.stream_ptr()), 'glamr_opt_apply')
             graph = None
             done = 0
@@ -759,7 +777,7 @@ class GlobalReconOptimizer:
             # fused into the Adam kernel over peer memory
             native = self.world == 1 or getattr(self, '_peer_ok', False)
             if native and opt_niters > 0:
-                L.check(lib.glamr_opt_iterate(self._opt, L.ptr(self._theta), L.ptr(self._reduce), float(opt_lr), L.ptr(hist), NUM_TERMS + 1,
+                L.check(lib.glamr_opt_iterate(self._opt, L.ptr(self._theta), L.ptr(self._reduce), float(opt_lr), L.ptr(hist), stride,
                                               1, int(self.use_cuda_graph), L.stream_ptr()), 'glamr_opt_iterate')
                 done = 1
             elif opt_niters > 0:
@@ -784,7 +802,7 @@ class GlobalReconOptimizer:
             while done < opt_niters:
                 todo = min(chunk, opt_niters - done)
                 if native:
-                    L.check(lib.glamr_opt_iterate(self._opt, L.ptr(self._theta), L.ptr(self._reduce), float(opt_lr), L.ptr(hist), NUM_TERMS + 1,
+                    L.check(lib.glamr_opt_iterate(self._opt, L.ptr(self._theta), L.ptr(self._reduce), float(opt_lr), L.ptr(hist), stride,
                                                   todo, int(self.use_cuda_graph), L.stream_ptr()), 'glamr_opt_iterate')
                 else:
                     for _ in range(todo):
@@ -794,18 +812,26 @@ class GlobalReconOptimizer:
                             one_iteration()
                 done += todo
                 if logging_on:
-                    logged = self._write_logs(hist, logged, done, opt_niters, opt_lr, loss_cfg, stage, data['seq_name'], t_stage)
+                    logged = self._write_group_logs(hist, ng, logged, done, opt_niters, opt_lr, loss_cfg, stage, seq_names, t_stage)
             ev1.record()
             ev1.synchronize()
             if opt_niters > 1:
                 self.iter_ms.append((stage, opt_niters - 1, ev0.elapsed_time(ev1) / (opt_niters - 1)))
             if self.log is not None or self.specs.get('print_logs', False):
-                self._write_logs(hist, logged, done, opt_niters, opt_lr, loss_cfg, stage, data['seq_name'], t_stage)
-            self.loss_history = hist
+                self._write_group_logs(hist, ng, logged, done, opt_niters, opt_lr, loss_cfg, stage, seq_names, t_stage)
+            # [iterations, terms + total]; seed groups: [iterations, groups, terms + total]
+            self.loss_history = hist if ng == 1 else hist.view(hist.shape[0], ng, NUM_TERMS + 1)
             self.cur_iter = max(opt_niters - 1, 0)
             if opt_niters > 0:
                 self._scatter_outputs(data)                      # state of the last closure, like the reference
         return data
+
+    def _write_group_logs(self, hist, ng, start, end, opt_niters, opt_lr, loss_cfg, stage, seq_names, t_stage):
+        """_write_logs for each seed group's columns of the loss history"""
+        for g in range(ng):
+            rows = hist if ng == 1 else hist.view(hist.shape[0], ng, NUM_TERMS + 1)[:, g]
+            self._write_logs(rows, start, end, opt_niters, opt_lr, loss_cfg, stage, seq_names[g], t_stage)
+        return end
 
     def _write_logs(self, hist, start, end, opt_niters, opt_lr, loss_cfg, stage, seq_name, t_stage):
         """:646-659 same line format; values are read back in blocks of `log_interval` iterations."""
@@ -844,6 +870,42 @@ class GlobalReconOptimizer:
         # host wall-clock of the three phases of the last call (init_data includes the learned prior; stages include the waits)
         self.phase_seconds = {'init_data': t1 - t0, 'stages': t2 - t1, 'to_numpy': time.perf_counter() - t2}
         return out
+
+    def optimize_seeds(self, in_dict, seeds):
+        """Optimise several seeds of one sequence as one problem.  Element k of the result is what
+        ``np.random.seed(s); torch.manual_seed(s); optimize(copy.deepcopy(in_dict))`` returns for s = seeds[k], bit for bit:
+        every seed's init_data (and the learned prior in it) runs as in the serial path after setting the RNGs the same way, then
+        the S data dicts are attached as S seed groups of one problem (glamr_b200/problem.py) and the stages run once for all of
+        them.  Each group's camera, terms and gradient are reduced exactly as in its own one-group problem.
+        ``self.seed_loss_histories[k]`` is seed k's loss history of the last stage (``loss_history`` of its serial run).
+        No continue_opt; one GPU only (run_dataset shards sequences over ranks, each rank batches its own seeds)."""
+        if self.world > 1:
+            raise ValueError('optimize_seeds runs on one GPU: shard sequences over ranks and batch the seeds on each rank')
+        seeds = [int(s) for s in seeds]
+        if not seeds:
+            return []
+        t0 = time.perf_counter()
+        datas = []
+        for s in seeds:                                # run_dataset's RNG setting, then the serial path's init
+            np.random.seed(s)
+            torch.manual_seed(s)
+            datas.append(self.init_data(copy.deepcopy(in_dict)))
+        t1 = time.perf_counter()
+        self._attach(datas)
+        for stage, stage_specs in self.opt_stage_specs.items():
+            opt_meta = {'stage': stage, 'opt_latent_start_iter': stage_specs.get('opt_latent_start_iter', 0)}
+            self.optimize_main(datas, stage_specs['opt_variables'], stage_specs['opt_lr'], stage_specs['opt_niters'],
+                               stage_specs['loss_cfg'], opt_meta)
+            if stage_specs.get('reinitialize_cam', False):
+                for data in datas:
+                    data['cam_pose'][:] = data['cam_pose'][[0]]
+                    data['cam_pose_inv'] = G.inverse_transform(data['cam_pose'])
+        t2 = time.perf_counter()
+        lh = self.loss_history
+        self.seed_loss_histories = [lh] if len(seeds) == 1 else [lh[:, g] for g in range(len(seeds))]
+        outs = [tensor_to_numpy(data) for data in datas]
+        self.phase_seconds = {'init_data': t1 - t0, 'stages': t2 - t1, 'to_numpy': time.perf_counter() - t2}
+        return outs
 
 
 def _device_view(addr, count, device):

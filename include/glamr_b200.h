@@ -170,6 +170,7 @@ enum glamr_traj_source {
 
 typedef struct glamr_person {
   int32_t start, len;              /* exist range [start, start+len) of this person (exist_frames)              */
+  int32_t group;                   /* seed group of this person (see glamr_problem_t.G): p / (P/G) for person p  */
   int32_t off_xy, off_heading, off_dxy, off_dheading, off_z, off_rot;     /* offsets into theta (floats)        */
   int32_t off_world_dheading, off_orient_res, off_trans_res;              /* [T], [T,3], [T,3]                  */
   int32_t off_world_dxy;           /* [T,2] world_dxy (read only with has_world_dxy)                              */
@@ -200,8 +201,15 @@ typedef struct glamr_person {
   float* world_dxy_base;
 } glamr_person_t;
 
+/* Seed groups: G independent copies of one sequence (same persons, frames, visibility and loss normalisers, each with its own
+ * initial state) optimised as one problem.  Group g owns persons [g*P/G, (g+1)*P/G) and theta [g*group_params, (g+1)*group_params):
+ * its camera variables sit at off_cam_rot / off_cam_trans + g*group_params.  Every per-frame table below has one [T,...] block per
+ * group, the rel_transform tables one [(P/G)^2,T,...] block per group (pairs only inside a group), the term sums and loss terms
+ * one row per group.  Each group's camera, camera terms and term sums are reduced over the same elements in the same order as
+ * the one-group problem of that group alone, so every group's results are those of its own one-group run bit for bit.  G > 1
+ * needs the whole frame-person range on one rank (n_begin 0, n_end P*T, owner).  G 0 (zero-initialised) = 1. */
 typedef struct glamr_problem {
-  int32_t P, T, J;                 /* persons, frames, joints per person (n_map of the SMPL handle)              */
+  int32_t P, T, J;                 /* persons (all groups), frames, joints per person (n_map of the SMPL handle)  */
   int32_t cam_mode;                /* enum glamr_cam_mode                                                         */
   int32_t off_cam_rot, off_cam_trans; /* variable offsets (modes 1,2: cam_rot_6d / cam_trans; mode 3: residuals)  */
   int32_t use_world_res, has_world_dheading;
@@ -220,6 +228,8 @@ typedef struct glamr_problem {
   int32_t world_dxy_alias;         /* that add also lands in the base (see glamr_person_t.world_dxy_base)          */
   int32_t has_person2cam;          /* flag_opt_person2cam_rot / _trans (:484-488): mode 3 composes each person's person2cam with
                                     * [rot6d(person2cam_res_rot) | person2cam_res_trans] before the mean; 0 = person2cam as is */
+  int32_t G;                       /* seed groups (see above); P % G == 0                                          */
+  int32_t group_params;            /* floats of theta per group (n_params = G * group_params; unused with one group) */
   float cam_up_first_weight;
   float rel_trans_weight;
   float term_weight[GLAMR_NUM_TERMS];   /* YAML weight, 0 if the term is absent                                  */
@@ -230,13 +240,13 @@ typedef struct glamr_problem {
   const float* smpl_pose_all;      /* [P,T,69] body pose (infilled), constant during optimisation                 */
   const float* smpl_beta_all;      /* [P,T,10]                                                                    */
   const float* scale_all;          /* [P,T] or NULL                                                               */
-  const float* cam_pose_const;     /* [T,12] world->cam 3x4 (mode 0)                                              */
-  const int32_t* empty_index;      /* [T] row of cam_inv_rot_residual for frames without any person, else -1     */
-  const int32_t* fill_src;         /* [T] forward-fill source frame (mode 3)                                      */
-  const float* inv_num_persons;    /* [T] 1/num visible persons (0 where none)                                    */
-  const float* rel_target;         /* [P*P,T,12] rel_transform_cam (i*P+j), or NULL                               */
-  const float* rel_w;              /* [P*P,T] squared frame weights for the rotation part (0 = frame unused)      */
-  const float* rel_wt;             /* [P*P,T] same for the translation part                                       */
+  const float* cam_pose_const;     /* [G,T,12] world->cam 3x4 (mode 0)                                            */
+  const int32_t* empty_index;      /* [G,T] row of cam_inv_rot_residual for frames without any person, else -1   */
+  const int32_t* fill_src;         /* [G,T] forward-fill source frame (mode 3), a frame of the same group         */
+  const float* inv_num_persons;    /* [G,T] 1/num visible persons of the group (0 where none)                     */
+  const float* rel_target;         /* [G,Q*Q,T,12] rel_transform_cam (i*Q+j, Q = P/G persons per group), or NULL  */
+  const float* rel_w;              /* [G,Q*Q,T] squared frame weights for the rotation part (0 = frame unused)    */
+  const float* rel_wt;             /* [G,Q*Q,T] same for the translation part                                     */
   const uint8_t* active;           /* [n_params] 1 where Adam updates theta                                       */
 } glamr_problem_t;
 
@@ -254,7 +264,7 @@ int glamr_opt_destroy(glamr_opt_t* st);
  * (global_recon_model.py:548,:642); bit 1 also zeroes all scratch (handle re-used for a new sequence).  A changed
  * frame-person range [n_begin, n_end) re-primes the pipelined blend: the next evaluation recomputes v_posed for it. */
 int glamr_opt_set_problem(glamr_opt_t* st, const glamr_problem_t* problem, int reset_adam, void* stream);
-/* length (floats) of the caller-owned reduce buffer: [grad (n_params) | un-normalised term sums (GLAMR_NUM_TERMS)] */
+/* length (floats) of the caller-owned reduce buffer: [grad (n_params) | un-normalised term sums (G x GLAMR_NUM_TERMS)] */
 size_t glamr_opt_reduce_count(const glamr_opt_t* st);
 /* kernels per optimiser iteration (glamr_opt_backward + glamr_opt_apply) for the current problem (bench.py: gpu_launches) */
 int glamr_opt_launch_count(const glamr_opt_t* st);
@@ -263,7 +273,7 @@ int glamr_opt_launch_count(const glamr_opt_t* st);
  * [grad | term sums] of THIS rank's share in reduce_buf.  With several GPUs the caller sums reduce_buf over ranks
  * (one NCCL allreduce) before glamr_opt_apply.  (closure of global_recon_model.py:551-557) */
 int glamr_opt_backward(glamr_opt_t* st, const float* theta, float* reduce_buf, void* stream);
-/* loss_terms [GLAMR_NUM_TERMS+1] (device): un-weighted term values (sum / normaliser) then the weighted total.
+/* loss_terms [G][GLAMR_NUM_TERMS+1] (device): per group, un-weighted term values (sum / normaliser) then the weighted total.
  * Then one torch.optim.Adam step (betas 0.9/0.999, eps 1e-8) on the active entries of theta; the step count and
  * bias corrections live on the device so the call sequence can be captured in a CUDA graph.  With
  * loss_hist_stride > 0 the terms of optimiser step k (0-based, counted on the device since the last reset) are
@@ -308,8 +318,8 @@ enum glamr_read {
   GLAMR_R_KP_PRED = 4,         /* [P,T,J,2] kp_2d_pred                   */
   GLAMR_R_ORIENT_CAM_IN_WORLD = 5, /* [P,T,3]                            */
   GLAMR_R_TRANS_CAM_IN_WORLD = 6,  /* [P,T,3]                            */
-  GLAMR_R_CAM_POSE = 7,        /* [T,12]    world->cam 3x4               */
-  GLAMR_R_CAM_POSE_INV = 8,    /* [T,12]                                 */
+  GLAMR_R_CAM_POSE = 7,        /* [G,T,12]  world->cam 3x4               */
+  GLAMR_R_CAM_POSE_INV = 8,    /* [G,T,12]                               */
   GLAMR_R_JOINTS_WORLD = 9,    /* [P,T,J,3]                              */
   GLAMR_R_TRAJ_LOCAL = 10,     /* [P,T,11]  traj_local (rows of the exist range, others 0) */
   GLAMR_R_ADAM_M = 11,         /* [n_params] Adam first moment                                */

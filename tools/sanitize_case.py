@@ -1,5 +1,5 @@
 """Small end-to-end case for compute-sanitizer (memcheck / racecheck): SMPL forward at a ragged size through both LBS paths,
-one prior inference, and a short optimisation through the iteration kernels.
+one prior inference, a short optimisation through the iteration kernels, and two seed groups of one sequence (optimize_seeds).
 
     compute-sanitizer --tool memcheck  python tools/sanitize_case.py
     compute-sanitizer --tool racecheck python tools/sanitize_case.py
@@ -43,4 +43,12 @@ for cfg_id in which:
     out = m.optimize(copy.deepcopy(in_dict))
     torch.cuda.synchronize()
     print(cfg_id, 'ok', float(out['cam_pose'].sum()))
+# two seed groups (glamr_problem_t.G = 2): camera from the persons, gaps, 2 persons; each seed draws its own prior latents
+cfg = Config('glamr_3dpw')
+for st in cfg.opt_stage_specs.values():
+    st['opt_niters'] = 3
+m = GlobalReconOptimizer(cfg, dev, None, smpl=smpl, mt_model=prior)
+outs = m.optimize_seeds(make_in_dict(a, 2, 40, seed=1, gaps=True), [1, 2])
+torch.cuda.synchronize()
+print('seed groups ok', [float(o['cam_pose'].sum()) for o in outs])
 print('sanitize case done')
