@@ -23,9 +23,9 @@ struct OptScratch {
   float* trans_base;    // [N][3]
   float* orient_world;  // [N][3]
   float* trans_world;   // [N][3]
-  float* cam;           // [G*T][12] world->cam (3x4 row-major), one block of T rows per seed group
-  float* cam_inv;       // [G*T][12]
-  float* cam_d6;        // [G*T][6]  6d of cam_inv rotation incl. residual (mode 3)
+  float* cam;           // [sum T][12] world->cam (3x4 row-major), one block of T rows per group
+  float* cam_inv;       // [sum T][12]
+  float* cam_d6;        // [sum T][6]  6d of cam_inv rotation incl. residual (mode 3)
   float* joints_world;  // [N][J][3]
   float* kp_pred;       // [N][J][2]
   float* orient_ciw;    // [N][3]  smpl_orient_cam_in_world
@@ -33,7 +33,7 @@ struct OptScratch {
   float* g_orient;      // [N][3]  dL/d smpl_orient_world
   float* g_trans;       // [N][3]  dL/d root_trans_world
   float* g_cam;         // [N][12] per frame-person dL/d cam (R 9, t 3)
-  float* g_cam_fix;     // [G*T][12] per-frame dL/d (cam_rot_6d, cam_trans) [9 used] in fixed-camera mode; mode 3: dL/d(mean cam_inv)
+  float* g_cam_fix;     // [sum T][12] per-frame dL/d (cam_rot_6d, cam_trans) [9 used] in fixed-camera mode; mode 3: dL/d(mean cam_inv)
   float* g_xy;          // [N][2]  backward scan buffer
   float* g_head;        // [N]
   float* grad;          // [n_params]
@@ -53,17 +53,46 @@ struct TermAcc {
   }
 };
 
-// Seed groups (include/glamr_b200.h, glamr_problem_t.G): group g owns persons [g*Q, (g+1)*Q), Q = P/G, the camera rows
-// [g*T, (g+1)*T) of every per-frame table and scratch array, and theta [g*group_params, ...).  A camera frame is addressed by its
-// row gt = g*T + t; with one group gt = t.
+// Groups (include/glamr_b200.h, glamr_group_t): group g owns persons [p0, p0+Q), frame-persons [n0, n0 + Q*T), camera rows
+// [c0, c0+T) of every per-frame table and scratch array, and the block of theta at theta0.  A camera frame is addressed by its row
+// c0 + t.  With one group there is no table and every lookup is the one-group problem: person p's frame t is row p*T + t, camera
+// row t, theta from 0.
 GLAMR_HD int num_groups(const glamr_problem_t& pb) { return pb.G > 1 ? pb.G : 1; }
-GLAMR_HD int group_persons(const glamr_problem_t& pb) { return pb.P / num_groups(pb); }
-GLAMR_HD int group_theta(const glamr_problem_t& pb, int g) { return g > 0 ? g * pb.group_params : 0; }
-// group of person p (persons are stored group by group; glamr_person_t.group records the same).  Computed from the index, so the
-// camera address of a frame-person does not wait on a load of its person record
-GLAMR_HD int person_group(const glamr_problem_t& pb, int p) { return pb.G > 1 ? p / group_persons(pb) : 0; }
+GLAMR_HD bool has_group_table(const glamr_problem_t& pb) { return pb.G > 1; }
+GLAMR_HD int group_persons(const glamr_problem_t& pb, int g = 0) { return has_group_table(pb) ? pb.groups[g].Q : pb.P; }
+GLAMR_HD int group_theta(const glamr_problem_t& pb, int g) { return has_group_table(pb) ? pb.groups[g].theta0 : 0; }
+GLAMR_HD int group_frames(const glamr_problem_t& pb, int g) { return has_group_table(pb) ? pb.groups[g].T : pb.T; }
+GLAMR_HD int group_first_person(const glamr_problem_t& pb, int g) { return has_group_table(pb) ? pb.groups[g].p0 : 0; }
+GLAMR_HD size_t group_first_row(const glamr_problem_t& pb, int g) { return has_group_table(pb) ? (size_t)pb.groups[g].n0 : 0; }
+GLAMR_HD size_t group_cam_row0(const glamr_problem_t& pb, int g) { return has_group_table(pb) ? (size_t)pb.groups[g].c0 : 0; }
+GLAMR_HD int group_off_cam_rot(const glamr_problem_t& pb, int g) { return has_group_table(pb) ? pb.groups[g].off_cam_rot : pb.off_cam_rot; }
+GLAMR_HD int group_off_cam_trans(const glamr_problem_t& pb, int g) { return has_group_table(pb) ? pb.groups[g].off_cam_trans : pb.off_cam_trans; }
+// first (pair, frame) entry of group g's rel_transform block
+GLAMR_HD size_t group_rel0(const glamr_problem_t& pb, int g) { return has_group_table(pb) ? (size_t)pb.groups[g].rel0 : 0; }
+// group of person p (persons are stored group by group)
+GLAMR_HD int person_group(const glamr_problem_t& pb, int p) { return has_group_table(pb) ? pb.persons[p].group : 0; }
+// frames of person p, and the frame-person row of its frame 0
+GLAMR_HD int person_frames(const glamr_problem_t& pb, int p) { return group_frames(pb, person_group(pb, p)); }
+GLAMR_HD size_t person_row(const glamr_problem_t& pb, int p) {
+  if (!has_group_table(pb)) return (size_t)p * pb.T;
+  const glamr_group_t& gr = pb.groups[pb.persons[p].group];
+  return (size_t)gr.n0 + (size_t)(p - gr.p0) * gr.T;
+}
+// group of camera row r: a binary search over the groups' first rows
+GLAMR_HD int cam_row_group(const glamr_problem_t& pb, int r) {
+  if (!has_group_table(pb)) return 0;
+  int lo = 0, hi = pb.G - 1;
+  while (lo < hi) {
+    const int mid = (lo + hi + 1) >> 1;
+    if (pb.groups[mid].c0 <= r) lo = mid; else hi = mid - 1;
+  }
+  return lo;
+}
 // camera row of frame t seen by person p
-GLAMR_HD size_t cam_row(const OptCtx& c, int p, int t) { return (size_t)person_group(c.pb, p) * c.pb.T + t; }
+GLAMR_HD size_t cam_row(const OptCtx& c, int p, int t) { return group_cam_row0(c.pb, person_group(c.pb, p)) + t; }
+// weight / normaliser of term k in group g (the handle's scale with one group)
+GLAMR_HD float term_gs(const OptCtx& c, int g, int k) { return has_group_table(c.pb) ? c.pb.groups[g].gs[k] : c.gs[k]; }
+GLAMR_HD float term_norm(const glamr_problem_t& pb, int g, int k) { return has_group_table(pb) ? pb.groups[g].term_norm[k] : pb.term_norm[k]; }
 
 GLAMR_HD void mat34_inverse(const float* M, float* I) {
   // lib/utils/torch_transform.py:274-279  [R^T | -R^T t]
@@ -121,7 +150,7 @@ GLAMR_HD float traj_pre_vals(const OptCtx& c, int p, int i, float* tl) {
   return safe_atan2(sh, ch);
 }
 GLAMR_HD void traj_pre(const OptCtx& c, int p, int i) {
-  const int n = p * c.pb.T + c.pb.persons[p].start + i;
+  const size_t n = person_row(c.pb, p) + c.pb.persons[p].start + i;
   float tl[11];
   c.sc.heading[n] = traj_pre_vals(c, p, i, tl);
 #pragma unroll
@@ -138,7 +167,7 @@ GLAMR_HD void rotate_dxy(float h, float& x, float& y) {
 // after the inclusive scan of heading: rotate d_xy of frame i >= 1 by heading[i-1]
 GLAMR_HD void traj_mid(const OptCtx& c, int p, int i) {
   const glamr_person_t& ps = c.pb.persons[p];
-  const int n = p * c.pb.T + ps.start + i;
+  const size_t n = person_row(c.pb, p) + ps.start + i;
   const float* tl = c.sc.traj_local + (size_t)n * 11;
   float x = tl[0], y = tl[1];
   if (i > 0) rotate_dxy(c.sc.heading[n - 1], x, y);
@@ -163,8 +192,7 @@ GLAMR_HD bool traj_codec_frame(const OptCtx& c, const glamr_person_t& ps, int i)
 // produce); writes orient/trans base + world of frame-person n, returns nothing else
 GLAMR_HD void traj_post_vals(const OptCtx& c, int p, int t, const float* tl, float heading, float x, float y) {
   const glamr_person_t& ps = c.pb.persons[p];
-  const int T = c.pb.T;
-  const int n = p * T + t;
+  const size_t n = person_row(c.pb, p) + t;
   const int i = t - ps.start;
   float ob[3], tb[3];
   if (traj_codec_frame(c, ps, i)) {
@@ -220,7 +248,7 @@ GLAMR_HD void traj_post_vals(const OptCtx& c, int p, int t, const float* tl, flo
 }
 GLAMR_HD void traj_post(const OptCtx& c, int p, int t) {
   const glamr_person_t& ps = c.pb.persons[p];
-  const int n = p * c.pb.T + t;
+  const size_t n = person_row(c.pb, p) + t;
   const int i = t - ps.start;
   float* tl = c.sc.traj_local + (size_t)n * 11;
   if (traj_codec_frame(c, ps, i)) {
@@ -235,7 +263,7 @@ GLAMR_HD void traj_post(const OptCtx& c, int p, int t) {
 // global_recon_model.py:473-508.  cam[t] is world->cam, cam_inv[t] its inverse.
 GLAMR_HD void person_world_transform(const OptCtx& c, int p, int t, float* M) {
   // person_transform_world = make_transform(smpl_orient_world, root_trans_world)  (:470)
-  const size_t n = (size_t)p * c.pb.T + t;
+  const size_t n = person_row(c.pb, p) + t;
   float R[9];
   aa_to_rotmat(c.sc.orient_world + n * 3, R);
   M[0] = R[0]; M[1] = R[1]; M[2] = R[2]; M[3] = c.sc.trans_world[n * 3 + 0];
@@ -266,8 +294,8 @@ GLAMR_HD void person2cam_with_residual(const OptCtx& c, const glamr_person_t& ps
 GLAMR_HD void mean_cam_inv(const OptCtx& c, int g, int s, float* M) {
 #pragma unroll
   for (int k = 0; k < 12; ++k) M[k] = 0.0f;
-  const int Q = group_persons(c.pb);
-  for (int p = g * Q; p < (g + 1) * Q; ++p) {
+  const int p0 = group_first_person(c.pb, g), Q = group_persons(c.pb, g);
+  for (int p = p0; p < p0 + Q; ++p) {
     const glamr_person_t& ps = c.pb.persons[p];
     if (ps.vis[s] == 0.0f) continue;
     float Tw[12], C[12];
@@ -282,15 +310,16 @@ GLAMR_HD void mean_cam_inv(const OptCtx& c, int g, int s, float* M) {
 #pragma unroll
     for (int k = 0; k < 12; ++k) M[k] += C[k];
   }
-  const float inv = c.pb.inv_num_persons[(size_t)g * c.pb.T + s];
+  const float inv = c.pb.inv_num_persons[group_cam_row0(c.pb, g) + s];
 #pragma unroll
   for (int k = 0; k < 12; ++k) M[k] *= inv;
 }
-// camera of row gt = g*T + t (frame t of group g)
+// camera of row gt = c0 + t (frame t of group g)
 GLAMR_HD void cam_forward(const OptCtx& c, int gt) {
   float cam[12], inv[12];
   const int mode = c.pb.cam_mode;
-  const int g = gt / c.pb.T, t = gt - g * c.pb.T, og = group_theta(c.pb, g);
+  const int g = cam_row_group(c.pb, gt), t = gt - (int)group_cam_row0(c.pb, g);
+  const int orot = group_off_cam_rot(c.pb, g), otr = group_off_cam_trans(c.pb, g);
   if (mode == GLAMR_CAM_CONST) {
 #pragma unroll
     for (int k = 0; k < 12; ++k) cam[k] = c.pb.cam_pose_const[(size_t)gt * 12 + k];
@@ -298,8 +327,8 @@ GLAMR_HD void cam_forward(const OptCtx& c, int gt) {
   } else if (mode == GLAMR_CAM_PER_FRAME || mode == GLAMR_CAM_FIXED) {
     const int r = (mode == GLAMR_CAM_FIXED) ? 0 : t;
     float R[9];
-    rot6d_to_rotmat(c.theta + og + c.pb.off_cam_rot + 6 * r, R);
-    const float* tc = c.theta + og + c.pb.off_cam_trans + 3 * r;
+    rot6d_to_rotmat(c.theta + orot + 6 * r, R);
+    const float* tc = c.theta + otr + 3 * r;
     cam[0] = R[0]; cam[1] = R[1]; cam[2] = R[2]; cam[3] = tc[0];
     cam[4] = R[3]; cam[5] = R[4]; cam[6] = R[5]; cam[7] = tc[1];
     cam[8] = R[6]; cam[9] = R[7]; cam[10] = R[8]; cam[11] = tc[2];
@@ -312,7 +341,7 @@ GLAMR_HD void cam_forward(const OptCtx& c, int gt) {
     const int e = c.pb.empty_index[gt];
     if (e >= 0) {
 #pragma unroll
-      for (int k = 0; k < 6; ++k) d6[k] += c.theta[og + c.pb.off_cam_rot + 6 * e + k];
+      for (int k = 0; k < 6; ++k) d6[k] += c.theta[orot + 6 * e + k];
     }
 #pragma unroll
     for (int k = 0; k < 6; ++k) c.sc.cam_d6[(size_t)gt * 6 + k] = d6[k];
@@ -320,10 +349,10 @@ GLAMR_HD void cam_forward(const OptCtx& c, int gt) {
     float tt[3] = {M[3], M[7], M[11]};
     if (c.pb.trans_res_all) {
 #pragma unroll
-      for (int k = 0; k < 3; ++k) tt[k] += c.theta[og + c.pb.off_cam_trans + 3 * t + k];
+      for (int k = 0; k < 3; ++k) tt[k] += c.theta[otr + 3 * t + k];
     } else if (e >= 0) {
 #pragma unroll
-      for (int k = 0; k < 3; ++k) tt[k] += c.theta[og + c.pb.off_cam_trans + 3 * e + k];
+      for (int k = 0; k < 3; ++k) tt[k] += c.theta[otr + 3 * e + k];
     }
     inv[0] = R[0]; inv[1] = R[1]; inv[2] = R[2]; inv[3] = tt[0];
     inv[4] = R[3]; inv[5] = R[4]; inv[6] = R[5]; inv[7] = tt[1];
@@ -358,9 +387,9 @@ GLAMR_HD void kp_joint_terms(const OptCtx& c, int p, int t, int k, const float* 
                              const float* tw, KpGrad& o) {
   const glamr_person_t& ps = c.pb.persons[p];
   const int J = c.pb.J;
-  const size_t n = (size_t)p * c.pb.T + t;
+  const size_t n = person_row(c.pb, p) + t;
   const float* K = ps.cam_K + (size_t)t * 9;
-  const float gsk = c.gs[GLAMR_T_KP_2D];
+  const float gsk = term_gs(c, person_group(c.pb, p), GLAMR_T_KP_2D);
   float Xc[3], uv[2];
   mat3_vec(Rc, jw, Xc);
   Xc[0] += tc[0]; Xc[1] += tc[1]; Xc[2] += tc[2];
@@ -426,8 +455,8 @@ GLAMR_HD void frame_rest(const OptCtx& c, int p, int t, const KpGrad& kg, TermAc
   GLAMR_STAMP(4);
   const glamr_problem_t& pb = c.pb;
   const glamr_person_t& ps = pb.persons[p];
-  const int T = pb.T;
-  const size_t n = (size_t)p * T + t;
+  const int grp = person_group(pb, p), T = group_frames(pb, grp);
+  const size_t n = person_row(pb, p) + t;
   const float* ow = c.sc.orient_world + n * 3;
   const float* tw = c.sc.trans_world + n * 3;
   const float* cam = c.sc.cam + cam_row(c, p, t) * 12;
@@ -441,7 +470,7 @@ GLAMR_HD void frame_rest(const OptCtx& c, int p, int t, const KpGrad& kg, TermAc
   for (int k = 0; k < 9; ++k) g_Rc[k] = kg.g_Rc[k];
   acc.v[GLAMR_T_KP_2D] += kg.kp;
   acc.v[GLAMR_T_KP_2D_DIST] += kg.dist;
-  if (c.gs[GLAMR_T_KP_2D] != 0.0f) {
+  if (term_gs(c, grp, GLAMR_T_KP_2D) != 0.0f) {
     float g[3];
     rodrigues_smplx_vjp(ow, kg.g_Rs, g);
     g_ow[0] += g[0]; g_ow[1] += g[1]; g_ow[2] += g[2];
@@ -468,7 +497,7 @@ GLAMR_HD void frame_rest(const OptCtx& c, int p, int t, const KpGrad& kg, TermAc
       const float* qt = ps.orient_cam_q + (size_t)t * 4;
       quat_angle_dot(qt, q1, dd, dw);
       acc.v[GLAMR_T_CAM_TRAJ_ROT] += (double)(wr * dd * dd);
-      const float gsr = c.gs[GLAMR_T_CAM_TRAJ_ROT];
+      const float gsr = term_gs(c, grp, GLAMR_T_CAM_TRAJ_ROT);
       if (gsr != 0.0f) {
         const float gw = 2.0f * gsr * wr * dd * dw;          // dL/d(dot)
         const float gq[4] = {gw * qt[0], gw * qt[1], gw * qt[2], gw * qt[3]};
@@ -490,7 +519,7 @@ GLAMR_HD void frame_rest(const OptCtx& c, int p, int t, const KpGrad& kg, TermAc
 #pragma unroll
       for (int k = 0; k < 6; ++k) { diff[k] = ps.orient_cam_6d[(size_t)t * 6 + k] - r6[k]; ss += diff[k] * diff[k]; }
       acc.v[GLAMR_T_CAM_TRAJ_ROT] += (double)(wr * ss);
-      const float gsr = c.gs[GLAMR_T_CAM_TRAJ_ROT];
+      const float gsr = term_gs(c, grp, GLAMR_T_CAM_TRAJ_ROT);
       if (gsr != 0.0f) {
         float g6[6], gRa[9], ga[3], gM[9], t1[9], gRw[9], g[3];
 #pragma unroll
@@ -512,7 +541,7 @@ GLAMR_HD void frame_rest(const OptCtx& c, int p, int t, const KpGrad& kg, TermAc
 #pragma unroll
       for (int k = 0; k < 3; ++k) { d[k] = tcw[k] - ps.trans_cam[(size_t)t * 3 + k]; ss += d[k] * d[k]; }
       acc.v[GLAMR_T_CAM_TRAJ_TRANS] += (double)(wt * ss);
-      const float gst = c.gs[GLAMR_T_CAM_TRAJ_TRANS];
+      const float gst = term_gs(c, grp, GLAMR_T_CAM_TRAJ_TRANS);
       if (gst != 0.0f) {
         float g[3], gw[3];
 #pragma unroll
@@ -535,7 +564,7 @@ GLAMR_HD void frame_rest(const OptCtx& c, int p, int t, const KpGrad& kg, TermAc
   // ---- trajectory smoothness over ALL frames of the person (loss_func.py:117-144)
   if (pb.term_enabled[GLAMR_T_TRAJ_ROT_SMOOTH] && pb.traj_rot_smooth_quat) {
     // rot_type 'quat' (loss_func.py:126-128): (30 * quat_angle_diff(q[t+1], q[t]))^2 per frame pair
-    const float gsm = c.gs[GLAMR_T_TRAJ_ROT_SMOOTH];
+    const float gsm = term_gs(c, grp, GLAMR_T_TRAJ_ROT_SMOOTH);
     float q0[4], gq[4] = {0, 0, 0, 0};
     aa_to_quat(ow, q0);
     if (t + 1 < T) {
@@ -564,7 +593,7 @@ GLAMR_HD void frame_rest(const OptCtx& c, int p, int t, const KpGrad& kg, TermAc
     float r6[6], rp[6], rn[6], R2[9];
     rotmat_to_rot6d(Rw, r6);
     float g6[6] = {0, 0, 0, 0, 0, 0};
-    const float gsm = c.gs[GLAMR_T_TRAJ_ROT_SMOOTH];
+    const float gsm = term_gs(c, grp, GLAMR_T_TRAJ_ROT_SMOOTH);
     if (t + 1 < T) {
       aa_to_rotmat(ow + 3, R2);
       rotmat_to_rot6d(R2, rn);
@@ -588,7 +617,7 @@ GLAMR_HD void frame_rest(const OptCtx& c, int p, int t, const KpGrad& kg, TermAc
     }
   }
   if (pb.term_enabled[GLAMR_T_TRAJ_TRANS_SMOOTH]) {
-    const float gsm = c.gs[GLAMR_T_TRAJ_TRANS_SMOOTH];
+    const float gsm = term_gs(c, grp, GLAMR_T_TRAJ_TRANS_SMOOTH);
     if (t + 1 < T) {
       float ss = 0.0f;
 #pragma unroll
@@ -605,22 +634,22 @@ GLAMR_HD void frame_rest(const OptCtx& c, int p, int t, const KpGrad& kg, TermAc
   // ---- relative transforms between the persons of one group (loss_func.py:248-271): W_ij = inv(T_i) T_j against C_ij.  i, j are
   // indices inside the group; the group's pair tables start at rel_target / rel_w / rel_wt + its block
   if (pb.rel_target && pb.term_enabled[GLAMR_T_REL_TRANSFORM]) {
-    const float gsr = c.gs[GLAMR_T_REL_TRANSFORM];
+    const float gsr = term_gs(c, grp, GLAMR_T_REL_TRANSFORM);
     const float twt = pb.rel_trans_weight;
-    const int Q = group_persons(pb), g = person_group(pb, p), i = p - g * Q;
-    const size_t pairs0 = (size_t)g * Q * Q;
+    const int Q = group_persons(pb, grp), i = p - group_first_person(pb, grp);
+    const size_t rel0 = group_rel0(pb, grp), row0 = group_first_row(pb, grp);
     for (int j = 0; j < Q; ++j) {
       if (j == i) continue;
-      const size_t nj = ((size_t)g * Q + j) * T + t;
-      const float w_ij = pb.rel_w[(pairs0 + (size_t)i * Q + j) * T + t], wt_ij = pb.rel_wt[(pairs0 + (size_t)i * Q + j) * T + t];
-      const float w_ji = pb.rel_w[(pairs0 + (size_t)j * Q + i) * T + t], wt_ji = pb.rel_wt[(pairs0 + (size_t)j * Q + i) * T + t];
+      const size_t nj = row0 + (size_t)j * T + t;
+      const float w_ij = pb.rel_w[rel0 + ((size_t)i * Q + j) * T + t], wt_ij = pb.rel_wt[rel0 + ((size_t)i * Q + j) * T + t];
+      const float w_ji = pb.rel_w[rel0 + ((size_t)j * Q + i) * T + t], wt_ji = pb.rel_wt[rel0 + ((size_t)j * Q + i) * T + t];
       if (w_ij == 0.0f && wt_ij == 0.0f && w_ji == 0.0f && wt_ji == 0.0f) continue;
       float Rj[9];
       aa_to_rotmat(c.sc.orient_world + nj * 3, Rj);
       const float* tj = c.sc.trans_world + nj * 3;
       const float dt[3] = {tj[0] - tw[0], tj[1] - tw[1], tj[2] - tw[2]};
       {  // pair (i,j): R_W = Ri^T Rj, t_W = Ri^T (tj - ti); this thread owns its loss value and dL/dT_i
-        const float* C = pb.rel_target + ((pairs0 + (size_t)i * Q + j) * T + t) * 12;
+        const float* C = pb.rel_target + (rel0 + ((size_t)i * Q + j) * T + t) * 12;
         float RW[9], tW[3], gRW[9] = {0, 0, 0, 0, 0, 0, 0, 0, 0}, gtW[3];
         mat3_tmul(Rw, Rj, RW);
         mat3_tvec(Rw, dt, tW);
@@ -653,7 +682,7 @@ GLAMR_HD void frame_rest(const OptCtx& c, int p, int t, const KpGrad& kg, TermAc
       }
       if (gsr != 0.0f && (w_ji != 0.0f || wt_ji != 0.0f)) {
         // pair (j,i): R_W' = Rj^T Ri, t_W' = Rj^T (ti - tj); only dL/dT_i here (thread (j,t) adds the value)
-        const float* C = pb.rel_target + ((pairs0 + (size_t)j * Q + i) * T + t) * 12;
+        const float* C = pb.rel_target + (rel0 + ((size_t)j * Q + i) * T + t) * 12;
         float RW[9], tW[3], gRW[9] = {0, 0, 0, 0, 0, 0, 0, 0, 0}, gtW[3];
         const float mdt[3] = {-dt[0], -dt[1], -dt[2]};
         mat3_tmul(Rj, Rw, RW);
@@ -691,7 +720,7 @@ GLAMR_HD void frame_rest(const OptCtx& c, int p, int t, const KpGrad& kg, TermAc
 
 // Sequential form (host harness): all joints of (p,t), then the rest.
 GLAMR_HD void frame_residuals(const OptCtx& c, int p, int t, TermAcc& acc) {
-  const size_t n = (size_t)p * c.pb.T + t;
+  const size_t n = person_row(c.pb, p) + t;
   const float* cam = c.sc.cam + cam_row(c, p, t) * 12;
   float Rc[9], tc[3], Rs[9];
   mat34_R(cam, Rc);
@@ -710,12 +739,12 @@ GLAMR_HD void frame_residuals(const OptCtx& c, int p, int t, TermAcc& acc) {
 // persons' world transforms).
 GLAMR_HD void camera_backward(const OptCtx& c, int gt, TermAcc& acc) {
   const glamr_problem_t& pb = c.pb;
-  const int T = pb.T;
-  const int grp = gt / T, t = gt - grp * T, Q = group_persons(pb);
-  const int off_rot = group_theta(pb, grp) + pb.off_cam_rot, off_trans = group_theta(pb, grp) + pb.off_cam_trans;
+  const int grp = cam_row_group(pb, gt), T = group_frames(pb, grp), t = gt - (int)group_cam_row0(pb, grp), Q = group_persons(pb, grp);
+  const int off_rot = group_off_cam_rot(pb, grp), off_trans = group_off_cam_trans(pb, grp);
+  const size_t row0 = group_first_row(pb, grp);
   float G[12] = {0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0};   // dL/dRc (9) , dL/dtc (3)
-  for (int p = grp * Q; p < (grp + 1) * Q; ++p) {          // frame-persons of other ranks hold zeros (frame_residuals_kernel)
-    const float* g = c.sc.g_cam + ((size_t)p * T + t) * 12;
+  for (int q = 0; q < Q; ++q) {          // frame-persons of other ranks hold zeros (frame_residuals_kernel)
+    const float* g = c.sc.g_cam + (row0 + (size_t)q * T + t) * 12;
 #pragma unroll
     for (int k = 0; k < 12; ++k) G[k] += g[k];
   }
@@ -724,7 +753,7 @@ GLAMR_HD void camera_backward(const OptCtx& c, int gt, TermAcc& acc) {
   float gRi[9] = {0, 0, 0, 0, 0, 0, 0, 0, 0}, gti[3] = {0, 0, 0};   // w.r.t. cam_inv
   if (pb.owner) {
     if (pb.term_enabled[GLAMR_T_CAM_INV_ROT_SMOOTH] && T > 1) {
-      const float gs = c.gs[GLAMR_T_CAM_INV_ROT_SMOOTH];
+      const float gs = term_gs(c, grp, GLAMR_T_CAM_INV_ROT_SMOOTH);
       float ss = 0.0f;
 #pragma unroll
       for (int a = 0; a < 3; ++a)
@@ -737,7 +766,7 @@ GLAMR_HD void camera_backward(const OptCtx& c, int gt, TermAcc& acc) {
       acc.v[GLAMR_T_CAM_INV_ROT_SMOOTH] += (double)(kFps2 * ss);
     }
     if (pb.term_enabled[GLAMR_T_CAM_ORIGIN_SMOOTH] && T > 1) {
-      const float gs = c.gs[GLAMR_T_CAM_ORIGIN_SMOOTH];
+      const float gs = term_gs(c, grp, GLAMR_T_CAM_ORIGIN_SMOOTH);
       float ss = 0.0f;
 #pragma unroll
       for (int a = 0; a < 3; ++a) {
@@ -750,7 +779,7 @@ GLAMR_HD void camera_backward(const OptCtx& c, int gt, TermAcc& acc) {
     if (pb.term_enabled[GLAMR_T_CAM_DEPTH_SMOOTH] && T > 1) {
       // loss_func.py:94-103: velocity of the camera origin along the NEXT frame's optical axis (third column of
       // cam_pose_inv[t+1]), squared and SUMMED over the T-1 frame pairs (the trailing .mean() acts on a 0-d tensor)
-      const float gs = c.gs[GLAMR_T_CAM_DEPTH_SMOOTH];
+      const float gs = term_gs(c, grp, GLAMR_T_CAM_DEPTH_SMOOTH);
       if (t + 1 < T) {            // pair (t, t+1): this frame is the "previous" origin
         float d = 0.0f;
 #pragma unroll
@@ -774,7 +803,7 @@ GLAMR_HD void camera_backward(const OptCtx& c, int gt, TermAcc& acc) {
       float w = (t < 10) ? pb.cam_up_first_weight : 1.0f;
       if (pb.cam_up_first_only && t > 0) w = 0.0f;
       acc.v[GLAMR_T_CAM_UP_REG] += (double)(w * inv[2 * 4 + 1]);
-      gRi[2 * 3 + 1] += c.gs[GLAMR_T_CAM_UP_REG] * w;
+      gRi[2 * 3 + 1] += term_gs(c, grp, GLAMR_T_CAM_UP_REG) * w;
     }
   }
   const int mode = pb.cam_mode;
@@ -797,7 +826,7 @@ GLAMR_HD void camera_backward(const OptCtx& c, int gt, TermAcc& acc) {
     if (pb.owner && mode == GLAMR_CAM_PER_FRAME) {
       // smoothness directly on the camera variables (loss_func.py:60-73)
       if (pb.term_enabled[GLAMR_T_CAM_ROT_SMOOTH] && T > 1) {
-        const float gs = c.gs[GLAMR_T_CAM_ROT_SMOOTH];
+        const float gs = term_gs(c, grp, GLAMR_T_CAM_ROT_SMOOTH);
         const float* x = c.theta + off_rot + 6 * t;
         float ss = 0.0f;
 #pragma unroll
@@ -808,7 +837,7 @@ GLAMR_HD void camera_backward(const OptCtx& c, int gt, TermAcc& acc) {
         acc.v[GLAMR_T_CAM_ROT_SMOOTH] += (double)(kFps2 * ss);
       }
       if (pb.term_enabled[GLAMR_T_CAM_TRANS_SMOOTH] && T > 1) {
-        const float gs = c.gs[GLAMR_T_CAM_TRANS_SMOOTH];
+        const float gs = term_gs(c, grp, GLAMR_T_CAM_TRANS_SMOOTH);
         const float* x = c.theta + off_trans + 3 * t;
         float ss = 0.0f;
 #pragma unroll
@@ -855,7 +884,7 @@ GLAMR_HD void camera_backward(const OptCtx& c, int gt, TermAcc& acc) {
     if (trow >= 0) {
       float gr[3] = {gti[0], gti[1], gti[2]};
       if (pb.owner && pb.term_enabled[GLAMR_T_CAM_INV_TRANS_RES_REG]) {
-        const float gs = c.gs[GLAMR_T_CAM_INV_TRANS_RES_REG];
+        const float gs = term_gs(c, grp, GLAMR_T_CAM_INV_TRANS_RES_REG);
         float ss = 0.0f;
 #pragma unroll
         for (int k = 0; k < 3; ++k) { const float x = c.theta[off_trans + 3 * trow + k]; ss += x * x; gr[k] += 2.0f * kFps2 * gs * x; }
@@ -878,26 +907,27 @@ GLAMR_HD void camera_backward(const OptCtx& c, int gt, TermAcc& acc) {
 // into their person2cam residuals at frame s (a person invisible at s gets none: the reference multiplies its term by vis_frames).
 GLAMR_HD void camera_scatter_to_persons(const OptCtx& c, int gs) {
   const glamr_problem_t& pb = c.pb;
-  const int T = pb.T;
-  const int grp = gs / T, s = gs - grp * T, Q = group_persons(pb);
-  const int32_t* fill = pb.fill_src + (size_t)grp * T;
+  const int grp = cam_row_group(pb, gs), T = group_frames(pb, grp), Q = group_persons(pb, grp), p0 = group_first_person(pb, grp);
+  const size_t c0 = group_cam_row0(pb, grp);
+  const int s = gs - (int)c0;
+  const int32_t* fill = pb.fill_src + c0;
   if (fill[s] != s || pb.inv_num_persons[gs] == 0.0f) return;
   float G[12] = {0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0};
   for (int t = 0; t < T; ++t) {
     if (fill[t] != s) continue;
-    const float* g = c.sc.g_cam_fix + ((size_t)grp * T + t) * 12;
+    const float* g = c.sc.g_cam_fix + (c0 + t) * 12;
 #pragma unroll
     for (int k = 0; k < 12; ++k) G[k] += g[k];
   }
   const float inv_n = pb.inv_num_persons[gs];
 #pragma unroll
   for (int k = 0; k < 12; ++k) G[k] *= inv_n;
-  for (int p = grp * Q; p < (grp + 1) * Q; ++p) {
+  for (int p = p0; p < p0 + Q; ++p) {
     const glamr_person_t& ps = pb.persons[p];
     if (ps.vis[s] == 0.0f) continue;
     // M = Tw @ P2C: R_M = Rw Rp, t_M = Rw tp + tw  ->  dRw = G_R Rp^T + G_t tp^T, dtw = G_t
     const float* P2C = ps.person2cam + (size_t)s * 12;
-    const size_t n = (size_t)p * T + s;
+    const size_t n = person_row(pb, p) + s;
     float Rp[9], gRw[9], g[3], tp[3];
     if (pb.has_person2cam) {
       float P2Cr[12];
@@ -937,8 +967,8 @@ GLAMR_HD void camera_scatter_to_persons(const OptCtx& c, int gs) {
 GLAMR_HD void traj_back_pre(const OptCtx& c, int p, int t, TermAcc& acc) {
   const glamr_problem_t& pb = c.pb;
   const glamr_person_t& ps = pb.persons[p];
-  const int T = pb.T;
-  const size_t n = (size_t)p * T + t;
+  const int grp = person_group(pb, p);
+  const size_t n = person_row(pb, p) + t;
   const int i = t - ps.start;
   float g_ow[3], g_tw[3];
 #pragma unroll
@@ -956,13 +986,13 @@ GLAMR_HD void traj_back_pre(const OptCtx& c, int p, int t, TermAcc& acc) {
       if (pb.term_enabled[GLAMR_T_ROT_RES]) {
         float ss = 0.0f;
 #pragma unroll
-        for (int k = 0; k < 3; ++k) { const float x = c.theta[ps.off_orient_res + t * 3 + k]; ss += x * x; go[k] += 2.0f * kFps2 * c.gs[GLAMR_T_ROT_RES] * x; }
+        for (int k = 0; k < 3; ++k) { const float x = c.theta[ps.off_orient_res + t * 3 + k]; ss += x * x; go[k] += 2.0f * kFps2 * term_gs(c, grp, GLAMR_T_ROT_RES) * x; }
         acc.v[GLAMR_T_ROT_RES] += (double)(kFps2 * ss);
       }
       if (pb.term_enabled[GLAMR_T_TRANS_RES]) {
         float ss = 0.0f;
 #pragma unroll
-        for (int k = 0; k < 3; ++k) { const float x = c.theta[ps.off_trans_res + t * 3 + k]; ss += x * x; gt[k] += 2.0f * kFps2 * c.gs[GLAMR_T_TRANS_RES] * x; }
+        for (int k = 0; k < 3; ++k) { const float x = c.theta[ps.off_trans_res + t * 3 + k]; ss += x * x; gt[k] += 2.0f * kFps2 * term_gs(c, grp, GLAMR_T_TRANS_RES) * x; }
         acc.v[GLAMR_T_TRANS_RES] += (double)(kFps2 * ss);
       }
     }
@@ -995,13 +1025,13 @@ GLAMR_HD void traj_back_pre(const OptCtx& c, int p, int t, TermAcc& acc) {
     for (int k = 0; k < 6; ++k) {
       const float x = c.theta[ps.off_rot + 6 * i + k];
       float g = 0.0f;
-      if (pb.owner) { ssr += x * x; g = 2.0f * kFps2 * c.gs[GLAMR_T_ROT_REG] * x; }
+      if (pb.owner) { ssr += x * x; g = 2.0f * kFps2 * term_gs(c, grp, GLAMR_T_ROT_REG) * x; }
       c.sc.grad[ps.off_rot + 6 * i + k] = g;
     }
     const float x = c.theta[ps.off_z + i];
     float g = 0.0f;
     if (pb.owner) {
-      g = 2.0f * kFps2 * c.gs[GLAMR_T_Z_REG] * x;
+      g = 2.0f * kFps2 * term_gs(c, grp, GLAMR_T_Z_REG) * x;
       if (pb.term_enabled[GLAMR_T_Z_REG]) acc.v[GLAMR_T_Z_REG] += (double)(kFps2 * x * x);
       if (pb.term_enabled[GLAMR_T_ROT_REG]) acc.v[GLAMR_T_ROT_REG] += (double)(kFps2 * ssr);
     }
@@ -1030,14 +1060,14 @@ GLAMR_HD void traj_back_pre(const OptCtx& c, int p, int t, TermAcc& acc) {
     for (int k = 0; k < 6; ++k) {
       const float x = c.theta[ps.off_rot + 6 * i + k];
       float g = g6[k] * rm;
-      if (pb.owner) { ssr += x * x; g += 2.0f * kFps2 * c.gs[GLAMR_T_ROT_REG] * x; }
+      if (pb.owner) { ssr += x * x; g += 2.0f * kFps2 * term_gs(c, grp, GLAMR_T_ROT_REG) * x; }
       c.sc.grad[ps.off_rot + 6 * i + k] = g;
     }
     {
       const float x = c.theta[ps.off_z + i];
       float g = g_tb[2];
       if (pb.owner) {
-        g += 2.0f * kFps2 * c.gs[GLAMR_T_Z_REG] * x;
+        g += 2.0f * kFps2 * term_gs(c, grp, GLAMR_T_Z_REG) * x;
         if (pb.term_enabled[GLAMR_T_Z_REG]) acc.v[GLAMR_T_Z_REG] += (double)(kFps2 * x * x);
         if (pb.term_enabled[GLAMR_T_ROT_REG]) acc.v[GLAMR_T_ROT_REG] += (double)(kFps2 * ssr);
       }
@@ -1055,7 +1085,8 @@ GLAMR_HD void traj_back_pre(const OptCtx& c, int p, int t, TermAcc& acc) {
 GLAMR_HD void traj_back_mid(const OptCtx& c, int p, int i, TermAcc& acc) {
   const glamr_problem_t& pb = c.pb;
   const glamr_person_t& ps = pb.persons[p];
-  const size_t n = (size_t)p * pb.T + ps.start + i;
+  const int grp = person_group(pb, p);
+  const size_t n = person_row(pb, p) + ps.start + i;
   const bool codec = pb.traj_source == GLAMR_TRAJ_PREDICTED;
   const float Gx = codec ? c.sc.g_xy[2 * n] : 0.0f, Gy = codec ? c.sc.g_xy[2 * n + 1] : 0.0f;
   if (i == 0) {
@@ -1071,8 +1102,8 @@ GLAMR_HD void traj_back_mid(const OptCtx& c, int p, int i, TermAcc& acc) {
     }
     const float x = c.theta[ps.off_dxy + 2 * (i - 1)], y = c.theta[ps.off_dxy + 2 * (i - 1) + 1];
     if (pb.owner) {
-      gx += 2.0f * kFps2 * c.gs[GLAMR_T_DXY_REG] * x;
-      gy += 2.0f * kFps2 * c.gs[GLAMR_T_DXY_REG] * y;
+      gx += 2.0f * kFps2 * term_gs(c, grp, GLAMR_T_DXY_REG) * x;
+      gy += 2.0f * kFps2 * term_gs(c, grp, GLAMR_T_DXY_REG) * y;
       if (pb.term_enabled[GLAMR_T_DXY_REG]) acc.v[GLAMR_T_DXY_REG] += (double)(kFps2 * (x * x + y * y));
     }
     c.sc.grad[ps.off_dxy + 2 * (i - 1)] = gx;
@@ -1095,7 +1126,8 @@ GLAMR_HD void traj_back_mid(const OptCtx& c, int p, int i, TermAcc& acc) {
 GLAMR_HD void traj_back_post(const OptCtx& c, int p, int i, TermAcc& acc) {
   const glamr_problem_t& pb = c.pb;
   const glamr_person_t& ps = pb.persons[p];
-  const size_t n = (size_t)p * pb.T + ps.start + i;
+  const int grp = person_group(pb, p);
+  const size_t n = person_row(pb, p) + ps.start + i;
   const float G = pb.traj_source == GLAMR_TRAJ_PREDICTED ? c.sc.g_head[n] : 0.0f;
   const int nc = pb.heading_vec ? 2 : 1;
   float gx = G, gy = 0.0f;
@@ -1117,7 +1149,7 @@ GLAMR_HD void traj_back_post(const OptCtx& c, int p, int i, TermAcc& acc) {
     float g = (k == 0 ? gx : gy) * m;
     if (pb.owner) {
       const float sx = sinf(x), cx = cosf(x);
-      g += 2.0f * kFps2 * c.gs[GLAMR_T_DHEADING_REG] * x + 2.0f * kFps2 * c.gs[GLAMR_T_DHEADING_REG_NEW] * sx;
+      g += 2.0f * kFps2 * term_gs(c, grp, GLAMR_T_DHEADING_REG) * x + 2.0f * kFps2 * term_gs(c, grp, GLAMR_T_DHEADING_REG_NEW) * sx;
       s_reg += (double)(kFps2 * x * x);
       s_reg_new += (double)(kFps2 * ((cx - 1.0f) * (cx - 1.0f) + sx * sx));
     }

@@ -11,6 +11,7 @@
 #include <stdlib.h>
 #include <algorithm>
 #include <string.h>
+#include <vector>
 
 #include "globalopt_frames.cuh"
 #include "smpl_model.cuh"
@@ -20,17 +21,48 @@ namespace glamr {
 
 constexpr int kFrameThreads = 128;
 
-// Partial-sum slots of the loss terms, per seed group (include/glamr_b200.h, glamr_problem_t.G): every group has its own block of
-// `per_group` slots, [res residual CTAs | Q persons | cam camera CTAs of traj_cam_backward_kernel | cam3 CTAs of
-// camera_backward_kernel], and each group's CTAs cover that group's frame-persons / frames exactly as the CTAs of the one-group
-// problem do, so that every group's term sums see the same elements in the same order as its one-group run.
-struct SlotLayout {
-  int res;          // residual CTAs per group: ceil(Q*T / 4)
-  int persons;      // Q = P / G
-  int cam;          // camera CTAs of kScanThreads frames per group (traj_cam_forward / traj_cam_backward)
-  int cam3;         // camera CTAs of kFrameThreads frames per group (camera_backward_kernel, mode 3)
-  int per_group;    // res + persons + cam + cam3
+// Partial-sum slots of the loss terms, per group (include/glamr_b200.h, glamr_group_t): every group has its own block of slots,
+// [residual CTAs | Q persons | camera CTAs of traj_cam_backward_kernel | camera CTAs of camera_backward_kernel], and each group's CTAs
+// cover that group's frame-persons / frames exactly as the CTAs of its one-group problem do, so that every group's term sums see the
+// same elements in the same order as its one-group run.
+struct GroupGrid {
+  int res0;         // first residual CTA of the group (4 frame-persons each)
+  int cam0;         // first camera CTA of kScanThreads frames (traj_cam_forward / traj_cam_backward)
+  int cam30;        // first camera CTA of kFrameThreads frames (camera_backward_kernel, mode 3)
+  int slot0;        // first partial-sum slot
 };
+struct SlotLayout {
+  int res;          // one group: residual CTAs, ceil(Q*T / 4)
+  int persons;      // one group: Q = P
+  int cam;          // one group: camera CTAs of kScanThreads frames
+  int cam3;         // one group: camera CTAs of kFrameThreads frames
+  int n_res, n_cam, n_cam3;    // CTAs of all groups
+  int cam_rows;     // camera rows of all groups (sum T)
+  const GroupGrid* grid;       // several groups: [G+1] first CTAs and slots of each group, entry G the totals
+};
+
+// The group whose CTAs [grid[g].*f, grid[g+1].*f) hold CTA b: a binary search over the G groups' first CTAs.  It runs only with
+// several groups; one group maps CTA b to itself without touching memory.
+__device__ int grid_group(const SlotLayout& sl, int G, int GroupGrid::*f, int b) {
+  int lo = 0, hi = G - 1;
+  while (lo < hi) {
+    const int mid = (lo + hi + 1) >> 1;
+    if (sl.grid[mid].*f <= b) lo = mid; else hi = mid - 1;
+  }
+  return lo;
+}
+// first slot of part `part` (0 residual CTAs, 1 persons, 2 camera CTAs, 3 mode-3 camera CTAs) of group g's block; part 4 = the end of
+// the block
+__host__ __device__ inline int group_slot(const SlotLayout& sl, const glamr_problem_t& pb, int g, int part) {
+  int s = 0, n[4] = {sl.res, sl.persons, sl.cam, sl.cam3};
+  if (num_groups(pb) > 1) {
+    const GroupGrid &a = sl.grid[g], &b = sl.grid[g + 1];
+    s = a.slot0;
+    n[0] = b.res0 - a.res0; n[1] = group_persons(pb, g); n[2] = b.cam0 - a.cam0; n[3] = b.cam30 - a.cam30;
+  }
+  for (int k = 0; k < part; ++k) s += n[k];
+  return s;
+}
 
 __device__ void block_reduce_terms(const TermAcc& acc, double* out /*[NUM_TERMS]*/, double* smem /*[warps][NUM_TERMS]*/) {
   const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5, nw = blockDim.x >> 5;
@@ -63,8 +95,8 @@ __device__ bool grid_last_block(unsigned int* ticket) {
   return last;
 }
 
-// blocks [0,P): trajectory codec of one person; blocks [P, P+G*cam_blocks): camera of 256 frames of one group each (modes 0-2)
-__global__ void __launch_bounds__(kScanThreads) traj_cam_forward_kernel(OptCtx c, int with_cam, int cam_blocks) {
+// blocks [0,P): trajectory codec of one person; blocks [P, P+sl.n_cam): camera of 256 frames of one group each (modes 0-2)
+__global__ void __launch_bounds__(kScanThreads) traj_cam_forward_kernel(OptCtx c, int with_cam, SlotLayout sl) {
   __shared__ float sm[kScanThreads / 32 + 1];
   pdl_launch_dependents();
   pdl_wait();
@@ -72,15 +104,16 @@ __global__ void __launch_bounds__(kScanThreads) traj_cam_forward_kernel(OptCtx c
   const int n_reduce = c.pb.n_params + num_groups(c.pb) * GLAMR_NUM_TERMS;
   for (int i = blockIdx.x * kScanThreads + threadIdx.x; i < n_reduce; i += gridDim.x * kScanThreads) c.sc.grad[i] = 0.0f;
   if ((int)blockIdx.x >= c.pb.P) {
-    const int b = blockIdx.x - c.pb.P, g = b / cam_blocks;
-    const int t = (b - g * cam_blocks) * kScanThreads + threadIdx.x;
-    if (with_cam && t < c.pb.T) cam_forward(c, g * c.pb.T + t);
+    const int b = blockIdx.x - c.pb.P, G = num_groups(c.pb);
+    const int g = G > 1 ? grid_group(sl, G, &GroupGrid::cam0, b) : 0;
+    const int t = (G > 1 ? b - sl.grid[g].cam0 : b) * kScanThreads + threadIdx.x;
+    if (with_cam && t < group_frames(c.pb, g)) cam_forward(c, (int)group_cam_row0(c.pb, g) + t);
     return;
   }
   const int p = blockIdx.x;
   const glamr_person_t& ps = c.pb.persons[p];
-  const int len = ps.len, T = c.pb.T;
-  const size_t n0 = (size_t)p * T + ps.start;
+  const int len = ps.len, T = person_frames(c.pb, p);
+  const size_t n0 = person_row(c.pb, p) + ps.start;
   if (c.pb.traj_source == GLAMR_TRAJ_PREDICTED) {          // uniform over the grid: the barriers below stay CTA-wide
     for (int i = threadIdx.x; i < len; i += kScanThreads) traj_pre(c, p, i);
     __syncthreads();
@@ -95,31 +128,33 @@ __global__ void __launch_bounds__(kScanThreads) traj_cam_forward_kernel(OptCtx c
   for (int t = threadIdx.x; t < T; t += kScanThreads) traj_post(c, p, t);
 }
 
-__global__ void __launch_bounds__(kFrameThreads) cam_forward_kernel(OptCtx c) {
+__global__ void __launch_bounds__(kFrameThreads) cam_forward_kernel(OptCtx c, int cam_rows) {
   pdl_launch_dependents();
   pdl_wait();
   const int gt = blockIdx.x * blockDim.x + threadIdx.x;
-  if (gt < num_groups(c.pb) * c.pb.T) cam_forward(c, gt);
+  if (gt < cam_rows) cam_forward(c, gt);
 }
 
 // One warp per frame-person: lanes = joints for the SMPL joint assembly (lib/models/smpl.py:299-315, fused here) and the
-// reprojection terms, warp-shuffle sums, then lane 0 finishes the per-frame terms.  4 frame-persons of one seed group per CTA:
-// sl.res CTAs per group (the last one of a group may run idle warps), so a group's partial sums match its one-group run.
+// reprojection terms, warp-shuffle sums, then lane 0 finishes the per-frame terms.  4 frame-persons of one group per CTA:
+// ceil(Q*T / 4) CTAs per group (the last one of a group may run idle warps), so a group's partial sums match its one-group run.
 __global__ void __launch_bounds__(kFrameThreads) frame_residuals_kernel(OptCtx c, SmplDev m, SmplWorkspace wo, int n_begin, double* partial,
                                                                         SlotLayout sl) {
   __shared__ double sm[(kFrameThreads / 32) * GLAMR_NUM_TERMS];
   pdl_launch_dependents();
   pdl_wait();
   const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
-  const int g = blockIdx.x / sl.res, lb = blockIdx.x - g * sl.res;
-  const int Ng = sl.persons * c.pb.T, J = c.pb.J;
+  const int G = num_groups(c.pb);
+  const int g = G > 1 ? grid_group(sl, G, &GroupGrid::res0, blockIdx.x) : 0;
+  const int lb = G > 1 ? blockIdx.x - sl.grid[g].res0 : blockIdx.x;
+  const int T = group_frames(c.pb, g), Ng = group_persons(c.pb, g) * T, J = c.pb.J;
   const int ng = lb * (kFrameThreads / 32) + wid;           // frame-person inside the group
-  const int n = g * Ng + ng;
+  const int n = (int)group_first_row(c.pb, g) + ng;
   GLAMR_STAMP(0);
   TermAcc acc;
   acc.clear();
   if (ng < Ng) {
-    const int p = n / c.pb.T, t = n - p * c.pb.T;
+    const int q = ng / T, t = ng - q * T, p = group_first_person(c.pb, g) + q;
     if (n >= c.pb.n_begin && n < c.pb.n_end) {
       const int nl = n - n_begin;
       const float* tw = c.sc.trans_world + (size_t)n * 3;
@@ -164,7 +199,7 @@ __global__ void __launch_bounds__(kFrameThreads) frame_residuals_kernel(OptCtx c
   if (threadIdx.x < GLAMR_NUM_TERMS) {
     double s = 0.0;
     for (int w = 0; w < kFrameThreads / 32; ++w) s += sm[w * GLAMR_NUM_TERMS + threadIdx.x];
-    partial[((size_t)g * sl.per_group + lb) * GLAMR_NUM_TERMS + threadIdx.x] = s;
+    partial[((size_t)group_slot(sl, c.pb, g, 0) + lb) * GLAMR_NUM_TERMS + threadIdx.x] = s;
   }
   GLAMR_STAMP(11);
 }
@@ -177,24 +212,26 @@ extern "C" int glamr_exp_frame_stamps(long long* out32) {     // experiment buil
 }
 #endif
 
-// sl.cam3 CTAs of kFrameThreads frames per seed group
+// ceil(T / kFrameThreads) CTAs per group
 __global__ void __launch_bounds__(kFrameThreads) camera_backward_kernel(OptCtx c, double* partial, SlotLayout sl) {
   __shared__ double sm[(kFrameThreads / 32) * GLAMR_NUM_TERMS];
   pdl_launch_dependents();
   pdl_wait();
-  const int g = blockIdx.x / sl.cam3, lb = blockIdx.x - g * sl.cam3;
+  const int G = num_groups(c.pb);
+  const int g = G > 1 ? grid_group(sl, G, &GroupGrid::cam30, blockIdx.x) : 0;
+  const int lb = G > 1 ? blockIdx.x - sl.grid[g].cam30 : blockIdx.x;
   const int t = lb * blockDim.x + threadIdx.x;
   TermAcc acc;
   acc.clear();
-  if (t < c.pb.T) camera_backward(c, g * c.pb.T + t, acc);
-  block_reduce_terms(acc, partial + ((size_t)g * sl.per_group + sl.res + sl.persons + sl.cam + lb) * GLAMR_NUM_TERMS, sm);
+  if (t < group_frames(c.pb, g)) camera_backward(c, (int)group_cam_row0(c.pb, g) + t, acc);
+  block_reduce_terms(acc, partial + ((size_t)group_slot(sl, c.pb, g, 3) + lb) * GLAMR_NUM_TERMS, sm);
 }
 
-__global__ void __launch_bounds__(kFrameThreads) camera_scatter_kernel(OptCtx c) {
+__global__ void __launch_bounds__(kFrameThreads) camera_scatter_kernel(OptCtx c, int cam_rows) {
   pdl_launch_dependents();
   pdl_wait();
   const int gs = blockIdx.x * blockDim.x + threadIdx.x;
-  if (gs < num_groups(c.pb) * c.pb.T) camera_scatter_to_persons(c, gs);
+  if (gs < cam_rows) camera_scatter_to_persons(c, gs);
 }
 
 // ---- cross-GPU reduction over NVLink peer memory (one process per GPU, buffers exchanged as CUDA IPC handles) --------
@@ -241,24 +278,26 @@ __device__ __forceinline__ float peer_take(const PeerCtx& pc, uint32_t e, int sr
   return __uint_as_float((uint32_t)w);
 }
 
-// loss partials -> un-normalised term sums of every group (reduce_buf tail: the first n_slots slots of each group's block, in slot
-// order); fixed camera: each group's per-frame gradients summed over its T frames
-__device__ void reduce_tail(const OptCtx& c, const double* partial, int n_slots, int per_group, float* reduce_buf, double* sm /*[8*16]*/) {
+// loss partials -> un-normalised term sums of every group (reduce_buf tail: the slots of each group's block that hold partial sums,
+// in slot order; cam3: the mode-3 camera slots too); fixed camera: each group's per-frame gradients summed over its T frames
+__device__ void reduce_tail(const OptCtx& c, const double* partial, const SlotLayout& sl, bool cam3, float* reduce_buf, double* sm /*[8*16]*/) {
   const int tid = threadIdx.x, lane = tid & 31, wid = tid >> 5;
   const int G = num_groups(c.pb);
   for (int i = tid; i < G * GLAMR_NUM_TERMS; i += blockDim.x) {
     const int g = i / GLAMR_NUM_TERMS, k0 = i - g * GLAMR_NUM_TERMS;
-    const double* pg = partial + (size_t)g * per_group * GLAMR_NUM_TERMS;
+    const int first = group_slot(sl, c.pb, g, 0), end = group_slot(sl, c.pb, g, cam3 ? 4 : 3);
+    const double* pg = partial + (size_t)first * GLAMR_NUM_TERMS;
     double s = 0.0;
-    for (int k = 0; k < n_slots; ++k) s += pg[(size_t)k * GLAMR_NUM_TERMS + k0];
+    for (int k = 0; k < end - first; ++k) s += pg[(size_t)k * GLAMR_NUM_TERMS + k0];
     reduce_buf[c.pb.n_params + i] = (float)s;
   }
   if (c.pb.cam_mode == GLAMR_CAM_FIXED) {
     for (int g = 0; g < G; ++g) {
-      const float* gcf = c.sc.g_cam_fix + (size_t)g * c.pb.T * 12;
+      const float* gcf = c.sc.g_cam_fix + group_cam_row0(c.pb, g) * 12;
+      const int T = group_frames(c.pb, g);
       double a[9];
       for (int k = 0; k < 9; ++k) a[k] = 0.0;
-      for (int t = tid; t < c.pb.T; t += blockDim.x)
+      for (int t = tid; t < T; t += blockDim.x)
         for (int k = 0; k < 9; ++k) a[k] += (double)gcf[(size_t)t * 12 + k];
       for (int k = 0; k < 9; ++k) {
         const double s = warp_sum(a[k]);
@@ -268,7 +307,7 @@ __device__ void reduce_tail(const OptCtx& c, const double* partial, int n_slots,
       if (tid < 9) {
         double s = 0.0;
         for (int w = 0; w < (int)(blockDim.x >> 5); ++w) s += sm[w * 16 + tid];
-        const int off = group_theta(c.pb, g) + ((tid < 6) ? c.pb.off_cam_rot + tid : c.pb.off_cam_trans + (tid - 6));
+        const int off = (tid < 6) ? group_off_cam_rot(c.pb, g) + tid : group_off_cam_trans(c.pb, g) + (tid - 6);
         reduce_buf[off] = (float)s;
       }
       __syncthreads();          // sm is rewritten by the next group
@@ -276,9 +315,9 @@ __device__ void reduce_tail(const OptCtx& c, const double* partial, int n_slots,
   }
 }
 
-// blocks [0,P): reverse trajectory codec of one person; blocks [P, P+G*sl.cam): camera backward of 256 frames of one group
+// blocks [0,P): reverse trajectory codec of one person; blocks [P, P+sl.n_cam): camera backward of 256 frames of one group
 // (modes 0-2; mode 3 runs camera_backward/scatter kernels first).  The last CTA to finish folds all partial sums.
-__global__ void __launch_bounds__(kScanThreads, 1) traj_cam_backward_kernel(OptCtx c, int with_cam, double* partial, int n_slots, SlotLayout sl,
+__global__ void __launch_bounds__(kScanThreads, 1) traj_cam_backward_kernel(OptCtx c, int with_cam, double* partial, SlotLayout sl,
                                                                          float* reduce_buf, unsigned int* ticket, PeerCtx pc) {
   __shared__ float sm[kScanThreads / 32 + 1];
   __shared__ double smd[(kScanThreads / 32) * GLAMR_NUM_TERMS];
@@ -288,16 +327,18 @@ __global__ void __launch_bounds__(kScanThreads, 1) traj_cam_backward_kernel(OptC
   acc.clear();
   size_t slot;
   if ((int)blockIdx.x >= c.pb.P) {
-    const int b = blockIdx.x - c.pb.P, g = b / sl.cam, lb = b - g * sl.cam;
+    const int b = blockIdx.x - c.pb.P, G = num_groups(c.pb);
+    const int g = G > 1 ? grid_group(sl, G, &GroupGrid::cam0, b) : 0;
+    const int lb = G > 1 ? b - sl.grid[g].cam0 : b;
     const int t = lb * kScanThreads + threadIdx.x;
-    if (with_cam && t < c.pb.T) camera_backward(c, g * c.pb.T + t, acc);
-    slot = (size_t)g * sl.per_group + sl.res + sl.persons + lb;
+    if (with_cam && t < group_frames(c.pb, g)) camera_backward(c, (int)group_cam_row0(c.pb, g) + t, acc);
+    slot = (size_t)group_slot(sl, c.pb, g, 2) + lb;
   } else {
-    const int p = blockIdx.x, g = p / sl.persons;
-    slot = (size_t)g * sl.per_group + sl.res + (p - g * sl.persons);
+    const int p = blockIdx.x, g = person_group(c.pb, p);
+    slot = (size_t)group_slot(sl, c.pb, g, 1) + (p - group_first_person(c.pb, g));
     const glamr_person_t& ps = c.pb.persons[p];
-    const int len = ps.len, T = c.pb.T;
-    const size_t n0 = (size_t)p * T + ps.start;
+    const int len = ps.len, T = person_frames(c.pb, p);
+    const size_t n0 = person_row(c.pb, p) + ps.start;
     const bool codec = c.pb.traj_source == GLAMR_TRAJ_PREDICTED;     // GLAMR_TRAJ_BASE: no reverse scans
     for (int t = threadIdx.x; t < T; t += kScanThreads) traj_back_pre(c, p, t, acc);
     __syncthreads();
@@ -316,7 +357,7 @@ __global__ void __launch_bounds__(kScanThreads, 1) traj_cam_backward_kernel(OptC
   }
   block_reduce_terms(acc, partial + slot * GLAMR_NUM_TERMS, smd);
   if (grid_last_block(ticket)) {
-    reduce_tail(c, partial, n_slots, sl.per_group, reduce_buf, smd);
+    reduce_tail(c, partial, sl, !with_cam, reduce_buf, smd);
   }
 }
 
@@ -343,12 +384,12 @@ struct AdamState {
   double* beta_pow;   // [0] beta1^t, [1] beta2^t, [2] step count (as a double)
 };
 
-__device__ void write_losses(const OptCtx& c, const float* term_sums /*[NUM_TERMS] un-normalised*/, float* loss_terms) {
+__device__ void write_losses(const OptCtx& c, int g, const float* term_sums /*[NUM_TERMS] un-normalised*/, float* loss_terms) {
   double total = 0.0;
   for (int k = 0; k < GLAMR_NUM_TERMS; ++k) {
     float val = 0.0f;
     if (c.pb.term_enabled[k]) {
-      val = term_sums[k] / c.pb.term_norm[k];
+      val = term_sums[k] / term_norm(c.pb, g, k);
       if (!c.pb.term_monitor[k]) total += (double)val * (double)c.pb.term_weight[k];
     }
     loss_terms[k] = val;
@@ -356,10 +397,10 @@ __device__ void write_losses(const OptCtx& c, const float* term_sums /*[NUM_TERM
   loss_terms[GLAMR_NUM_TERMS] = (float)total;
 }
 
-// thread g: the loss terms of seed group g
+// thread g: the loss terms of group g
 __global__ void __launch_bounds__(32) losses_kernel(OptCtx c, const float* __restrict__ reduce_buf, float* __restrict__ loss_terms) {
   for (int g = threadIdx.x; g < num_groups(c.pb); g += blockDim.x)
-    write_losses(c, reduce_buf + c.pb.n_params + g * GLAMR_NUM_TERMS, loss_terms + g * (GLAMR_NUM_TERMS + 1));
+    write_losses(c, g, reduce_buf + c.pb.n_params + g * GLAMR_NUM_TERMS, loss_terms + g * (GLAMR_NUM_TERMS + 1));
 }
 
 // loss terms (block 0) + torch.optim.Adam step; the last CTA to finish advances the step count / beta powers.
@@ -388,10 +429,10 @@ __global__ void __launch_bounds__(256) apply_kernel(OptCtx c, float* __restrict_
     for (int r = 0; r < pc.world; ++r) g += peer_take(pc, epoch, r, i);
     return g;
   };
-  for (int g = threadIdx.x; blockIdx.x == 0 && g < num_groups(c.pb) && loss_terms; g += blockDim.x) {   // the loss terms of seed group g
+  for (int g = threadIdx.x; blockIdx.x == 0 && g < num_groups(c.pb) && loss_terms; g += blockDim.x) {   // the loss terms of group g
     float sums[GLAMR_NUM_TERMS];
     for (int k = 0; k < GLAMR_NUM_TERMS; ++k) sums[k] = grad_at(c.pb.n_params + g * GLAMR_NUM_TERMS + k);
-    write_losses(c, sums, loss_terms + (hist_stride > 0 ? (size_t)step * hist_stride : 0) + g * (GLAMR_NUM_TERMS + 1));
+    write_losses(c, g, sums, loss_terms + (hist_stride > 0 ? (size_t)step * hist_stride : 0) + g * (GLAMR_NUM_TERMS + 1));
   }
   const float bc2s = (float)sqrt(1.0 - b2);
   const float step_size = (float)(lr / (1.0 - b1));
@@ -425,7 +466,11 @@ struct glamr_opt {
   SmplWorkspace ws;
   AdamState adam;
   double* partial;
-  SlotLayout sl;                                   // partial-sum slots of one seed group; G blocks of sl.per_group
+  SlotLayout sl;                                   // partial-sum slots and CTAs of every group
+  size_t N;                                        // frame-persons of all groups
+  int n_slots;                                     // partial-sum slots of all groups
+  glamr_group_t* shapes;                           // host copy of the group table read at create: the shapes every later problem keeps
+  GroupGrid* grid;                                 // device [G+1] (sl.grid), its own allocation: a scratch reset must not clear it
   unsigned int* tickets;                           // [0] backward tail, [1] apply, [3] peer all-reduce ([2] unused)
   void* arena;
   size_t arena_bytes;
@@ -471,37 +516,73 @@ static OptCtx make_ctx(const glamr_opt* st, const float* theta, float* grad) {
   return c;
 }
 
-// seed groups: P splits into G equal groups; with several groups every frame-person lives on this rank, and theta holds G
-// equal blocks
-static bool groups_valid(const glamr_problem_t* pb) {
+// The groups of a problem on the host: its table (read once from the device), or the one group of a problem without one
+static int host_groups(const glamr_problem_t* pb, std::vector<glamr_group_t>& out) {
   const int G = num_groups(*pb);
-  if (pb->P % G != 0) return false;
-  if (G == 1) return true;
-  return pb->n_begin == 0 && pb->n_end == pb->P * pb->T && pb->owner && pb->group_params > 0 &&
-         (long long)pb->group_params * G == (long long)pb->n_params;
+  out.assign(G, glamr_group_t{});
+  if (has_group_table(*pb)) {
+    if (!pb->groups) return GLAMR_EINVAL;
+    GLAMR_CUDA_TRY(cudaMemcpy(out.data(), pb->groups, sizeof(glamr_group_t) * G, cudaMemcpyDeviceToHost));
+    return GLAMR_OK;
+  }
+  out[0].Q = pb->P;
+  out[0].T = pb->T;
+  return GLAMR_OK;
+}
+
+// groups tile the persons, frame-persons and camera rows in order; with several groups every frame-person lives on this rank
+static bool groups_valid(const glamr_problem_t* pb, const std::vector<glamr_group_t>& gr) {
+  long long p = 0, n = 0, r = 0;
+  for (const glamr_group_t& g : gr) {
+    if (g.p0 != p || g.n0 != n || g.c0 != r || g.Q <= 0 || g.T <= 0 || g.T > pb->T || g.theta0 < 0 || g.theta0 >= pb->n_params) return false;
+    p += g.Q; n += (long long)g.Q * g.T; r += g.T;
+  }
+  if (p != pb->P || n > INT32_MAX) return false;
+  return num_groups(*pb) == 1 || (pb->n_begin == 0 && pb->n_end == n && pb->owner);
 }
 
 extern "C" int glamr_opt_create(glamr_opt_t** out, const glamr_smpl_t* smpl, const glamr_problem_t* pb) {
   if (!out || !smpl || !pb || pb->P <= 0 || pb->T <= 0 || pb->J <= 0 || pb->n_params <= 0) return GLAMR_EINVAL;
   if (pb->J != smpl->dev.n_map) return GLAMR_EINVAL;
   if (pb->traj_source != GLAMR_TRAJ_PREDICTED && pb->traj_source != GLAMR_TRAJ_BASE) return GLAMR_EINVAL;
-  if (!groups_valid(pb)) return GLAMR_EINVAL;
+  std::vector<glamr_group_t> gr;
+  {
+    const int rc = host_groups(pb, gr);
+    if (rc) return rc;
+  }
+  if (!groups_valid(pb, gr)) return GLAMR_EINVAL;
   glamr_opt* st = (glamr_opt*)calloc(1, sizeof(glamr_opt));
   if (!st) return GLAMR_EINVAL;
   st->smpl = smpl->dev;
   st->pb = *pb;
   compute_gs(st);
-  const size_t N = (size_t)pb->P * pb->T, T = pb->T, J = pb->J, G = num_groups(*pb);
-  const size_t GT = G * T;                 // camera rows of all groups
-  st->sl.persons = pb->P / (int)G;
-  st->sl.res = (int)(((size_t)st->sl.persons * T + kFrameThreads / 32 - 1) / (kFrameThreads / 32));
-  st->sl.cam3 = (int)((T + kFrameThreads - 1) / kFrameThreads);
-  st->sl.cam = (int)((T + kScanThreads - 1) / kScanThreads);
-  st->sl.per_group = st->sl.res + st->sl.persons + st->sl.cam + st->sl.cam3;
+  const int G = num_groups(*pb);
+  // each group's CTAs and slots, as its one-group problem has them
+  std::vector<GroupGrid> grid(G + 1);
+  GroupGrid acc{0, 0, 0, 0};
+  size_t N = 0, GT = 0;
+  for (int g = 0; g < G; ++g) {
+    grid[g] = acc;
+    const int res = (gr[g].Q * gr[g].T + kFrameThreads / 32 - 1) / (kFrameThreads / 32);
+    const int cam = (gr[g].T + kScanThreads - 1) / kScanThreads, cam3 = (gr[g].T + kFrameThreads - 1) / kFrameThreads;
+    acc.res0 += res; acc.cam0 += cam; acc.cam30 += cam3; acc.slot0 += res + gr[g].Q + cam + cam3;
+    N += (size_t)gr[g].Q * gr[g].T;
+    GT += gr[g].T;                        // camera rows of all groups
+  }
+  grid[G] = acc;
+  const size_t J = pb->J;
+  st->N = N;
+  st->n_slots = acc.slot0;
+  st->sl.persons = gr[0].Q;
+  st->sl.res = grid[1].res0;
+  st->sl.cam = grid[1].cam0;
+  st->sl.cam3 = grid[1].cam30;
+  st->sl.n_res = acc.res0; st->sl.n_cam = acc.cam0; st->sl.n_cam3 = acc.cam30;
+  st->sl.cam_rows = (int)GT;
   // one arena for all scratch (floats), doubles first for alignment
   size_t floats = 0;
   auto take = [&](size_t nfl) { size_t o = floats; floats += (nfl + 63) & ~(size_t)63; return o; };
-  const size_t o_partial = take(G * st->sl.per_group * GLAMR_NUM_TERMS * 2);
+  const size_t o_partial = take((size_t)st->n_slots * GLAMR_NUM_TERMS * 2);
   const size_t o_beta = take(8);
   const size_t o_ticket = take(4);
   const size_t o_heading = take(N), o_xy = take(2 * N), o_tl = take(11 * N), o_ob = take(3 * N), o_tb = take(3 * N),
@@ -539,7 +620,13 @@ extern "C" int glamr_opt_create(glamr_opt_t** out, const glamr_smpl_t* smpl, con
   st->ws = smpl_carve_workspace(b + o_ws, (int)N, smpl->dev.S);
   const double one[3] = {1.0, 1.0, 0.0};
   e = cudaMemcpy(st->adam.beta_pow, one, sizeof(one), cudaMemcpyHostToDevice);
-  if (e != cudaSuccess) { cudaFree(st->arena); free(st); return (int)e; }
+  if (e == cudaSuccess) e = cudaMalloc(&st->grid, sizeof(GroupGrid) * (G + 1));
+  if (e == cudaSuccess) e = cudaMemcpy(st->grid, grid.data(), sizeof(GroupGrid) * (G + 1), cudaMemcpyHostToDevice);
+  st->shapes = (glamr_group_t*)malloc(sizeof(glamr_group_t) * G);
+  if (e == cudaSuccess && !st->shapes) e = cudaErrorMemoryAllocation;
+  if (e != cudaSuccess) { cudaFree(st->grid); cudaFree(st->arena); free(st->shapes); free(st); return (int)e; }
+  memcpy(st->shapes, gr.data(), sizeof(glamr_group_t) * G);
+  st->sl.grid = st->grid;
   *out = st;
   return GLAMR_OK;
 }
@@ -643,6 +730,8 @@ extern "C" int glamr_opt_destroy(glamr_opt_t* st) {
     cudaEventDestroy(st->ev_fork); cudaEventDestroy(st->ev_join); cudaEventDestroy(st->ev_sup);
   }
   cudaFree(st->arena);
+  cudaFree(st->grid);
+  free(st->shapes);
   free(st);
   return GLAMR_OK;
 }
@@ -652,7 +741,19 @@ static int join_pending(glamr_opt_t* st, cudaStream_t s);
 extern "C" int glamr_opt_set_problem(glamr_opt_t* st, const glamr_problem_t* pb, int reset_adam, void* stream) {
   if (!st || !pb) return GLAMR_EINVAL;
   if (pb->P != st->pb.P || pb->T != st->pb.T || pb->J != st->pb.J || pb->n_params != st->pb.n_params) return GLAMR_EINVAL;
-  if (num_groups(*pb) != num_groups(st->pb) || !groups_valid(pb)) return GLAMR_EINVAL;
+  // a later problem has the group shapes read at create (the CTAs, slots and scratch are laid out for them); its table may carry
+  // other theta bases, camera offsets and normalisers.  One small device->host copy per call checks it.
+  if (num_groups(*pb) != num_groups(st->pb)) return GLAMR_EINVAL;
+  if (num_groups(*pb) > 1) {
+    std::vector<glamr_group_t> gr;
+    const int rc = host_groups(pb, gr);
+    if (rc) return rc;
+    if (!groups_valid(pb, gr)) return GLAMR_EINVAL;
+    for (int g = 0; g < num_groups(*pb); ++g) {
+      const glamr_group_t &a = gr[g], &b = st->shapes[g];
+      if (a.p0 != b.p0 || a.Q != b.Q || a.n0 != b.n0 || a.c0 != b.c0 || a.T != b.T) return GLAMR_EINVAL;
+    }
+  }
   if (pb->traj_source != GLAMR_TRAJ_PREDICTED && pb->traj_source != GLAMR_TRAJ_BASE) return GLAMR_EINVAL;
   {
     const int rc = join_pending(st, (cudaStream_t)stream);
@@ -792,12 +893,11 @@ static int backward_impl(glamr_opt_t* st, const float* theta, float* reduce_buf,
     }
   }
   const SlotLayout sl = st->sl;
-  const int G = num_groups(pb);
-  const int cam_rows_ctas = (G * pb.T + kFrameThreads - 1) / kFrameThreads;      // one thread per camera row of every group
-  GLAMR_CUDA_TRY(launch_pdl(1, traj_cam_forward_kernel, dim3(pb.P + G * sl.cam), dim3(kScanThreads), 0, s, c, from_persons ? 0 : 1, sl.cam));   // also zeroes reduce_buf
+  const int cam_rows_ctas = (sl.cam_rows + kFrameThreads - 1) / kFrameThreads;      // one thread per camera row of every group
+  GLAMR_CUDA_TRY(launch_pdl(1, traj_cam_forward_kernel, dim3(pb.P + sl.n_cam), dim3(kScanThreads), 0, s, c, from_persons ? 0 : 1, sl));   // also zeroes reduce_buf
   GLAMR_MARK();
   if (from_persons) {          // the camera is the mean of the persons' world transforms: needs traj_forward of all persons
-    GLAMR_CUDA_TRY(launch_pdl(1, cam_forward_kernel, dim3(cam_rows_ctas), dim3(kFrameThreads), 0, s, c));
+    GLAMR_CUDA_TRY(launch_pdl(1, cam_forward_kernel, dim3(cam_rows_ctas), dim3(kFrameThreads), 0, s, c, sl.cam_rows));
   }
   GLAMR_MARK();
   if (n_end > n_begin) {
@@ -839,17 +939,16 @@ static int backward_impl(glamr_opt_t* st, const float* theta, float* reduce_buf,
     GLAMR_MARK();
   }
   if (!(exp_skip & 4))
-    GLAMR_CUDA_TRY(launch_pdl(8, frame_residuals_kernel, dim3(G * sl.res), dim3(kFrameThreads), 0, s, c, st->smpl, wo, n_begin, st->partial, sl));
+    GLAMR_CUDA_TRY(launch_pdl(8, frame_residuals_kernel, dim3(sl.n_res), dim3(kFrameThreads), 0, s, c, st->smpl, wo, n_begin, st->partial, sl));
   GLAMR_MARK();
   if (from_persons) {
-    GLAMR_CUDA_TRY(launch_pdl(16, camera_backward_kernel, dim3(G * sl.cam3), dim3(kFrameThreads), 0, s, c, st->partial, sl));
-    GLAMR_CUDA_TRY(launch_pdl(16, camera_scatter_kernel, dim3(cam_rows_ctas), dim3(kFrameThreads), 0, s, c));
+    GLAMR_CUDA_TRY(launch_pdl(16, camera_backward_kernel, dim3(sl.n_cam3), dim3(kFrameThreads), 0, s, c, st->partial, sl));
+    GLAMR_CUDA_TRY(launch_pdl(16, camera_scatter_kernel, dim3(cam_rows_ctas), dim3(kFrameThreads), 0, s, c, sl.cam_rows));
     GLAMR_MARK();
   }
-  const int n_slots = sl.res + sl.persons + sl.cam + (from_persons ? sl.cam3 : 0);      // slots of each group that hold partial sums
   if (!(exp_skip & 8))
-    GLAMR_CUDA_TRY(launch_pdl(16, traj_cam_backward_kernel, dim3(pb.P + G * sl.cam), dim3(kScanThreads), 0, s, c, from_persons ? 0 : 1, st->partial,
-                              n_slots, sl, reduce_buf, st->tickets, pc));
+    GLAMR_CUDA_TRY(launch_pdl(16, traj_cam_backward_kernel, dim3(pb.P + sl.n_cam), dim3(kScanThreads), 0, s, c, from_persons ? 0 : 1, st->partial,
+                              sl, reduce_buf, st->tickets, pc));
   GLAMR_MARK();
   if (forked) {
     if (defer_join) st->join_pending = 1;
@@ -999,7 +1098,7 @@ extern "C" int glamr_opt_iterate(glamr_opt_t* st, float* theta, float* reduce_bu
 
 extern "C" int glamr_opt_read(glamr_opt_t* st, int what, const float** ptr, size_t* count) {
   if (!st || !ptr || !count) return GLAMR_EINVAL;
-  const size_t N = (size_t)st->pb.P * st->pb.T, T = (size_t)num_groups(st->pb) * st->pb.T, J = st->pb.J;   // T: camera rows of all groups
+  const size_t N = st->N, T = (size_t)st->sl.cam_rows, J = st->pb.J;   // T: camera rows of all groups
   switch (what) {
     case GLAMR_R_ORIENT_WORLD: *ptr = st->sc.orient_world; *count = 3 * N; break;
     case GLAMR_R_TRANS_WORLD: *ptr = st->sc.trans_world; *count = 3 * N; break;

@@ -13,6 +13,11 @@ r, r + world, ... on its own GPU; there is no collective on the data path.
 ``optimize`` call per seed: same files, same contents; each seed's recorded time is the call's time divided by the number of
 seeds it ran.
 
+``--batch_sequences K`` optimises a rank's sequences K at a time as the groups of one ``optimize_batch`` call: all remaining
+seeds of those sequences with ``--batch_seeds``, one seed per call otherwise.  Same files, same contents; each (sequence, seed)
+pair's recorded time is the call's time divided by the number of pairs it ran.  The GPU scratch grows with the frame-persons of
+the call (sum of persons x frames over its pairs): about 350 MB at 4,000 frame-persons, mostly the SMPL vertices.
+
     python -m glamr_b200.global_recon.run_dataset --cfg glamr_3dpw --synthetic 32 --frames 300 --out_dir out/sweep
     python -m torch.distributed.run --nproc-per-node 8 --master-addr 127.0.0.1 -m glamr_b200.global_recon.run_dataset ...
 """
@@ -107,6 +112,8 @@ def run(args, make_model=None, make_in_dict=None):
         gt_file = os.path.join(args.gt_pose_root, f'{seq_name}.pkl') if args.gt_pose_root else None
         return load_in_dict(find_pose_file(args.pose_root, seq_name), seq_name, gt_file)
 
+    if args.batch_sequences > 0:
+        return done + _run_batches(args, model, mine, seeds, load, rank)
     for i, seq_name in enumerate(mine):
         if args.batch_seeds:
             todo = []
@@ -155,6 +162,53 @@ def run(args, make_model=None, make_in_dict=None):
     return done
 
 
+def _run_batches(args, model, mine, seeds, load, rank):
+    """--batch_sequences: the rank's sequences K at a time, every remaining (sequence, seed) pair of a chunk in optimize_batch calls"""
+    done = []
+    K = args.batch_sequences
+    for c0 in range(0, len(mine), K):
+        chunk = mine[c0:c0 + K]
+        todo = {}                                            # sequence -> seeds whose file is still missing
+        for seq_name in chunk:
+            for seed in seeds:
+                out_file = out_file_of(args.out_dir, seq_name, seed)
+                if args.cached and os.path.exists(out_file):
+                    done.append((seq_name, seed, out_file, 0.0))
+                else:
+                    todo.setdefault(seq_name, []).append(seed)
+        calls = []                                           # (sequences, seeds) of one optimize_batch call each
+        if args.batch_seeds:
+            by_seeds = {}
+            for seq_name, ss in todo.items():
+                by_seeds.setdefault(tuple(ss), []).append(seq_name)
+            calls = [(seqs, list(ss)) for ss, seqs in by_seeds.items()]
+        else:
+            for seed in seeds:
+                seqs = [q for q, ss in todo.items() if seed in ss]
+                if seqs:
+                    calls.append((seqs, [seed]))
+        in_dicts = {}
+        for seqs, ss in calls:
+            for q in seqs:
+                if q not in in_dicts:
+                    in_dicts[q] = load(q)
+            dicts = [in_dicts[q] for q in seqs]
+            t0 = time.perf_counter()
+            outs = model.optimize_batch(dicts, ss)           # sets the RNGs of every pair itself
+            n = len(seqs) * len(ss)
+            dt = (time.perf_counter() - t0) / n
+            for seq_name, row in zip(seqs, outs):
+                for seed, out_dict in zip(ss, row):
+                    out_file = out_file_of(args.out_dir, seq_name, seed)
+                    os.makedirs(os.path.dirname(out_file), exist_ok=True)
+                    with open(out_file, 'wb') as f:
+                        pickle.dump(out_dict, f)
+                    done.append((seq_name, seed, out_file, dt))
+                    if not args.quiet:
+                        print(f'[rank {rank}] seed {seed} {seq_name}: {dt * 1e3:.1f} ms (batch of {n}) -> {out_file}', flush=True)
+    return done
+
+
 def parse(argv=None):
     ap = argparse.ArgumentParser(description=__doc__, formatter_class=argparse.RawDescriptionHelpFormatter)
     ap.add_argument('--cfg', default='glamr_3dpw')
@@ -171,6 +225,8 @@ def parse(argv=None):
     ap.add_argument('--gaps', action='store_true', help='synthetic sequences with occlusion gaps')
     ap.add_argument('--real_assets', action='store_true', help='with --synthetic: still load SMPL files / checkpoints from disk')
     ap.add_argument('--batch_seeds', action='store_true', help='optimise all seeds of a sequence in one optimize_seeds call')
+    ap.add_argument('--batch_sequences', type=int, default=0,
+                    help='optimise K sequences of this rank at a time in one optimize_batch call (0: one sequence at a time)')
     ap.add_argument('--quiet', action='store_true')
     return ap.parse_args(argv)
 

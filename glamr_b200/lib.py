@@ -52,6 +52,11 @@ class Person(ctypes.Structure):
                  'world_dxy_base']]
 
 
+class Group(ctypes.Structure):
+    _fields_ = [(n, ctypes.c_int32) for n in ['p0', 'Q', 'n0', 'c0', 'T', 'theta0', 'off_cam_rot', 'off_cam_trans', 'rel0']] + \
+               [('term_norm', ctypes.c_float * NUM_TERMS), ('gs', ctypes.c_float * NUM_TERMS)]
+
+
 class Problem(ctypes.Structure):
     _fields_ = [(n, ctypes.c_int32) for n in
                 ['P', 'T', 'J', 'cam_mode', 'off_cam_rot', 'off_cam_trans', 'use_world_res', 'has_world_dheading',
@@ -61,7 +66,7 @@ class Problem(ctypes.Structure):
                 ('term_weight', ctypes.c_float * NUM_TERMS), ('term_norm', ctypes.c_float * NUM_TERMS),
                 ('term_enabled', ctypes.c_int32 * NUM_TERMS), ('term_monitor', ctypes.c_int32 * NUM_TERMS)] + \
                [(n, _vp) for n in
-                ['persons', 'smpl_pose_all', 'smpl_beta_all', 'scale_all', 'cam_pose_const', 'empty_index', 'fill_src',
+                ['persons', 'groups', 'smpl_pose_all', 'smpl_beta_all', 'scale_all', 'cam_pose_const', 'empty_index', 'fill_src',
                  'inv_num_persons', 'rel_target', 'rel_w', 'rel_wt', 'active']]
 
 

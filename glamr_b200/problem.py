@@ -7,10 +7,15 @@
 * ``StageCompiler`` turns ``loss_cfg`` (global_recon/models/loss_func.py semantics: min_conf, first_frame_only,
   first_frame_weight, visibility masks, normalisers) into per-frame weight arrays and scalar term tables.
 
-Seed groups: ``make_layout`` / ``bind_variables`` / ``begin_stage_variables`` / ``StageCompiler`` also take a list of G data
-dicts, the seeds of one sequence (same persons, frames, visibility and loss normalisers, each with its own initial state).  theta
-then holds group 0's blocks, group 1's, and so on; the G*Q persons are simply more persons, each with its group index
-(include/glamr_b200.h, glamr_problem_t.G).  One dict is one group, with exactly the layout it always had.
+Groups: ``make_layout`` / ``bind_variables`` / ``begin_stage_variables`` / ``StageCompiler`` also take
+* a list of G data dicts, the seeds of one sequence (same persons, frames, visibility and loss normalisers, each with its own
+  initial state), or
+* a list of such lists, ``[[seq0 seed dicts], [seq1 seed dicts], ...]``: a batch of sequences that share one config and may differ
+  in frames, persons, exist ranges, frames without persons and visibility.  Each group is compiled from its own data alone,
+  normalisers included.
+theta then holds group 0's blocks, group 1's, and so on; the persons of all groups are simply more persons, each with its group
+index, and StageCompiler uploads one row per group of include/glamr_b200.h's glamr_group_t.  One dict is one group, with exactly the
+layout it always had.
 
 Pure tensor bookkeeping, device agnostic (tests build it on the CPU for the host harness); nothing here computes
 on the optimisation path.
@@ -56,6 +61,16 @@ class VariableLayout:
         self.lens = self.lens * self.G
         self.n_params = self.G * off
 
+    def group_layout(self, g):
+        """(one-group layout, first float of its block in theta) of group g"""
+        if self.G == 1:
+            return self, 0
+        return (VariableLayout(self.T, self.n_empty, self.trans_res_rows, self.lens[:self.Q], heading_dim=self.heading_dim,
+                               world_dxy=self.world_dxy, person2cam=self.person2cam), g * self.group_params)
+
+    def group_persons(self, g):
+        return range(g * self.Q, (g + 1) * self.Q)
+
     def views(self, theta, p=None, group=0):
         """name -> view of theta with the reference's tensor shape: the camera variables of `group` (p None), else those of
         person p (counted over all groups)"""
@@ -83,12 +98,55 @@ class VariableLayout:
         return out
 
 
+class BatchLayout:
+    """Groups of a batch of sequences: theta is the concatenation of one one-group VariableLayout per group, each at its own base
+    (``bases``).  ``persons`` / ``lens`` list the persons of all groups, group by group, with offsets into the whole theta."""
+
+    def __init__(self, lays):
+        self.layouts = list(lays)
+        self.G = len(self.layouts)
+        self.bases, self.p0s, off, p = [], [], 0, 0
+        for lay in self.layouts:
+            self.bases.append(off)
+            self.p0s.append(p)
+            off += lay.n_params
+            p += lay.Q
+        self.n_params = off
+        self.persons = [{k: o + b for k, o in d.items()} for lay, b in zip(self.layouts, self.bases) for d in lay.persons]
+        self.lens = [n for lay in self.layouts for n in lay.lens]
+        self.person_group = [g for g, lay in enumerate(self.layouts) for _ in range(lay.Q)]
+        l0 = self.layouts[0]
+        self.heading_dim, self.world_dxy, self.person2cam = l0.heading_dim, l0.world_dxy, l0.person2cam
+        self.T = max(lay.T for lay in self.layouts)              # the longest group's frames (glamr_problem_t.T)
+
+    def group_layout(self, g):
+        return self.layouts[g], self.bases[g]
+
+    def group_persons(self, g):
+        return range(self.p0s[g], self.p0s[g] + self.layouts[g].Q)
+
+    def views(self, theta, p=None, group=0):
+        """as VariableLayout.views: the camera variables of `group` (p None), else those of person p (counted over all groups)"""
+        if p is not None:
+            group = self.person_group[p]
+        lay, b = self.group_layout(group)
+        sub = theta[b:b + lay.n_params]
+        return lay.views(sub) if p is None else lay.views(sub, p - self.p0s[group])
+
+
 def _f32(x, device):
     return torch.as_tensor(x).to(device=device, dtype=torch.float32).contiguous()
 
 
+def _is_batch(data):
+    """a list of per-sequence lists of seed dicts (a batch of sequences)"""
+    return isinstance(data, (list, tuple)) and len(data) > 0 and isinstance(data[0], (list, tuple))
+
+
 def _groups(data):
-    """one data dict, or the list of the seed groups' data dicts -> list"""
+    """one data dict, the list of the seed groups' data dicts, or a batch's list of such lists -> flat list of group dicts"""
+    if _is_batch(data):
+        return [d for seq in data for d in seq]
     return list(data) if isinstance(data, (list, tuple)) else [data]
 
 
@@ -96,22 +154,35 @@ class StageCompiler:
     """Holds the per-person constant tensors and builds a ``Problem`` for every stage."""
 
     def __init__(self, data, layout, flags, device, aa_to_rot6d, num_joints=26, aa_to_quat=None):
-        """data: one data dict, or the list of the seed groups' data dicts (see the module docstring).
+        """data: one data dict, the list of the seed groups' data dicts, or a batch of sequences (see the module docstring).
         flags: dict with flag_fixed_cam, flag_opt_cam, flag_opt_cam_from_person_pose, flag_cam_inv_trans_res_all,
         flag_opt_vis_local_rot, cam_fix_frames and optionally flag_opt_traj / traj_source (when absent they are read off
         `data`: a predicted trajectory leaves traj_local_pred, flag_opt_traj leaves the world_res variables), heading_vec
         (heading_type 'vec'; default: the layout's heading size) and flag_opt_person2cam_rot / _trans (default false).
         aa_to_rot6d: callable (device math lives in the CUDA library)."""
+        self.batch = _is_batch(data) and len(data) > 1       # one sequence in a batch: its seed groups
         self.datas = _groups(data)
         data = self.datas[0]
         self.data, self.layout, self.flags, self.device, self.J = data, layout, flags, device, num_joints
         self.pids = list(data['person_data'].keys())
-        self.G, self.Q, self.T = len(self.datas), len(self.pids), data['seq_len']
-        self.P = self.G * self.Q                     # persons of all groups, group by group
-        T, dev = self.T, device
-        persons = [d for dd in self.datas for d in dd['person_data'].values()]
-        if any(len(dd['person_data']) != self.Q or dd['seq_len'] != T for dd in self.datas):
+        self.Qs = [len(dd['person_data']) for dd in self.datas]
+        self.Ts = [int(dd['seq_len']) for dd in self.datas]
+        if not self.batch and any(q != self.Qs[0] or t != self.Ts[0] for q, t in zip(self.Qs, self.Ts)):
             raise ValueError('seed groups need the same persons and frame count')
+        self.G, self.P, self.T = len(self.datas), sum(self.Qs), max(self.Ts)   # T: every group's frames when they agree
+        self.Q = self.Qs[0] if len(set(self.Qs)) == 1 else None                 # persons per group when they agree
+        # first person / frame-person / camera row of each group, and the group and frames of each person
+        self.p0s, self.n0s, self.c0s, p, n, r = [], [], [], 0, 0, 0
+        for q, t in zip(self.Qs, self.Ts):
+            self.p0s.append(p)
+            self.n0s.append(n)
+            self.c0s.append(r)
+            p, n, r = p + q, n + q * t, r + t
+        self.N = n                                   # frame-persons of all groups
+        self.person_group = [g for g, q in enumerate(self.Qs) for _ in range(q)]
+        self.person_T = [self.Ts[g] for g in self.person_group]
+        dev = device
+        persons = [d for dd in self.datas for d in dd['person_data'].values()]
         self.persons = persons
         self.traj_source = flags.get('traj_source', L.TRAJ_PREDICTED if all('traj_local_pred' in d for d in persons) else L.TRAJ_BASE)
         self.opt_traj = flags.get('flag_opt_traj', all('smpl_orient_world_res' in d for d in persons))
@@ -131,12 +202,12 @@ class StageCompiler:
                 'traj_local_pred': _f32(d['traj_local_pred'] if 'traj_local_pred' in d else torch.zeros(Ln, 11), dev),
                 'orient_base_init': _f32(d['smpl_orient_world_base'], dev).clone(),
                 'trans_base_init': _f32(d['root_trans_world_base'], dev).clone(),
-                'cam_K': _f32(d['cam_K'], dev).reshape(T, 9),
+                'cam_K': _f32(d['cam_K'], dev).reshape(-1, 9),
                 'kp_target': _f32(d['kp_2d_aligned'], dev),
                 'orient_cam_6d': _f32(aa_to_rot6d(_f32(d['smpl_orient_cam'], dev)), dev),
                 'orient_cam_q': None if aa_to_quat is None else _f32(aa_to_quat(_f32(d['smpl_orient_cam'], dev)), dev),
                 'trans_cam': _f32(d['root_trans_cam'], dev),
-                'person2cam': _f32(d['person2cam'], dev)[:, :3, :].reshape(T, 12).contiguous(),
+                'person2cam': _f32(d['person2cam'], dev)[:, :3, :].reshape(-1, 12).contiguous(),
                 'dheading_mask': _f32(mask, dev),
                 'rot_mask': _f32(d['vis_frames'][start:start + Ln], dev) if flags.get('flag_opt_vis_local_rot', False) else None,
                 'vis': _f32(d['vis_frames'], dev),
@@ -147,20 +218,22 @@ class StageCompiler:
             pose_all.append(_f32(d['smpl_pose'], dev))
             beta_all.append(_f32(d['smpl_beta'], dev))
             scale_all.append(None if d['scale'] is None else _f32(d['scale'], dev))
-        self.pose_all = torch.stack(pose_all).contiguous()
-        self.beta_all = torch.stack(beta_all).contiguous()
-        self.scale_all = None if scale_all[0] is None else torch.stack(scale_all).contiguous()
+        # [P,T,...] when every group has T frames, else the [N,...] rows of all persons (the same memory order)
+        cat = torch.stack if len(set(self.Ts)) == 1 else torch.cat
+        self.pose_all = cat(pose_all).contiguous()
+        self.beta_all = cat(beta_all).contiguous()
+        self.scale_all = None if scale_all[0] is None else cat(scale_all).contiguous()
         # host copies of what the per-stage weight tables are built from (visibility, keypoint scores, persons per frame):
         # ONE device->host copy here instead of several per person and stage
-        P_, J_, G_, Q_ = self.P, self.J, self.G, self.Q
-        packed = torch.cat([torch.stack([torch.as_tensor(d['vis_frames']).to(dev).double() for d in persons]).reshape(-1),
-                            torch.stack([torch.as_tensor(d['kp_2d_score']).to(dev).double() for d in persons]).reshape(-1),
-                            torch.stack([torch.as_tensor(dd['fr_num_persons']).to(dev).double().reshape(-1) for dd in self.datas]).reshape(-1)]).cpu()
-        self.host_vis = packed[:P_ * T].reshape(P_, T) > 0.5
-        self.host_score = packed[P_ * T:P_ * T + P_ * T * J_].reshape(P_, T, J_)
+        J_, N_ = self.J, self.N
+        packed = torch.cat([torch.cat([torch.as_tensor(d['vis_frames']).to(dev).double().reshape(-1) for d in persons]),
+                            torch.cat([torch.as_tensor(d['kp_2d_score']).to(dev).double().reshape(-1) for d in persons]),
+                            torch.cat([torch.as_tensor(dd['fr_num_persons']).to(dev).double().reshape(-1) for dd in self.datas])]).cpu()
+        self.host_vis = [v > 0.5 for v in packed[:N_].split(self.person_T)]                       # per person [T]
+        self.host_score = [v.reshape(-1, J_) for v in packed[N_:N_ + N_ * J_].split([t * J_ for t in self.person_T])]   # [T, J]
         # camera-from-persons bookkeeping (global_recon_model.py:489-506), one [T] block per group
         src, empty_idx, inv_num = [], [], []
-        for npers in packed[P_ * T + P_ * T * J_:].to(torch.int64).reshape(G_, T):
+        for npers, T in zip(packed[N_ + N_ * J_:].to(torch.int64).split(self.Ts), self.Ts):
             has = npers > 0
             last, ne = int(torch.where(has)[0][0]), 0
             for t in range(T):
@@ -175,19 +248,25 @@ class StageCompiler:
         self.fill_src = torch.tensor(src, dtype=torch.int32, device=dev)
         self.empty_index = torch.tensor(empty_idx, dtype=torch.int32, device=dev)
         self.inv_num = _f32(torch.cat(inv_num), dev)
-        # rel_transform targets: pairs (i, j) inside each group, one [Q*Q] block per group
-        if data.get('rel_transform_cam'):
-            tgt = torch.zeros(G_ * Q_ * Q_, T, 12, device=dev)
+        # rel_transform targets: pairs (i, j) inside each group, one [Q*Q, T] block per group starting at (pair, frame) entry rel0
+        self.rel0, n_rel = [], 0
+        for q, t in zip(self.Qs, self.Ts):
+            self.rel0.append(n_rel)
+            n_rel += q * q * t
+        if any(dd.get('rel_transform_cam') for dd in self.datas):
+            tgt = torch.zeros(n_rel, 12, device=dev)
             for g, dd in enumerate(self.datas):
-                for (i, j), C in dd['rel_transform_cam'].items():
-                    tgt[(g * Q_ + i) * Q_ + j] = torch.as_tensor(C).detach().to(dev).float()[:, :3, :].reshape(T, 12)
+                Q_, T = self.Qs[g], self.Ts[g]
+                for (i, j), C in (dd.get('rel_transform_cam') or {}).items():
+                    r = self.rel0[g] + (i * Q_ + j) * T
+                    tgt[r:r + T] = torch.as_tensor(C).detach().to(dev).float()[:, :3, :].reshape(T, 12)
             self.rel_target = tgt.contiguous()
         else:
             self.rel_target = None
 
     # ------------------------------------------------------------------------------------------------ per stage
     def _person_weights(self, p, loss_cfg):
-        T, J = self.T, self.J
+        T, J = self.person_T[p], self.J
         vis, score = self.host_vis[p], self.host_score[p]
         vis_idx = torch.where(vis)[0]
         nvis = int(vis.sum())
@@ -233,8 +312,8 @@ class StageCompiler:
 
     def compile(self, theta, opt_variables, loss_cfg, stage, n_begin=0, n_end=None, owner=True):
         data, lay, fl, dev, P, T, J = self.data, self.layout, self.flags, self.device, self.P, self.T, self.J
-        G, Q, persons_all = self.G, self.Q, self.persons
-        n_end = P * T if n_end is None else n_end
+        G, persons_all = self.G, self.persons
+        n_end = self.N if n_end is None else n_end
         if 'person2cam_res_trans_reg' in loss_cfg:           # loss_func.py:244-245
             raise ValueError("residual 'person2cam_res_trans_reg' reads data['person2cam_res_trans'], a key the reference never creates "
                              "(the residuals live per person), so the reference fails with KeyError; it has no defined meaning to implement")
@@ -243,7 +322,7 @@ class StageCompiler:
                 raise NotImplementedError(f"residual '{name}' has no CUDA implementation (no CPU fallback)")
         pb = L.Problem()
         pb.P, pb.T, pb.J, pb.n_params = P, T, J, lay.n_params
-        pb.G, pb.group_params = G, lay.group_params
+        pb.G, pb.group_params = G, getattr(lay, 'group_params', 0)          # a batch describes its groups in the table below
         pb.n_begin, pb.n_end, pb.owner = n_begin, n_end, int(owner)
         keep = []
         # ---- camera mode (global_recon_model.py:473-508)
@@ -254,13 +333,15 @@ class StageCompiler:
             elif fl['flag_opt_cam_from_person_pose']:
                 mode = L.CAM_FROM_PERSONS
         pb.cam_mode = mode
-        if mode == L.CAM_FIXED:
-            pb.off_cam_rot, pb.off_cam_trans = lay.cam_rot_fix, lay.cam_trans_fix
-        elif mode == L.CAM_PER_FRAME:
-            pb.off_cam_rot, pb.off_cam_trans = lay.cam_rot, lay.cam_trans
-        else:
-            pb.off_cam_rot, pb.off_cam_trans = lay.cam_inv_rot_res, lay.cam_inv_trans_res
-        cam_const = torch.cat([_f32(dd['cam_pose'], dev)[:, :3, :].reshape(T, 12) for dd in self.datas]).contiguous().clone()
+
+        def cam_offsets(lg):
+            if mode == L.CAM_FIXED:
+                return lg.cam_rot_fix, lg.cam_trans_fix
+            if mode == L.CAM_PER_FRAME:
+                return lg.cam_rot, lg.cam_trans
+            return lg.cam_inv_rot_res, lg.cam_inv_trans_res
+        pb.off_cam_rot, pb.off_cam_trans = cam_offsets(lay.group_layout(0)[0])
+        cam_const = torch.cat([_f32(dd['cam_pose'], dev)[:, :3, :].reshape(-1, 12) for dd in self.datas]).contiguous().clone()
         keep.append(cam_const)
         pb.cam_pose_const = cam_const.data_ptr()
         pb.trans_res_all = int(fl['flag_cam_inv_trans_res_all'])
@@ -309,22 +390,25 @@ class StageCompiler:
         pb.scale_all = None if self.scale_all is None else self.scale_all.data_ptr()
         # ---- persons
         persons = (L.Person * P)()
-        group_norms = [{} for _ in range(G)]                 # normalisers of each group's persons: the groups must agree
-        host_w = torch.zeros(P, 2 * T * J + 2 * T, dtype=torch.float32)        # [kp_w | kp_dist_mask | ctr_w | ctt_w] per person
+        # normalisers of each group's persons: seed groups of one sequence must agree, the groups of a batch have their own
+        group_norms = [{} for _ in range(G)]
+        host_w, w_off, o = [], [], 0            # [kp_w | kp_dist_mask | ctr_w | ctt_w] per person, persons one after another
         for p in range(P):
             kp_w, kp_dm, ctr_w, ctt_w, nrm = self._person_weights(p, loss_cfg)
-            host_w[p] = torch.cat([kp_w.reshape(-1), kp_dm.reshape(-1), ctr_w, ctt_w]).float()
+            host_w.append(torch.cat([kp_w.reshape(-1), kp_dm.reshape(-1), ctr_w, ctt_w]).float())
+            w_off.append(o)
+            o += host_w[-1].numel()
+            gn = group_norms[self.person_group[p]]
             for k, v in nrm.items():
-                group_norms[p // Q][k] = group_norms[p // Q].get(k, 0) + v
-        if any(n != group_norms[0] for n in group_norms[1:]):
+                gn[k] = gn.get(k, 0) + v
+        if not self.batch and any(n != group_norms[0] for n in group_norms[1:]):
             raise ValueError('seed groups need the same loss normalisers (visibility and keypoint scores of one sequence)')
-        norms = group_norms[0]
-        dev_w = host_w.to(dev)                                                   # one upload for all persons
+        dev_w = torch.cat(host_w).to(dev)                                        # one upload for all persons
         keep.append(dev_w)
         for p in range(P):
             c, o = self.const[p], lay.persons[p]
             ps = persons[p]
-            ps.start, ps.len, ps.group = c['start'], c['len'], p // Q
+            ps.start, ps.len, ps.group = c['start'], c['len'], self.person_group[p]
             ps.off_xy, ps.off_heading, ps.off_dxy, ps.off_dheading = o['xy'], o['heading'], o['dxy'], o['dheading']
             ps.off_z, ps.off_rot, ps.off_world_dheading = o['z'], o['rot'], o['world_dheading']
             ps.off_orient_res, ps.off_trans_res, ps.off_world_dxy = o['orient_res'], o['trans_res'], o['world_dxy']
@@ -332,9 +416,9 @@ class StageCompiler:
             for name in ['traj_local_pred', 'orient_base_init', 'trans_base_init', 'cam_K', 'kp_target', 'orient_cam_6d',
                          'orient_cam_q', 'trans_cam', 'person2cam', 'dheading_mask', 'rot_mask', 'vis', 'world_dxy_base']:
                 setattr(ps, name, None if c[name] is None else c[name].data_ptr())
-            base = dev_w.data_ptr() + p * dev_w.shape[1] * 4
-            ps.kp_w, ps.kp_dist_mask = base, base + T * J * 4
-            ps.ctr_w, ps.ctt_w = base + 2 * T * J * 4, base + (2 * T * J + T) * 4
+            base, Tp = dev_w.data_ptr() + w_off[p] * 4, self.person_T[p]
+            ps.kp_w, ps.kp_dist_mask = base, base + Tp * J * 4
+            ps.ctr_w, ps.ctt_w = base + 2 * Tp * J * 4, base + (2 * Tp * J + Tp) * 4
         persons_dev = torch.frombuffer(bytearray(bytes(persons)), dtype=torch.uint8).to(dev)
         keep.append(persons_dev)
         pb.persons = persons_dev.data_ptr()
@@ -342,39 +426,45 @@ class StageCompiler:
         if self.rel_target is not None and 'rel_transform' in loss_cfg:
             sp = loss_cfg['rel_transform']
             ffw = sp.get('first_frame_weight', 10)
-            rw, rwt = torch.zeros(G * Q * Q, T), torch.zeros(G * Q * Q, T)
-            n_rel = T * len(data['rel_transform_cam'])
+            rw, rwt = torch.zeros(self.rel_target.shape[0]), torch.zeros(self.rel_target.shape[0])
             for g, dd in enumerate(self.datas):
-                for (i, j) in dd['rel_transform_cam'].keys():
-                    both = self.host_vis[g * Q + i] & self.host_vis[g * Q + j]
+                Q, Tg, p0 = self.Qs[g], self.Ts[g], self.p0s[g]
+                pairs = dd.get('rel_transform_cam') or {}
+                for (i, j) in pairs.keys():
+                    both = self.host_vis[p0 + i] & self.host_vis[p0 + j]
                     if both.sum() == 0:
                         continue
                     f0 = int(torch.where(both)[0][0])
                     wv = both.float()
                     wv[f0] = float(ffw) ** 2
-                    rw[(g * Q + i) * Q + j] = wv
+                    r = self.rel0[g] + (i * Q + j) * Tg
+                    rw[r:r + Tg] = wv
                     wt = wv.clone()
                     if sp.get('first_frame_trans_only', False):
                         wt[:] = 0
                         wt[f0] = float(ffw) ** 2
-                    rwt[(g * Q + i) * Q + j] = wt
+                    rwt[r:r + Tg] = wt
+                group_norms[g]['rel_transform'] = Tg * len(pairs)
             rw, rwt = rw.to(dev).contiguous(), rwt.to(dev).contiguous()
             keep += [rw, rwt]
             pb.rel_target, pb.rel_w, pb.rel_wt = self.rel_target.data_ptr(), rw.data_ptr(), rwt.data_ptr()
             pb.rel_trans_weight = sp.get('trans_weight', 1.0)
-            norms['rel_transform'] = n_rel
         elif 'rel_transform' in loss_cfg:
-            norms['rel_transform'] = 0
-        # ---- scalar term tables
-        lens = lay.lens[:Q]                                  # one group's persons
-        norms.update({
-            'traj_rot_smoothness': Q * (T - 1), 'traj_trans_smoothness': Q * (T - 1),
-            'local_traj_dxy_reg': sum(n - 1 for n in lens), 'local_traj_dheading_reg': sum(n - 1 for n in lens),
-            'local_traj_dheading_reg_new': sum(n - 1 for n in lens), 'local_traj_rot_reg': sum(lens), 'local_traj_z_reg': sum(lens),
-            'traj_rot_res': Q * T, 'traj_trans_res': Q * T, 'cam_inv_trans_residual_reg': lay.trans_res_rows,
-            'cam_inv_rot_smoothness': T - 1, 'cam_origin_smoothness': T - 1, 'cam_rot_smoothness': T - 1, 'cam_trans_smoothness': T - 1,
-            'cam_depth_smoothness': 1,          # loss_func.py:102 sums over the T-1 frame pairs (the .mean() sees a 0-d tensor)
-        })
+            for gn in group_norms:
+                gn['rel_transform'] = 0
+        # ---- scalar term tables, each group's from its own persons and frames
+        for g, norms in enumerate(group_norms):
+            lg = lay.group_layout(g)[0]
+            Q, Tg, lens = self.Qs[g], self.Ts[g], lg.lens
+            norms.update({
+                'traj_rot_smoothness': Q * (Tg - 1), 'traj_trans_smoothness': Q * (Tg - 1),
+                'local_traj_dxy_reg': sum(n - 1 for n in lens), 'local_traj_dheading_reg': sum(n - 1 for n in lens),
+                'local_traj_dheading_reg_new': sum(n - 1 for n in lens), 'local_traj_rot_reg': sum(lens), 'local_traj_z_reg': sum(lens),
+                'traj_rot_res': Q * Tg, 'traj_trans_res': Q * Tg, 'cam_inv_trans_residual_reg': lg.trans_res_rows,
+                'cam_inv_rot_smoothness': Tg - 1, 'cam_origin_smoothness': Tg - 1, 'cam_rot_smoothness': Tg - 1,
+                'cam_trans_smoothness': Tg - 1,
+                'cam_depth_smoothness': 1,          # loss_func.py:102 sums over the T-1 frame pairs (the .mean() sees a 0-d tensor)
+            })
         pb.cam_traj_rot_quat = int(loss_cfg.get('cam_traj_rot', {}).get('rot_type', '6d') == 'quat')
         pb.traj_rot_smooth_quat = int(loss_cfg.get('traj_rot_smoothness', {}).get('rot_type', '6d') == 'quat')
         if (pb.cam_traj_rot_quat or pb.traj_rot_smooth_quat) and self.const[0]['orient_cam_q'] is None:
@@ -383,7 +473,8 @@ class StageCompiler:
             sp = loss_cfg['cam_up_reg']
             pb.cam_up_first_weight = sp.get('first_frame_weight', 1.0)
             pb.cam_up_first_only = int(sp.get('first_frame_only', False))
-            norms['cam_up_reg'] = 1 if pb.cam_up_first_only else T
+            for norms, Tg in zip(group_norms, self.Ts):
+                norms['cam_up_reg'] = 1 if pb.cam_up_first_only else Tg
         if ('cam_rot_smoothness' in loss_cfg or 'cam_trans_smoothness' in loss_cfg) and mode != L.CAM_PER_FRAME:
             raise NotImplementedError('cam_rot/trans_smoothness need per-frame camera variables')
         for name, sp in loss_cfg.items():
@@ -391,27 +482,45 @@ class StageCompiler:
             pb.term_enabled[k] = 1
             pb.term_monitor[k] = int(sp.get('monitor_only', False))
             pb.term_weight[k] = float(sp['weight'])
-            n = float(norms.get(name, 1))
+            n = float(group_norms[0].get(name, 1))
             pb.term_norm[k] = n if n > 0 else 1.0
+        if G > 1:                                            # the group table (include/glamr_b200.h, glamr_group_t)
+            table = (L.Group * G)()
+            for g, gr in enumerate(table):
+                lg, base = lay.group_layout(g)
+                gr.p0, gr.Q, gr.n0, gr.c0, gr.T = self.p0s[g], self.Qs[g], self.n0s[g], self.c0s[g], self.Ts[g]
+                gr.theta0, gr.rel0 = base, self.rel0[g]
+                gr.off_cam_rot, gr.off_cam_trans = (base + o for o in cam_offsets(lg))
+                for name in loss_cfg:
+                    k, n = L.TERM_INDEX[name], float(group_norms[g].get(name, 1))
+                    gr.term_norm[k] = n if n > 0 else 1.0
+                for k in range(L.NUM_TERMS):                 # the handle's weight / normaliser (float32 division)
+                    if pb.term_enabled[k] and not pb.term_monitor[k] and gr.term_norm[k] != 0.0:
+                        gr.gs[k] = float(np.float32(pb.term_weight[k]) / np.float32(gr.term_norm[k]))
+            table_dev = torch.frombuffer(bytearray(bytes(table)), dtype=torch.uint8).to(dev)
+            keep.append(table_dev)
+            pb.groups = table_dev.data_ptr()
+            self.table = table
         # ---- which entries of theta Adam updates (get_parameter, :591-633)
         active = torch.zeros(lay.n_params, dtype=torch.uint8)
 
         def on(o, n):
             active[o:o + n] = 1
-        for g0 in range(0, lay.n_params, lay.group_params):        # each group's camera variables
+        for g in range(G):                                    # each group's camera variables
+            lg, g0 = lay.group_layout(g)
             if 'cam' not in opt_variables:
-                on(g0 + lay.cam_inv_rot_res, 6 * lay.n_empty)
-                on(g0 + lay.cam_inv_trans_res, 3 * lay.trans_res_rows)
+                on(g0 + lg.cam_inv_rot_res, 6 * lg.n_empty)
+                on(g0 + lg.cam_inv_trans_res, 3 * lg.trans_res_rows)
             elif fl['flag_fixed_cam']:
-                on(g0 + lay.cam_rot_fix, 6)
-                on(g0 + lay.cam_trans_fix, 3)
+                on(g0 + lg.cam_rot_fix, 6)
+                on(g0 + lg.cam_trans_fix, 3)
             else:
-                on(g0 + lay.cam_rot, 6 * T)
-                on(g0 + lay.cam_trans, 3 * T)
+                on(g0 + lg.cam_rot, 6 * lg.T)
+                on(g0 + lg.cam_trans, 3 * lg.T)
         hd = lay.heading_dim
         sizes = lambda Ln: {'xy': 2, 'heading': hd, 'dxy': 2 * (Ln - 1), 'dheading': hd * (Ln - 1), 'z': Ln, 'rot': 6 * Ln}
         for p in range(P):
-            o, sz = lay.persons[p], sizes(lay.lens[p])
+            o, sz, T = lay.persons[p], sizes(lay.lens[p]), self.person_T[p]
             for key in opt_variables:
                 if key == 'world_res' and self.opt_traj:
                     on(o['orient_res'], 3 * T)
@@ -439,8 +548,25 @@ class StageCompiler:
 
 
 # ---------------------------------------------------------------------------------------------------- variables
+_KINDS = [('heading_dim', 'heading variables (heading_type)'), ('world_dxy', 'world_dxy variables'),
+          ('person2cam', 'person2cam residuals')]
+
+
 def make_layout(data, flags):
-    """layout of one data dict, or of the seed groups in a list of data dicts (which must agree on every block)"""
+    """layout of one data dict, of the seed groups in a list of data dicts (which must agree on every block), or of a batch of
+    sequences (a list of such lists): a BatchLayout of one one-group layout per group, which must agree on the variable kinds"""
+    if _is_batch(data) and len(data) == 1:                 # one sequence: its seed groups
+        return make_layout(list(data[0]), flags)
+    if _is_batch(data):
+        lays = []
+        for seq in data:
+            one = make_layout(list(seq), flags)                # the seeds of one sequence agree on every block
+            lays += [one.group_layout(g)[0] for g in range(one.G)]
+        for attr, what in _KINDS:
+            vals = sorted({getattr(l, attr) for l in lays})
+            if len(vals) > 1:
+                raise ValueError(f'the groups of one problem share one config, but their {what} differ ({attr}: {vals})')
+        return lays[0] if len(lays) == 1 else BatchLayout(lays)
     datas = _groups(data)
     lays = [_one_group_layout(d, flags) for d in datas]
     key = lambda l: (l.T, l.n_empty, l.trans_res_rows, l.lens, l.heading_dim, l.world_dxy, l.person2cam)
@@ -478,8 +604,8 @@ def bind_variables(data, layout, theta):
         for name in ['cam_inv_rot_residual', 'cam_inv_trans_residual']:
             gv[name].copy_(torch.as_tensor(dd[name]).to(theta))
             dd[name] = gv[name]
-        for q, d in enumerate(dd['person_data'].values()):
-            pv = layout.views(theta, g * layout.Q + q)
+        for p, d in zip(layout.group_persons(g), dd['person_data'].values()):
+            pv = layout.views(theta, p)
             for name in ['traj_local_xy', 'traj_local_heading', 'traj_local_dxy', 'traj_local_dheading', 'traj_local_z',
                          'traj_local_rot', 'smpl_orient_world_res', 'root_trans_world_res', 'world_dheading', 'world_dxy',
                          'person2cam_res_rot', 'person2cam_res_trans']:
@@ -499,6 +625,7 @@ def begin_stage_variables(data, layout, theta, flags, opt_variables):
                          "(make_layout(..., flags={'world_dxy': True, ...}))")
     for g, data in enumerate(_groups(data)):
         gv = layout.views(theta, group=g)
+        T = layout.group_layout(g)[0].T
         if 'cam' in opt_variables:
             cam = torch.as_tensor(data['cam_pose']).to(theta)
             d6 = torch.cat([cam[:, :3, 0], cam[:, :3, 1]], dim=-1)           # rotmat_to_rot6d: first two columns
@@ -506,14 +633,14 @@ def begin_stage_variables(data, layout, theta, flags, opt_variables):
                 gv['cam_rot_6d_fix'].copy_(d6[:1])
                 gv['cam_trans_fix'].copy_(cam[:1, :3, 3])
                 data['cam_rot_6d_fix'], data['cam_trans_fix'] = gv['cam_rot_6d_fix'], gv['cam_trans_fix']
-                data['cam_rot_6d'] = gv['cam_rot_6d_fix'].expand(layout.T, -1)
-                data['cam_trans'] = gv['cam_trans_fix'].expand(layout.T, -1)
+                data['cam_rot_6d'] = gv['cam_rot_6d_fix'].expand(T, -1)
+                data['cam_trans'] = gv['cam_trans_fix'].expand(T, -1)
             else:
                 gv['cam_rot_6d'].copy_(d6)
                 gv['cam_trans'].copy_(cam[:, :3, 3])
                 data['cam_rot_6d'], data['cam_trans'] = gv['cam_rot_6d'], gv['cam_trans']
-        for q, d in enumerate(data['person_data'].values()):
+        for p, d in zip(layout.group_persons(g), data['person_data'].values()):
             if 'world_dheading' in opt_variables and 'world_dheading' not in d:
-                d['world_dheading'] = layout.views(theta, g * layout.Q + q)['world_dheading']
+                d['world_dheading'] = layout.views(theta, p)['world_dheading']
             if 'world_dxy' in opt_variables and 'world_dxy' not in d:
-                d['world_dxy'] = layout.views(theta, g * layout.Q + q)['world_dxy']
+                d['world_dxy'] = layout.views(theta, p)['world_dxy']

@@ -3,8 +3,9 @@
 
 Same constructor, ``optimize(in_dict, continue_opt=False) -> dict`` (numpy), ``init_data``, ``forward``,
 ``compute_loss``, ``optimize_main``; same YAML stage specs; same output keys / shapes / dtypes (SURVEY.md Appendix B).
-``optimize_seeds(in_dict, seeds) -> [dict]`` runs several seeds of one sequence as one problem (seed groups, see
-glamr_b200/problem.py): every seed's result is the one ``optimize`` gives for that seed.
+``optimize_seeds(in_dict, seeds) -> [dict]`` runs several seeds of one sequence as one problem, and
+``optimize_batch(in_dicts, seeds) -> [[dict]]`` every (sequence, seed) pair of several sequences (groups, see glamr_b200/problem.py):
+every pair's result is the one ``optimize`` gives for that sequence and seed.
 Host Python does what the reference does on the host (dict bookkeeping, SciPy rotation-vector conversion and linear
 gap interpolation, log lines); every formula of the per-iteration path -- trajectory codec, camera, SMPL, projection,
 residuals, analytic backward, Adam -- is a kernel of glamr_b200/csrc.  No autograd, no CPU fallback.
@@ -558,11 +559,11 @@ class GlobalReconOptimizer:
     # ------------------------------------------------------------------------------------------------ device state
     def _attach(self, data):
         """Pack the optimisation variables into theta and build the constant tables.  The CUDA handle (scratch arena,
-        Adam moments, captured iteration graph) is kept across calls while (P, T, J, n_params) stay the same.  `data`: one
-        data dict, or the list of the seed groups' data dicts (optimize_seeds)."""
+        Adam moments, captured iteration graph) is kept across calls while (P, T, J, n_params) and the group shapes stay the same.
+        `data`: one data dict, or the groups of optimize_batch (a list of per-sequence lists of seed dicts)."""
         self._fresh_attach = True
         self._data = data
-        self._n_groups = len(data) if isinstance(data, list) else 1
+        self._n_groups = len(PB._groups(data))
         self._layout = PB.make_layout(data, self._flags)
         self._theta = torch.zeros(self._layout.n_params, device=self.device)
         PB.bind_variables(data, self._layout, self._theta)
@@ -574,7 +575,7 @@ class GlobalReconOptimizer:
         self._stage_key = None
         # multi-GPU: contiguous shards of the frame-persons n = p*T + t (SMPL + per-frame residuals are independent per
         # frame-person, so a person may straddle two ranks; P persons on P GPUs gives one person each)
-        N = self._comp.P * self._comp.T
+        N = self._comp.N
         self._n_range = (N * self.rank // self.world, N * (self.rank + 1) // self.world)
 
     def _release(self, at_exit=False):
@@ -654,7 +655,7 @@ class GlobalReconOptimizer:
         pb = self._comp.compile(self._theta, opt_variables, loss_cfg, stage, n_begin=self._n_range[0], n_end=self._n_range[1],
                                 owner=(self.rank == 0))
         self._pb = pb
-        dims = (pb.P, pb.T, pb.J, pb.n_params)
+        dims = (pb.P, pb.T, pb.J, pb.n_params, tuple(zip(self._comp.Qs, self._comp.Ts)))
         if self._opt is not None and dims != getattr(self, '_opt_dims', None):
             self._release()
         with torch.cuda.device(self.device):
@@ -690,43 +691,45 @@ class GlobalReconOptimizer:
 
     def _scatter_outputs(self, data):
         """copy what forward() stores into the data dict (each seed group's, for a list) in the reference (:421-528)"""
-        P, T, J, Q = self._comp.P, self._comp.T, self._comp.J, self._comp.Q
-        ow, tw = self._read(L.R_ORIENT_WORLD, P, T, 3), self._read(L.R_TRANS_WORLD, P, T, 3)
-        ob, tb = self._read(L.R_ORIENT_BASE, P, T, 3), self._read(L.R_TRANS_BASE, P, T, 3)
-        kp = self._read(L.R_KP_PRED, P, T, J, 2)
-        ociw, tciw = self._read(L.R_ORIENT_CIW, P, T, 3), self._read(L.R_TRANS_CIW, P, T, 3)
-        tl = self._read(L.R_TRAJ_LOCAL, P, T, 11) if self.traj_source == L.TRAJ_PREDICTED else None
-        jw = self._read(L.R_JOINTS_WORLD, P, T, J, 3)
+        comp = self._comp
+        N, J = comp.N, comp.J
+        ow, tw = self._read(L.R_ORIENT_WORLD, N, 3), self._read(L.R_TRANS_WORLD, N, 3)
+        ob, tb = self._read(L.R_ORIENT_BASE, N, 3), self._read(L.R_TRANS_BASE, N, 3)
+        kp = self._read(L.R_KP_PRED, N, J, 2)
+        ociw, tciw = self._read(L.R_ORIENT_CIW, N, 3), self._read(L.R_TRANS_CIW, N, 3)
+        tl = self._read(L.R_TRAJ_LOCAL, N, 11) if self.traj_source == L.TRAJ_PREDICTED else None
+        jw = self._read(L.R_JOINTS_WORLD, N, J, 3)
         if self.world > 1:
             # per-frame-person outputs exist only on the rank that evaluated that frame-person: keep the own shard, sum over ranks
-            own = torch.zeros(P * T, device=self.device)
+            own = torch.zeros(N, device=self.device)
             own[self._n_range[0]:self._n_range[1]] = 1.0
-            own = own.view(P, T)
-            packed = torch.cat([(x * own.view(P, T, *([1] * (x.dim() - 2)))).reshape(P * T, -1) for x in (kp, ociw, tciw, jw)], dim=1).contiguous()
+            packed = torch.cat([(x * own.view(N, *([1] * (x.dim() - 1)))).reshape(N, -1) for x in (kp, ociw, tciw, jw)], dim=1).contiguous()
             torch.distributed.all_reduce(packed)
             o = 0
             outs = []
             for x in (kp, ociw, tciw, jw):
-                w = x[0, 0].numel()
+                w = x[0].numel()
                 outs.append(packed[:, o:o + w].reshape(x.shape))
                 o += w
             kp, ociw, tciw, jw = outs
-        datas = data if isinstance(data, list) else [data]
-        ng = len(datas)
-        cam, cam_inv = self._read(L.R_CAM_POSE, ng, T, 12), self._read(L.R_CAM_POSE_INV, ng, T, 12)
+        datas = PB._groups(data)
+        cam, cam_inv = self._read(L.R_CAM_POSE, sum(comp.Ts), 12), self._read(L.R_CAM_POSE_INV, sum(comp.Ts), 12)
         for g, dg in enumerate(datas):
-            dg['cam_pose'] = G.from34(cam[g] if ng > 1 else cam.view(T, 12))
-            dg['cam_pose_inv'] = G.from34(cam_inv[g] if ng > 1 else cam_inv.view(T, 12))
+            r, T = comp.c0s[g], comp.Ts[g]
+            dg['cam_pose'] = G.from34(cam[r:r + T])
+            dg['cam_pose_inv'] = G.from34(cam_inv[r:r + T])
             for q, d in enumerate(dg['person_data'].values()):
-                p = g * Q + q
-                d['smpl_orient_world'], d['root_trans_world'] = ow[p], tw[p]
-                d['smpl_orient_world_base'], d['root_trans_world_base'] = ob[p], tb[p]
-                d['kp_2d_pred'] = kp[p]
-                d['smpl_orient_cam_in_world'], d['root_trans_cam_in_world'] = ociw[p], tciw[p]
+                p = comp.p0s[g] + q
+                rows = slice(comp.n0s[g] + q * T, comp.n0s[g] + (q + 1) * T)
+                ow_p, tw_p = ow[rows], tw[rows]
+                d['smpl_orient_world'], d['root_trans_world'] = ow_p, tw_p
+                d['smpl_orient_world_base'], d['root_trans_world_base'] = ob[rows], tb[rows]
+                d['kp_2d_pred'] = kp[rows]
+                d['smpl_orient_cam_in_world'], d['root_trans_cam_in_world'] = ociw[rows], tciw[rows]
                 if self.traj_source == L.TRAJ_PREDICTED:           # without the codec the reference has no traj_local
-                    d['traj_local'] = tl[p][d['exist_frames']]
-                d['joints_world'] = jw[p]
-                d['person_transform_world'] = G.make_transform(ow[p], tw[p], 'axis_angle')
+                    d['traj_local'] = tl[rows][d['exist_frames']]
+                d['joints_world'] = jw[rows]
+                d['person_transform_world'] = G.make_transform(ow_p, tw_p, 'axis_angle')
 
     # ------------------------------------------------------------------------------------------------ reference API
     def forward(self, data, opt_variables, opt_meta):
@@ -750,11 +753,11 @@ class GlobalReconOptimizer:
 
     def optimize_main(self, data, opt_variables, opt_lr, opt_niters, loss_cfg, opt_meta):
         """:547-570 -- opt_niters fused iterations (forward + residuals + backward [+ allreduce] + Adam).  `data` may be the
-        list of the seed groups' data dicts attached by optimize_seeds."""
+        groups attached by optimize_batch."""
         stage = opt_meta['stage']
         self._cur_vars, self._cur_stage, self._loss_cfg = opt_variables, stage, loss_cfg
         lib = self._lib
-        datas = data if isinstance(data, list) else [data]
+        datas = PB._groups(data)
         ng = len(datas)
         seq_names = [d['seq_name'] for d in datas]
         if ng > 1:
@@ -872,40 +875,70 @@ class GlobalReconOptimizer:
         return out
 
     def optimize_seeds(self, in_dict, seeds):
-        """Optimise several seeds of one sequence as one problem.  Element k of the result is what
-        ``np.random.seed(s); torch.manual_seed(s); optimize(copy.deepcopy(in_dict))`` returns for s = seeds[k], bit for bit:
-        every seed's init_data (and the learned prior in it) runs as in the serial path after setting the RNGs the same way, then
-        the S data dicts are attached as S seed groups of one problem (glamr_b200/problem.py) and the stages run once for all of
-        them.  Each group's camera, terms and gradient are reduced exactly as in its own one-group problem.
-        ``self.seed_loss_histories[k]`` is seed k's loss history of the last stage (``loss_history`` of its serial run).
-        No continue_opt; one GPU only (run_dataset shards sequences over ranks, each rank batches its own seeds)."""
+        """Optimise several seeds of one sequence as one problem: ``optimize_batch([in_dict], seeds)[0]``.  Element k of the result
+        is what ``np.random.seed(s); torch.manual_seed(s); optimize(copy.deepcopy(in_dict))`` returns for s = seeds[k], bit for bit.
+        ``self.seed_loss_histories[k]`` is seed k's loss history of the last stage (``loss_history`` of its serial run)."""
         if self.world > 1:
             raise ValueError('optimize_seeds runs on one GPU: shard sequences over ranks and batch the seeds on each rank')
-        seeds = [int(s) for s in seeds]
-        if not seeds:
+        if not list(seeds):
             return []
+        outs = self.optimize_batch([in_dict], seeds)[0]
+        self.seed_loss_histories = self.batch_loss_histories[0]
+        return outs
+
+    def optimize_batch(self, in_dicts, seeds):
+        """Optimise every (sequence, seed) pair of `in_dicts` x `seeds` as one group of one problem.  The sequences share this
+        optimiser's config and may differ in frames, persons, exist ranges and visibility.  ``outs[i][k]`` is what
+        ``np.random.seed(s); torch.manual_seed(s); optimize(copy.deepcopy(in_dicts[i]))`` returns for s = seeds[k], bit for bit:
+        every pair's init_data (and the learned prior in it) runs as in the serial path after setting the RNGs the same way, then
+        the data dicts are attached as the groups of one problem (glamr_b200/problem.py) and the stages run once for all of them.
+        Each group's camera, terms and gradient are reduced exactly as in its own one-group problem, from its own normalisers.
+        ``self.batch_loss_histories[i][k]`` is that pair's loss history of the last stage.  Scratch grows with the frame-persons of
+        all groups (sum of persons x frames).  No continue_opt; one GPU only (run_dataset shards sequences over ranks)."""
+        if self.world > 1:
+            raise ValueError('optimize_batch runs on one GPU: shard sequences over ranks and batch them on each rank')
+        seeds = [int(s) for s in seeds]
+        in_dicts = list(in_dicts)
+        if not seeds or not in_dicts:
+            return [[] for _ in in_dicts]
         t0 = time.perf_counter()
-        datas = []
-        for s in seeds:                                # run_dataset's RNG setting, then the serial path's init
-            np.random.seed(s)
-            torch.manual_seed(s)
-            datas.append(self.init_data(copy.deepcopy(in_dict)))
+        batch = self._init_groups(in_dicts, seeds)
         t1 = time.perf_counter()
-        self._attach(datas)
+        self._optimize_groups(batch)
+        t2 = time.perf_counter()
+        outs = [[tensor_to_numpy(data) for data in seq] for seq in batch]
+        self.phase_seconds = {'init_data': t1 - t0, 'stages': t2 - t1, 'to_numpy': time.perf_counter() - t2}
+        return outs
+
+    def _init_groups(self, in_dicts, seeds):
+        """init_data of every (sequence, seed) pair, serially with the RNGs set as run_dataset sets them -> [[data dict]]"""
+        batch = []
+        for in_dict in in_dicts:
+            seq = []
+            for s in seeds:
+                np.random.seed(s)
+                torch.manual_seed(s)
+                seq.append(self.init_data(copy.deepcopy(in_dict)))
+            batch.append(seq)
+        return batch
+
+    def _optimize_groups(self, batch):
+        """the stages of optimize for the groups of `batch` ([[data dict]] from _init_groups) as one problem; each pair's loss history
+        of the last stage goes to batch_loss_histories"""
+        datas = [d for seq in batch for d in seq]
+        groups = batch[0] if len(batch) == 1 else batch        # one sequence: its seed groups, with the layout they always had
+        self._attach(groups)
         for stage, stage_specs in self.opt_stage_specs.items():
             opt_meta = {'stage': stage, 'opt_latent_start_iter': stage_specs.get('opt_latent_start_iter', 0)}
-            self.optimize_main(datas, stage_specs['opt_variables'], stage_specs['opt_lr'], stage_specs['opt_niters'],
+            self.optimize_main(groups, stage_specs['opt_variables'], stage_specs['opt_lr'], stage_specs['opt_niters'],
                                stage_specs['loss_cfg'], opt_meta)
             if stage_specs.get('reinitialize_cam', False):
                 for data in datas:
                     data['cam_pose'][:] = data['cam_pose'][[0]]
                     data['cam_pose_inv'] = G.inverse_transform(data['cam_pose'])
-        t2 = time.perf_counter()
-        lh = self.loss_history
-        self.seed_loss_histories = [lh] if len(seeds) == 1 else [lh[:, g] for g in range(len(seeds))]
-        outs = [tensor_to_numpy(data) for data in datas]
-        self.phase_seconds = {'init_data': t1 - t0, 'stages': t2 - t1, 'to_numpy': time.perf_counter() - t2}
-        return outs
+        lh, S = self.loss_history, len(batch[0])
+        hists = [lh] if len(datas) == 1 else [lh[:, g] for g in range(len(datas))]
+        self.batch_loss_histories = [hists[i * S:(i + 1) * S] for i in range(len(batch))]
 
 
 def _device_view(addr, count, device):

@@ -170,7 +170,7 @@ enum glamr_traj_source {
 
 typedef struct glamr_person {
   int32_t start, len;              /* exist range [start, start+len) of this person (exist_frames)              */
-  int32_t group;                   /* seed group of this person (see glamr_problem_t.G): p / (P/G) for person p  */
+  int32_t group;                   /* group of this person (see glamr_group_t)                                    */
   int32_t off_xy, off_heading, off_dxy, off_dheading, off_z, off_rot;     /* offsets into theta (floats)        */
   int32_t off_world_dheading, off_orient_res, off_trans_res;              /* [T], [T,3], [T,3]                  */
   int32_t off_world_dxy;           /* [T,2] world_dxy (read only with has_world_dxy)                              */
@@ -201,22 +201,35 @@ typedef struct glamr_person {
   float* world_dxy_base;
 } glamr_person_t;
 
-/* Seed groups: G independent copies of one sequence (same persons, frames, visibility and loss normalisers, each with its own
- * initial state) optimised as one problem.  Group g owns persons [g*P/G, (g+1)*P/G) and theta [g*group_params, (g+1)*group_params):
- * its camera variables sit at off_cam_rot / off_cam_trans + g*group_params.  Every per-frame table below has one [T,...] block per
- * group, the rel_transform tables one [(P/G)^2,T,...] block per group (pairs only inside a group), the term sums and loss terms
- * one row per group.  Each group's camera, camera terms and term sums are reduced over the same elements in the same order as
- * the one-group problem of that group alone, so every group's results are those of its own one-group run bit for bit.  G > 1
- * needs the whole frame-person range on one rank (n_begin 0, n_end P*T, owner).  G 0 (zero-initialised) = 1. */
+/* Groups: G independent problems that share one configuration (stages, variables, loss settings) optimised as one problem: the
+ * seeds of one sequence, or any (sequence, seed) pairs.  Group g owns persons [p0, p0+Q), frame-persons [n0, n0 + Q*T) (frame t of
+ * its person p0+q is row n0 + q*T + t), camera rows [c0, c0+T) of every per-frame table and camera read-back, and the block of theta
+ * that starts at theta0.  Its rel_transform pairs (only inside the group) are the [Q*Q, T] block at rel0, its term sums and loss
+ * terms one row each.  Each group's camera, camera terms and term sums are reduced over the same elements in the same order as the
+ * one-group problem of that group alone, so every group's results are those of its own one-group run bit for bit.  G > 1 needs the
+ * whole frame-person range on one rank (n_begin 0, n_end = sum Q*T, owner).  G 0 (zero-initialised) = 1. */
+typedef struct glamr_group {
+  int32_t p0, Q;                   /* first person, persons                                                        */
+  int32_t n0;                      /* first frame-person                                                           */
+  int32_t c0, T;                   /* first camera row, frames                                                     */
+  int32_t theta0;                  /* first float of the group's block of theta                                    */
+  int32_t off_cam_rot, off_cam_trans; /* theta offsets of the group's camera variables (as glamr_problem_t's)       */
+  int32_t rel0;                    /* first (pair, frame) entry of the group's block of rel_target / rel_w / rel_wt */
+  float term_norm[GLAMR_NUM_TERMS];  /* the group's normalisers (denominators of the reference's means)             */
+  float gs[GLAMR_NUM_TERMS];       /* term_weight / term_norm in float32 where the term enters the total, else 0   */
+} glamr_group_t;
+
 typedef struct glamr_problem {
-  int32_t P, T, J;                 /* persons (all groups), frames, joints per person (n_map of the SMPL handle)  */
+  int32_t P, T, J;                 /* persons (all groups), frames (the longest group's), joints per person (n_map of the
+                                    * SMPL handle)                                                                  */
   int32_t cam_mode;                /* enum glamr_cam_mode                                                         */
-  int32_t off_cam_rot, off_cam_trans; /* variable offsets (modes 1,2: cam_rot_6d / cam_trans; mode 3: residuals)  */
+  int32_t off_cam_rot, off_cam_trans; /* variable offsets (modes 1,2: cam_rot_6d / cam_trans; mode 3: residuals); with
+                                    * groups, those of group 0 (glamr_group_t has every group's)                       */
   int32_t use_world_res, has_world_dheading;
   int32_t trans_res_all;           /* mode 3: cam_inv_trans_residual has T rows (else one row per empty frame)    */
   int32_t cam_up_first_only;
   int32_t n_params;                /* length of theta / grad / adam state                                         */
-  int32_t n_begin, n_end;          /* frame-persons n = p*T + t whose SMPL / per-frame residuals this rank evaluates
+  int32_t n_begin, n_end;          /* frame-persons n = p*T + t (n0 + q*T + t with groups) whose SMPL / per-frame residuals this rank evaluates
                                     * (multi-GPU shard; any contiguous range, a person may straddle two ranks)         */
   int32_t owner;                   /* != 0: this rank also evaluates the replicated terms (camera, regs, rel)    */
   int32_t cam_traj_rot_quat;       /* cam_traj_rot: rot_type 'quat' (loss_func.py:158-161) instead of '6d'          */
@@ -228,8 +241,9 @@ typedef struct glamr_problem {
   int32_t world_dxy_alias;         /* that add also lands in the base (see glamr_person_t.world_dxy_base)          */
   int32_t has_person2cam;          /* flag_opt_person2cam_rot / _trans (:484-488): mode 3 composes each person's person2cam with
                                     * [rot6d(person2cam_res_rot) | person2cam_res_trans] before the mean; 0 = person2cam as is */
-  int32_t G;                       /* seed groups (see above); P % G == 0                                          */
-  int32_t group_params;            /* floats of theta per group (n_params = G * group_params; unused with one group) */
+  int32_t G;                       /* groups (see above); G > 1 needs `groups`                                     */
+  int32_t group_params;            /* floats of theta per group when all groups have one layout (seed groups), else 0;
+                                    * informational, the table holds every group's base                            */
   float cam_up_first_weight;
   float rel_trans_weight;
   float term_weight[GLAMR_NUM_TERMS];   /* YAML weight, 0 if the term is absent                                  */
@@ -237,16 +251,19 @@ typedef struct glamr_problem {
   int32_t term_enabled[GLAMR_NUM_TERMS];
   int32_t term_monitor[GLAMR_NUM_TERMS];
   const glamr_person_t* persons;   /* DEVICE array [P]                                                            */
-  const float* smpl_pose_all;      /* [P,T,69] body pose (infilled), constant during optimisation                 */
-  const float* smpl_beta_all;      /* [P,T,10]                                                                    */
-  const float* scale_all;          /* [P,T] or NULL                                                               */
-  const float* cam_pose_const;     /* [G,T,12] world->cam 3x4 (mode 0)                                            */
-  const int32_t* empty_index;      /* [G,T] row of cam_inv_rot_residual for frames without any person, else -1   */
-  const int32_t* fill_src;         /* [G,T] forward-fill source frame (mode 3), a frame of the same group         */
-  const float* inv_num_persons;    /* [G,T] 1/num visible persons of the group (0 where none)                     */
-  const float* rel_target;         /* [G,Q*Q,T,12] rel_transform_cam (i*Q+j, Q = P/G persons per group), or NULL  */
-  const float* rel_w;              /* [G,Q*Q,T] squared frame weights for the rotation part (0 = frame unused)    */
-  const float* rel_wt;             /* [G,Q*Q,T] same for the translation part                                     */
+  const glamr_group_t* groups;     /* DEVICE array [G] (G > 1; unused with one group).  glamr_opt_set_problem accepts
+                                    * only a table with the p0, Q, n0, c0, T of the one given to glamr_opt_create
+                                    * (theta0, camera offsets, rel0 and the normalisers may change)                */
+  const float* smpl_pose_all;      /* [N,69] body pose (infilled) of every frame-person, constant during optimisation */
+  const float* smpl_beta_all;      /* [N,10]                                                                      */
+  const float* scale_all;          /* [N] or NULL                                                                 */
+  const float* cam_pose_const;     /* [sum T,12] world->cam 3x4 (mode 0), one block of T rows per group           */
+  const int32_t* empty_index;      /* [sum T] row of cam_inv_rot_residual for frames without any person, else -1  */
+  const int32_t* fill_src;         /* [sum T] forward-fill source frame (mode 3), a frame of the same group        */
+  const float* inv_num_persons;    /* [sum T] 1/num visible persons of the group (0 where none)                   */
+  const float* rel_target;         /* per group [Q*Q,T,12] rel_transform_cam (pair i*Q+j inside the group), or NULL */
+  const float* rel_w;              /* per group [Q*Q,T] squared frame weights for the rotation part (0 = unused)  */
+  const float* rel_wt;             /* per group [Q*Q,T] same for the translation part                             */
   const uint8_t* active;           /* [n_params] 1 where Adam updates theta                                       */
 } glamr_problem_t;
 
@@ -255,11 +272,11 @@ size_t glamr_sizeof_problem(void);
 
 typedef struct glamr_opt glamr_opt_t;
 
-/* The handle owns scratch sized for (P,T,J) and the Adam moments.  `problem` is copied (host struct; its embedded
+/* The handle owns scratch sized for N = sum Q*T frame-persons (P*T with one group), sum T camera rows and J, and the Adam moments.  `problem` is copied (host struct; its embedded
  * pointers are device pointers that must stay alive while the handle uses them). */
 int glamr_opt_create(glamr_opt_t** out, const glamr_smpl_t* smpl, const glamr_problem_t* problem);
 int glamr_opt_destroy(glamr_opt_t* st);
-/* Re-read a modified problem description (new stage: weights, active mask, camera mode; same P, T, J, n_params).
+/* Re-read a modified problem description (new stage: weights, active mask, camera mode; same P, T, J, n_params and group shapes).
  * reset_adam bit 0 zeroes the Adam moments and step count: the reference builds a fresh torch.optim.Adam per stage
  * (global_recon_model.py:548,:642); bit 1 also zeroes all scratch (handle re-used for a new sequence).  A changed
  * frame-person range [n_begin, n_end) re-primes the pipelined blend: the next evaluation recomputes v_posed for it. */
@@ -310,6 +327,7 @@ int glamr_opt_last_lbs_ms(glamr_opt_t* st, float* ms);
  * stream: the mesh skinning and the blend after it (features + GEMM) */
 int glamr_opt_kernel_times(glamr_opt_t* st, float* ms, int* n);
 
+/* [P,T,...] below: one row per frame-person, N = sum Q*T rows with groups */
 enum glamr_read {
   GLAMR_R_ORIENT_WORLD = 0,    /* [P,T,3]   smpl_orient_world            */
   GLAMR_R_TRANS_WORLD = 1,     /* [P,T,3]   root_trans_world             */
@@ -318,8 +336,8 @@ enum glamr_read {
   GLAMR_R_KP_PRED = 4,         /* [P,T,J,2] kp_2d_pred                   */
   GLAMR_R_ORIENT_CAM_IN_WORLD = 5, /* [P,T,3]                            */
   GLAMR_R_TRANS_CAM_IN_WORLD = 6,  /* [P,T,3]                            */
-  GLAMR_R_CAM_POSE = 7,        /* [G,T,12]  world->cam 3x4               */
-  GLAMR_R_CAM_POSE_INV = 8,    /* [G,T,12]                               */
+  GLAMR_R_CAM_POSE = 7,        /* [sum T,12]  world->cam 3x4 of every group */
+  GLAMR_R_CAM_POSE_INV = 8,    /* [sum T,12]                             */
   GLAMR_R_JOINTS_WORLD = 9,    /* [P,T,J,3]                              */
   GLAMR_R_TRAJ_LOCAL = 10,     /* [P,T,11]  traj_local (rows of the exist range, others 0) */
   GLAMR_R_ADAM_M = 11,         /* [n_params] Adam first moment                                */

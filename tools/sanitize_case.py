@@ -1,5 +1,6 @@
 """Small end-to-end case for compute-sanitizer (memcheck / racecheck): SMPL forward at a ragged size through both LBS paths,
-one prior inference, a short optimisation through the iteration kernels, and two seed groups of one sequence (optimize_seeds).
+one prior inference, a short optimisation through the iteration kernels, two seed groups of one sequence (optimize_seeds) and a
+batch of sequences of mixed lengths (optimize_batch).
 
     compute-sanitizer --tool memcheck  python tools/sanitize_case.py
     compute-sanitizer --tool racecheck python tools/sanitize_case.py
@@ -51,4 +52,9 @@ m = GlobalReconOptimizer(cfg, dev, None, smpl=smpl, mt_model=prior)
 outs = m.optimize_seeds(make_in_dict(a, 2, 40, seed=1, gaps=True), [1, 2])
 torch.cuda.synchronize()
 print('seed groups ok', [float(o['cam_pose'].sum()) for o in outs])
+# a batch of sequences (glamr_group_t): mixed lengths, person counts and gaps, two seeds each, every group with its own normalisers
+outs = m.optimize_batch([make_in_dict(a, 1, 41, seed=2, gaps=True), make_in_dict(a, 3, 23, seed=3, gaps=False),
+                         make_in_dict(a, 2, 137, seed=4, gaps=True)], [1, 2])
+torch.cuda.synchronize()
+print('sequence batch ok', [float(o['cam_pose'].sum()) for row in outs for o in row])
 print('sanitize case done')
