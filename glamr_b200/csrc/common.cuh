@@ -29,9 +29,8 @@
 #endif
 
 // Which implementation runs when the environment does not say otherwise.  A path becomes the default only after its parity
-// tests passed on the GPU (GLAMR_LBS_PATH=tc|tcblend|simt and GLAMR_NET_WIMG=0|1 select explicitly for A/B runs).
+// tests passed on the GPU (GLAMR_LBS_PATH=tc|tcblend|simt selects explicitly for A/B runs).
 #define GLAMR_DEFAULT_LBS_TC 2        /* 2 = tensor-core blend + tensor-core skinning, 1 = tensor-core blend + SIMT skinning, 0 = FP32 SIMT kernel */
-#define GLAMR_DEFAULT_NET_WIMG 0       /* prior-network GEMMs: weight operand as a pre-split image fetched by bulk TMA (GLAMR_NET_WIMG=1) */
 
 namespace glamr {
 
@@ -142,15 +141,6 @@ __device__ __forceinline__ void wgmma_fence_acc(float (&d)[R]) {
 }
 // D[64 x N] (+)= A[64 x 8] B[N x 8]^T, both operands tf32 in shared memory.  Accumulator fragment of thread t of the warpgroup:
 // d[4 i + 2 h + e] = D[16 (t / 32) + (t % 32) / 4 + 8 h][8 i + 2 (t % 4) + e]
-__device__ __forceinline__ void wgmma_m64n32k8_tf32(float (&d)[16], uint64_t da, uint64_t db, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %18, 0;\n\t"
-      "wgmma.mma_async.sync.aligned.m64n32k8.f32.tf32.tf32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, %16, %17, p, 1, 1;\n\t}\n"
-      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
-        "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
-      : "l"(da), "l"(db), "r"(accumulate));
-}
 __device__ __forceinline__ void wgmma_m64n128k8_tf32(float (&d)[64], uint64_t da, uint64_t db, uint32_t accumulate) {
   asm volatile(
       "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %66, 0;\n\t"

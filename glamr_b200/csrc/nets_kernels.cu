@@ -8,7 +8,6 @@
 // Weights are addressed by their reference state-dict names so Lightning checkpoints map 1:1.
 #include <limits.h>
 #include <math.h>
-#include <stdlib.h>
 #include <string.h>
 
 #include <map>
@@ -81,13 +80,14 @@ __global__ void __launch_bounds__(256) gemm_bias_act_kernel(int M, int N, int K,
 // FP32 accuracy is kept with the 3xTF32 split  x = hi + lo (hi = tf32(x), lo = tf32(x - hi)):
 //   X W^T ~= Xhi Whi^T + Xlo Whi^T + Xhi Wlo^T     (error ~2^-21 relative per product; partial sums per K step of 32 are
 //   folded in FP32, see the main loop)
-// CTA = 256 threads = two warpgroups, tile 128 (M) x NT (N), K step 32; warpgroup g computes rows 64 g .. 64 g + 63 (m64nNTk8).
+// CTA = 256 threads = two warpgroups, tile 128 (M) x 128 (N), K step 32; warpgroup g computes rows 64 g .. 64 g + 63 (m64n128k8).
 // Both operands are K-major (X [M,K] and W [N,K] row-major), written by the CTA into shared memory in the canonical no-swizzle
 // layout (8-row x 16-byte core matrices: element (r,k) at ((k/4)*128 + r)*16 + (k%4)*4 bytes => LBO = 2048 B between K groups,
 // SBO = 128 B between 8-row groups) and made visible to the async proxy with fence.proxy.async; the epilogue adds the bias to the
 // accumulator fragment, applies the activation and stores.
-constexpr int TCM = 128, TCK = 32;                              // N tile (NT) is a template parameter: 128, or 32 for one-tile-high problems
+constexpr int TCM = 128, TCN = 128, TCK = 32;
 constexpr int kTcATileFloats = TCM * TCK;                       // 4096 floats = 16 KB (hi or lo of the X tile)
+constexpr int kTcBTileFloats = TCN * TCK;                       // 4096 floats = 16 KB (hi or lo of the W tile)
 
 __device__ __forceinline__ float4 split_tf32_4(const float4 v, float4& lo) {
   float4 hi;
@@ -95,25 +95,16 @@ __device__ __forceinline__ float4 split_tf32_4(const float4 v, float4& lo) {
   return hi;
 }
 
-#ifdef GLAMR_EXPERIMENT
-__device__ int g_tc_dbg = 0;   // experiment switches (tools/tc_gemm_exp.py, env GLAMR_TC_DEBUG); not in the release build
-#endif
 constexpr int kTcThreads = 256;
 constexpr int kTcStages = 2;
-template <int NT>
-struct TcCfg {
-  static constexpr int kBTileFloats = NT * TCK;
-  static constexpr int kStageFloats = 2 * kTcATileFloats + 2 * kBTileFloats;            // Xhi | Xlo | Whi | Wlo
-  static constexpr int kXVec = (TCM * TCK / 4) / kTcThreads;                            // 16-byte loads per thread and K step
-  static constexpr int kWVec = (NT * TCK / 4) / kTcThreads;
-  static constexpr size_t kSmemBytes = (size_t)kTcStages * kStageFloats * sizeof(float) + 16;
-  static_assert(kWVec >= 1, "W tile smaller than one 16-byte load per thread");
-};
+constexpr int kTcStageFloats = 2 * kTcATileFloats + 2 * kTcBTileFloats;                  // Xhi | Xlo | Whi | Wlo
+constexpr int kTcXVec = (TCM * TCK / 4) / kTcThreads;                                    // 16-byte loads per thread and K step
+constexpr int kTcWVec = (TCN * TCK / 4) / kTcThreads;
+constexpr size_t kTcSmemBytes = (size_t)kTcStages * kTcStageFloats * sizeof(float);
 
-// one K step (32 columns) of the 128-row X tile and the NT-row W tile, in flight in registers
-template <int NT>
+// one K step (32 columns) of the 128-row X tile and the 128-row W tile, in flight in registers
 struct TcRegs {
-  float4 x[TcCfg<NT>::kXVec], w[TcCfg<NT>::kWVec];
+  float4 x[kTcXVec], w[kTcWVec];
 };
 template <bool VEC>
 __device__ __forceinline__ float4 tc_load_row4(const float* __restrict__ P, int ld, int row, int nrows, int k, int K) {
@@ -126,31 +117,28 @@ __device__ __forceinline__ float4 tc_load_row4(const float* __restrict__ P, int 
   for (int q = 0; q < 4; ++q) a[q] = (row < nrows && k + q < K) ? P[(size_t)row * ld + k + q] : 0.0f;
   return make_float4(a[0], a[1], a[2], a[3]);
 }
-template <int NT, bool VEC, bool WIMG = false>
-__device__ __forceinline__ void tc_load_tiles(TcRegs<NT>& r, int tid, int M, int N, int K, const float* __restrict__ X, int ldx,
+template <bool VEC>
+__device__ __forceinline__ void tc_load_tiles(TcRegs& r, int tid, int M, int N, int K, const float* __restrict__ X, int ldx,
                                               const float* __restrict__ W, int m0, int n0, int k0) {
 #pragma unroll
-  for (int i = 0; i < TcCfg<NT>::kXVec; ++i) {
+  for (int i = 0; i < kTcXVec; ++i) {
     const int idx = tid + i * kTcThreads;
     r.x[i] = tc_load_row4<VEC>(X, ldx, m0 + (idx & (TCM - 1)), M, k0 + (idx / TCM) * 4, K);      // row, 16-byte K group (0..7)
   }
-  if (!WIMG) {
 #pragma unroll
-    for (int i = 0; i < TcCfg<NT>::kWVec; ++i) {
-      const int idx = tid + i * kTcThreads;
-      r.w[i] = tc_load_row4<VEC>(W, K, n0 + (idx & (NT - 1)), N, k0 + (idx / NT) * 4, K);
-    }
+  for (int i = 0; i < kTcWVec; ++i) {
+    const int idx = tid + i * kTcThreads;
+    r.w[i] = tc_load_row4<VEC>(W, K, n0 + (idx & (TCN - 1)), N, k0 + (idx / TCN) * 4, K);
   }
 }
 // split into tf32 hi / lo and store as K-major 8x16-byte core matrices (the layout wgmma_desc_kmajor_noswizzle describes)
-template <int NT, bool WIMG = false>
-__device__ __forceinline__ void tc_store_tiles(float* st, int tid, const TcRegs<NT>& r) {
+__device__ __forceinline__ void tc_store_tiles(float* st, int tid, const TcRegs& r) {
   float* Ahi = st;
   float* Alo = st + kTcATileFloats;
   float* Bhi = st + 2 * kTcATileFloats;
-  float* Blo = Bhi + TcCfg<NT>::kBTileFloats;
+  float* Blo = Bhi + kTcBTileFloats;
 #pragma unroll
-  for (int i = 0; i < TcCfg<NT>::kXVec; ++i) {
+  for (int i = 0; i < kTcXVec; ++i) {
     const int idx = tid + i * kTcThreads;
     const int off = ((idx / TCM) * TCM + (idx & (TCM - 1))) * 4;
     float4 lo;
@@ -158,83 +146,35 @@ __device__ __forceinline__ void tc_store_tiles(float* st, int tid, const TcRegs<
     *reinterpret_cast<float4*>(Ahi + off) = hi;
     *reinterpret_cast<float4*>(Alo + off) = lo;
   }
-  if (!WIMG) {
 #pragma unroll
-    for (int i = 0; i < TcCfg<NT>::kWVec; ++i) {
-      const int idx = tid + i * kTcThreads;
-      const int off = ((idx / NT) * NT + (idx & (NT - 1))) * 4;
-      float4 lo;
-      const float4 hi = split_tf32_4(r.w[i], lo);
-      *reinterpret_cast<float4*>(Bhi + off) = hi;
-      *reinterpret_cast<float4*>(Blo + off) = lo;
-    }
-  }
-}
-
-// ---- weights as a pre-split operand image -------------------------------------------------------------------------
-// A weight matrix W [N,K] is constant between glamr_net_set_tensor calls: it is split into tf32 hi / lo and tiled ONCE into the
-// shared-memory image the MMA reads, [N tile][K step of 32][hi | lo][8 K groups][NT rows][4] (zero padded), so that the kernel
-// fetches the W half of a pipeline stage with one 1-D bulk TMA copy instead of loading, splitting and storing it with all threads
-// on every launch.
-template <int NT>
-__global__ void build_w_image_kernel(const float* __restrict__ W, int N, int K, int ksteps, float* __restrict__ img) {
-  const size_t total = (size_t)((N + NT - 1) / NT) * ksteps * NT * TCK;
-  for (size_t e = (size_t)blockIdx.x * blockDim.x + threadIdx.x; e < total; e += (size_t)gridDim.x * blockDim.x) {
-    const int kk = (int)(e % TCK);
-    const int r = (int)((e / TCK) % NT);
-    const size_t tile = e / ((size_t)TCK * NT);              // tn * ksteps + ks
-    const int ks = (int)(tile % ksteps), tn = (int)(tile / ksteps);
-    const int n = tn * NT + r, k = ks * TCK + kk;
-    const float v = (n < N && k < K) ? W[(size_t)n * K + k] : 0.0f;
-    float hi, lo;
-    split_tf32(v, hi, lo);
-    float* q = img + tile * (2 * TcCfg<NT>::kBTileFloats) + ((size_t)(kk >> 2) * NT + r) * 4 + (kk & 3);
-    q[0] = hi;
-    q[TcCfg<NT>::kBTileFloats] = lo;
+  for (int i = 0; i < kTcWVec; ++i) {
+    const int idx = tid + i * kTcThreads;
+    const int off = ((idx / TCN) * TCN + (idx & (TCN - 1))) * 4;
+    float4 lo;
+    const float4 hi = split_tf32_4(r.w[i], lo);
+    *reinterpret_cast<float4*>(Bhi + off) = hi;
+    *reinterpret_cast<float4*>(Blo + off) = lo;
   }
 }
 
 // 256 threads; two shared-memory stages: while the tensor core works on stage s (12 wgmma per K step and warpgroup, one commit
 // group) all threads split and store K step it+1 into stage s^1 and already have the global loads of step it+2 in flight in
 // registers, so the L2 latency never sits on the critical path of these small GEMMs.
-// NT = 128: 128x128 tiles.  NT = 32: 128x32 tiles for problems one tile high (M <= 128, a single 120-frame window): 4x more
-// CTAs, each with a quarter of the W traffic, split work and epilogue.
-// WIMG: W points at the pre-split operand image of the weight (build_w_image_kernel) and arrives by bulk TMA (wbar[s]).
-template <int NT>
-__device__ __forceinline__ void wgmma_tf32_nt(float (&d)[NT / 2], uint64_t da, uint64_t db, uint32_t accumulate) {
-  if constexpr (NT == 128) wgmma_m64n128k8_tf32(d, da, db, accumulate);
-  else wgmma_m64n32k8_tf32(d, da, db, accumulate);
-}
-template <int ACT, bool VEC, int NT, bool WIMG>
+template <int ACT, bool VEC>
 __global__ void __launch_bounds__(kTcThreads) gemm_tf32x3_wgmma_kernel(int M, int N, int K, const float* __restrict__ X, int ldx,
                                                                        const float* __restrict__ W, const float* __restrict__ bias,
                                                                        const float* __restrict__ bias2, float* __restrict__ Y, int ldy) {
-  static_assert(NT == 128 || NT == 32, "N tile");
-  using Cfg = TcCfg<NT>;
   extern __shared__ __align__(128) unsigned char tc_smem[];
   float* stage0 = reinterpret_cast<float*>(tc_smem);
-  uint64_t* wbar = reinterpret_cast<uint64_t*>(stage0 + kTcStages * Cfg::kStageFloats);   // [2] weight image landed (WIMG)
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const int g = warp >> 2;                                                                // warpgroup: rows 64 g .. 64 g + 63
-  const int m0 = blockIdx.y * TCM, n0 = blockIdx.x * NT;
+  const int m0 = blockIdx.y * TCM, n0 = blockIdx.x * TCN;
 
   const int nk = (K + TCK - 1) / TCK;
-  constexpr uint32_t kWBytes = 2 * Cfg::kBTileFloats * sizeof(float);
-  const float* wimg = W + (size_t)blockIdx.x * nk * (2 * Cfg::kBTileFloats);            // this column tile's K steps, contiguous
-  if (tid == 0) {
-    mbar_init(&wbar[0], 1);
-    mbar_init(&wbar[1], 1);
-    mbar_fence_init();
-    if (WIMG) {
-      mbar_expect_tx(&wbar[0], kWBytes);
-      tma_bulk_g2s(stage0 + 2 * kTcATileFloats, wimg, kWBytes, &wbar[0]);
-    }
-  }
-  const int dbg = GLAMR_DBG(g_tc_dbg);
-  TcRegs<NT> regs;
-  tc_load_tiles<NT, VEC, WIMG>(regs, tid, M, N, K, X, ldx, W, m0, n0, 0);
-  tc_store_tiles<NT, WIMG>(stage0, tid, regs);
-  if (nk > 1) tc_load_tiles<NT, VEC, WIMG>(regs, tid, M, N, K, X, ldx, W, m0, n0, TCK);
+  TcRegs regs;
+  tc_load_tiles<VEC>(regs, tid, M, N, K, X, ldx, W, m0, n0, 0);
+  tc_store_tiles(stage0, tid, regs);
+  if (nk > 1) tc_load_tiles<VEC>(regs, tid, M, N, K, X, ldx, W, m0, n0, TCK);
   asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // generic-proxy smem writes -> visible to the tensor core
   __syncthreads();
 
@@ -242,159 +182,82 @@ __global__ void __launch_bounds__(kTcThreads) gemm_tf32x3_wgmma_kernel(int M, in
   // accumulation does not round to nearest, so a 3xTF32 sum kept in its accumulator over all of K drifts with K (a Linear missed a
   // float64 product by 4.6x, the infiller's output a float64 oracle by ~20x, what the FP32 kernels miss by); 32-wide partial sums
   // bound that drift to one K step.
-  float acc[NT / 2], part[NT / 2];
+  float acc[TCN / 2], part[TCN / 2];
 #pragma unroll
-  for (int i = 0; i < NT / 2; ++i) acc[i] = 0.0f;
+  for (int i = 0; i < TCN / 2; ++i) acc[i] = 0.0f;
   for (int it = 0; it < nk; ++it) {
     const int s = it & 1;
-    float* st = stage0 + s * Cfg::kStageFloats;
-    if (WIMG) mbar_wait(&wbar[s], (it >> 1) & 1);                         // this stage's weight image has landed
+    float* st = stage0 + s * kTcStageFloats;
     wgmma_fence();
 #pragma unroll
-    for (int k8 = 0; k8 < ((dbg & 1) ? 0 : TCK / 8); ++k8) {             // one tf32 wgmma consumes K = 8 (two 16-byte K groups)
-      const size_t koa = (size_t)k8 * 2 * TCM * 4 + g * 64 * 4, kob = (size_t)k8 * 2 * NT * 4;   // floats
+    for (int k8 = 0; k8 < TCK / 8; ++k8) {                               // one tf32 wgmma consumes K = 8 (two 16-byte K groups)
+      const size_t koa = (size_t)k8 * 2 * TCM * 4 + g * 64 * 4, kob = (size_t)k8 * 2 * TCN * 4;   // floats
       const uint64_t dah = wgmma_desc_kmajor_noswizzle(st + koa, TCM), dal = wgmma_desc_kmajor_noswizzle(st + kTcATileFloats + koa, TCM);
-      const uint64_t dbh = wgmma_desc_kmajor_noswizzle(st + 2 * kTcATileFloats + kob, NT);
-      const uint64_t dbl = wgmma_desc_kmajor_noswizzle(st + 2 * kTcATileFloats + Cfg::kBTileFloats + kob, NT);
-      wgmma_tf32_nt<NT>(part, dal, dbh, k8 > 0 ? 1u : 0u);             // the small cross terms first
-      wgmma_tf32_nt<NT>(part, dah, dbl, 1u);
-      wgmma_tf32_nt<NT>(part, dah, dbh, 1u);
+      const uint64_t dbh = wgmma_desc_kmajor_noswizzle(st + 2 * kTcATileFloats + kob, TCN);
+      const uint64_t dbl = wgmma_desc_kmajor_noswizzle(st + 2 * kTcATileFloats + kTcBTileFloats + kob, TCN);
+      wgmma_m64n128k8_tf32(part, dal, dbh, k8 > 0 ? 1u : 0u);            // the small cross terms first
+      wgmma_m64n128k8_tf32(part, dah, dbl, 1u);
+      wgmma_m64n128k8_tf32(part, dah, dbh, 1u);
     }
     wgmma_commit();
     if (it + 1 < nk) {
       // stage s^1 was last read by step it-1, which every warpgroup retired before the barrier that ended that step: refill it
       // while step `it` computes
-      if (WIMG && tid == 0) {                                            // stage s^1 is free: fetch the weight image of step it+1
-        mbar_expect_tx(&wbar[s ^ 1], kWBytes);
-        tma_bulk_g2s(stage0 + (s ^ 1) * Cfg::kStageFloats + 2 * kTcATileFloats, wimg + (size_t)(it + 1) * (2 * Cfg::kBTileFloats), kWBytes, &wbar[s ^ 1]);
-      }
-      if (!(dbg & 2)) tc_store_tiles<NT, WIMG>(stage0 + (s ^ 1) * Cfg::kStageFloats, tid, regs);
-      if (it + 2 < nk && !(dbg & 8)) tc_load_tiles<NT, VEC, WIMG>(regs, tid, M, N, K, X, ldx, W, m0, n0, (it + 2) * TCK);
+      tc_store_tiles(stage0 + (s ^ 1) * kTcStageFloats, tid, regs);
+      if (it + 2 < nk) tc_load_tiles<VEC>(regs, tid, M, N, K, X, ldx, W, m0, n0, (it + 2) * TCK);
       asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
     }
     wgmma_wait<0>();
     wgmma_fence_acc(part);
 #pragma unroll
-    for (int i = 0; i < NT / 2; ++i) acc[i] += part[i];
+    for (int i = 0; i < TCN / 2; ++i) acc[i] += part[i];
     if (it + 1 < nk) __syncthreads();
   }
 
   // ---- epilogue: acc[4 i + 2 h + e] = Y[m0 + 64 g + 16 (warp % 4) + lane / 4 + 8 h][n0 + 8 i + 2 (lane % 4) + e]
-  if (!(dbg & 4)) {
-    const bool yvec = (ldy & 1) == 0 && (reinterpret_cast<uintptr_t>(Y) & 7) == 0;
+  const bool yvec = (ldy & 1) == 0 && (reinterpret_cast<uintptr_t>(Y) & 7) == 0;
 #pragma unroll
-    for (int i = 0; i < NT / 8; ++i) {
-      const int n = n0 + 8 * i + 2 * (lane & 3);
-      if (n >= N) continue;
-      const bool pair = n + 1 < N;
-      float b0 = 0.0f, b1 = 0.0f;
-      if (bias) { b0 += __ldg(bias + n); if (pair) b1 += __ldg(bias + n + 1); }
-      if (bias2) { b0 += __ldg(bias2 + n); if (pair) b1 += __ldg(bias2 + n + 1); }
+  for (int i = 0; i < TCN / 8; ++i) {
+    const int n = n0 + 8 * i + 2 * (lane & 3);
+    if (n >= N) continue;
+    const bool pair = n + 1 < N;
+    float b0 = 0.0f, b1 = 0.0f;
+    if (bias) { b0 += __ldg(bias + n); if (pair) b1 += __ldg(bias + n + 1); }
+    if (bias2) { b0 += __ldg(bias2 + n); if (pair) b1 += __ldg(bias2 + n + 1); }
 #pragma unroll
-      for (int h = 0; h < 2; ++h) {
-        const int m = m0 + g * 64 + (warp & 3) * 16 + (lane >> 2) + 8 * h;
-        if (m >= M) continue;
-        float o0 = acc[4 * i + 2 * h] + b0, o1 = acc[4 * i + 2 * h + 1] + b1;
-        if (ACT == 1) { o0 = fmaxf(o0, 0.0f); o1 = fmaxf(o1, 0.0f); }
-        float* y = Y + (size_t)m * ldy + n;
-        if (pair && yvec) {
-          *reinterpret_cast<float2*>(y) = make_float2(o0, o1);
-        } else {
-          y[0] = o0;
-          if (pair) y[1] = o1;
-        }
+    for (int h = 0; h < 2; ++h) {
+      const int m = m0 + g * 64 + (warp & 3) * 16 + (lane >> 2) + 8 * h;
+      if (m >= M) continue;
+      float o0 = acc[4 * i + 2 * h] + b0, o1 = acc[4 * i + 2 * h + 1] + b1;
+      if (ACT == 1) { o0 = fmaxf(o0, 0.0f); o1 = fmaxf(o1, 0.0f); }
+      float* y = Y + (size_t)m * ldy + n;
+      if (pair && yvec) {
+        *reinterpret_cast<float2*>(y) = make_float2(o0, o1);
+      } else {
+        y[0] = o0;
+        if (pair) y[1] = o1;
       }
     }
   }
 }
 
-static int g_gemm_mode = 1;   // 1 = wgmma 3xTF32 for the transformer (default), 0 = FP32 SIMT everywhere (A/B verification)
-// The trajectory predictor (MLP + LSTM, M = T*B rows, outputs integrated over T frames by the trajectory codec) stays on the
-// FP32 SIMT GEMM: its matrices are launch-latency sized and its per-frame heading error accumulates through the prefix sum.
-struct ScopedFp32Gemm {
-  int saved;
-  ScopedFp32Gemm() : saved(g_gemm_mode) { g_gemm_mode = 0; }
-  ~ScopedFp32Gemm() { g_gemm_mode = saved; }
-};
-
-// ---- weight operand images, keyed by (device pointer, N, K, tile width).  A cache belongs to whoever owns the weights: a
-// glamr_net keeps the images of its own tensors until it replaces one or is destroyed; glamr_linear_forward, whose W is a caller
-// buffer that may be rewritten in place between calls, builds its images for one call only.  g_wimg_cache is the cache of the
-// call in progress (NULL: no images).
-struct WImgKey {
-  const float* w; int N, K, NT;
-  bool operator<(const WImgKey& o) const { return w != o.w ? w < o.w : (N != o.N ? N < o.N : (K != o.K ? K < o.K : NT < o.NT)); }
-};
-using WImgCache = std::map<WImgKey, float*>;
-static WImgCache* g_wimg_cache = nullptr;
-static int g_wimg_enabled = -1;     // GLAMR_NET_WIMG=0|1 (default: GLAMR_DEFAULT_NET_WIMG)
-static void wimg_free(WImgCache& c) {   // the caller has made sure no queued work reads the images
-  for (auto& kv : c) cudaFree(kv.second);
-  c.clear();
-}
-struct ScopedWImgCache {
-  WImgCache* saved;
-  explicit ScopedWImgCache(WImgCache* c) : saved(g_wimg_cache) { g_wimg_cache = c; }
-  ~ScopedWImgCache() { g_wimg_cache = saved; }
-};
-template <int NT>
-static int wimg_get(cudaStream_t s, const float* W, int N, int K, const float** out) {
-  const WImgKey key{W, N, K, NT};
-  WImgCache& cache = *g_wimg_cache;
-  auto it = cache.find(key);
-  if (it != cache.end()) { *out = it->second; return GLAMR_OK; }
-  cudaStreamCaptureStatus cap = cudaStreamCaptureStatusNone;
-  cudaStreamIsCapturing(s, &cap);
-  if (cap != cudaStreamCaptureStatusNone) { *out = nullptr; return GLAMR_OK; }      // never allocate while a graph is being captured
-  const int ksteps = (K + TCK - 1) / TCK, tiles = (N + NT - 1) / NT;
-  float* img = nullptr;
-  GLAMR_CUDA_TRY(cudaMalloc(&img, (size_t)tiles * ksteps * 2 * TcCfg<NT>::kBTileFloats * sizeof(float)));
-  const size_t total = (size_t)tiles * ksteps * NT * TCK;
-  build_w_image_kernel<NT><<<(unsigned)((total + 255) / 256 < 1056 ? (total + 255) / 256 : 1056), 256, 0, s>>>(W, N, K, ksteps, img);
-  GLAMR_LAUNCH_CHECK();
-  cache[key] = img;
-  *out = img;
-  return GLAMR_OK;
-}
-
-template <int NT>
 static int gemm_tc_launch(cudaStream_t s, int M, int N, int K, const float* X, int ldx, const float* W, const float* b, const float* b2,
                           float* Y, int ldy, int act) {
   static bool attr = false;
-  constexpr size_t smem = TcCfg<NT>::kSmemBytes;
   if (!attr) {
-    GLAMR_CUDA_TRY(cudaFuncSetAttribute(gemm_tf32x3_wgmma_kernel<0, true, NT, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    GLAMR_CUDA_TRY(cudaFuncSetAttribute(gemm_tf32x3_wgmma_kernel<1, true, NT, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    GLAMR_CUDA_TRY(cudaFuncSetAttribute(gemm_tf32x3_wgmma_kernel<0, false, NT, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    GLAMR_CUDA_TRY(cudaFuncSetAttribute(gemm_tf32x3_wgmma_kernel<1, false, NT, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    GLAMR_CUDA_TRY(cudaFuncSetAttribute(gemm_tf32x3_wgmma_kernel<0, true, NT, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    GLAMR_CUDA_TRY(cudaFuncSetAttribute(gemm_tf32x3_wgmma_kernel<1, true, NT, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    GLAMR_CUDA_TRY(cudaFuncSetAttribute(gemm_tf32x3_wgmma_kernel<0, false, NT, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    GLAMR_CUDA_TRY(cudaFuncSetAttribute(gemm_tf32x3_wgmma_kernel<1, false, NT, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    GLAMR_CUDA_TRY(cudaFuncSetAttribute(gemm_tf32x3_wgmma_kernel<0, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kTcSmemBytes));
+    GLAMR_CUDA_TRY(cudaFuncSetAttribute(gemm_tf32x3_wgmma_kernel<1, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kTcSmemBytes));
+    GLAMR_CUDA_TRY(cudaFuncSetAttribute(gemm_tf32x3_wgmma_kernel<0, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kTcSmemBytes));
+    GLAMR_CUDA_TRY(cudaFuncSetAttribute(gemm_tf32x3_wgmma_kernel<1, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kTcSmemBytes));
     attr = true;
   }
-  if (g_wimg_enabled < 0) {
-    const char* e = getenv("GLAMR_NET_WIMG");
-    g_wimg_enabled = e ? atoi(e) : GLAMR_DEFAULT_NET_WIMG;
-  }
-  dim3 grid((N + NT - 1) / NT, (M + TCM - 1) / TCM);
+  const dim3 grid((N + TCN - 1) / TCN, (M + TCM - 1) / TCM);
   const bool vec = (K % 4 == 0) && (ldx % 4 == 0) && (((uintptr_t)X | (uintptr_t)W) % 16 == 0);
-  const float* img = nullptr;
-  if (g_wimg_enabled && g_wimg_cache) {
-    const int rc = wimg_get<NT>(s, W, N, K, &img);
-    if (rc) return rc;
-  }
-  auto go = [&](auto kernel, const float* wptr) {
-    kernel<<<grid, kTcThreads, smem, s>>>(M, N, K, X, ldx, wptr, b, b2, Y, ldy);
-  };
-  if (img) {
-    const bool xvec = (K % 4 == 0) && (ldx % 4 == 0) && ((uintptr_t)X % 16 == 0);
-    if (xvec) { if (act == 1) go(gemm_tf32x3_wgmma_kernel<1, true, NT, true>, img); else go(gemm_tf32x3_wgmma_kernel<0, true, NT, true>, img); }
-    else { if (act == 1) go(gemm_tf32x3_wgmma_kernel<1, false, NT, true>, img); else go(gemm_tf32x3_wgmma_kernel<0, false, NT, true>, img); }
-  } else if (vec) {
-    if (act == 1) go(gemm_tf32x3_wgmma_kernel<1, true, NT, false>, W); else go(gemm_tf32x3_wgmma_kernel<0, true, NT, false>, W);
+  auto go = [&](auto kernel) { kernel<<<grid, kTcThreads, kTcSmemBytes, s>>>(M, N, K, X, ldx, W, b, b2, Y, ldy); };
+  if (vec) {
+    if (act == 1) go(gemm_tf32x3_wgmma_kernel<1, true>); else go(gemm_tf32x3_wgmma_kernel<0, true>);
   } else {
-    if (act == 1) go(gemm_tf32x3_wgmma_kernel<1, false, NT, false>, W); else go(gemm_tf32x3_wgmma_kernel<0, false, NT, false>, W);
+    if (act == 1) go(gemm_tf32x3_wgmma_kernel<1, false>); else go(gemm_tf32x3_wgmma_kernel<0, false>);
   }
   GLAMR_LAUNCH_CHECK();
   return GLAMR_OK;
@@ -486,29 +349,12 @@ static int gemm_skinny_launch(cudaStream_t s, int M, int N, int K, const float* 
   return GLAMR_OK;
 }
 
-static int g_skinny = -1;       // GLAMR_NET_SKINNY=0 sends the small problems to the tile kernels again (A/B runs)
-static int gemm(cudaStream_t s, int M, int N, int K, const float* X, int ldx, const float* W, const float* b, const float* b2, float* Y,
-                int ldy, int act) {
-  if (g_skinny < 0) {
-    const char* e = getenv("GLAMR_NET_SKINNY");
-    g_skinny = e ? atoi(e) : 1;
-  }
-  if (g_skinny && M <= kSkinnyMaxM) return gemm_skinny_launch(s, M, N, K, X, ldx, W, b, b2, Y, ldy, act);
-  if (g_gemm_mode == 1) {
-    static int ntile = -1;     // GLAMR_TC_NTILE = 32 | 128 forces one tile shape (experiments); default: by problem height
-    if (ntile < 0) {
-#ifdef GLAMR_EXPERIMENT
-      if (const char* e = getenv("GLAMR_TC_DEBUG")) {
-        const int v = atoi(e);
-        GLAMR_CUDA_TRY(cudaMemcpyToSymbol(g_tc_dbg, &v, sizeof(int)));
-      }
-#endif
-      const char* t = getenv("GLAMR_TC_NTILE");
-      ntile = t ? atoi(t) : 0;
-    }
-    const bool narrow = ntile == 32 || (ntile != 128 && M <= TCM);
-    return narrow ? gemm_tc_launch<32>(s, M, N, K, X, ldx, W, b, b2, Y, ldy, act) : gemm_tc_launch<128>(s, M, N, K, X, ldx, W, b, b2, Y, ldy, act);
-  }
+// Arithmetic of a Linear with more than kSkinnyMaxM rows; smaller ones run the exact FP32 skinny kernel either way.
+enum GemmPrec { kTf32x3, kFp32 };
+static int gemm(cudaStream_t s, GemmPrec prec, int M, int N, int K, const float* X, int ldx, const float* W, const float* b, const float* b2,
+                float* Y, int ldy, int act) {
+  if (M <= kSkinnyMaxM) return gemm_skinny_launch(s, M, N, K, X, ldx, W, b, b2, Y, ldy, act);
+  if (prec == kTf32x3) return gemm_tc_launch(s, M, N, K, X, ldx, W, b, b2, Y, ldy, act);
   dim3 grid((N + GT - 1) / GT, (M + GT - 1) / GT);
   if (act == 1)
     gemm_bias_act_kernel<1><<<grid, 256, 0, s>>>(M, N, K, X, ldx, W, b, b2, Y, ldy);
@@ -737,7 +583,6 @@ using namespace glamr;
 struct glamr_net {
   std::map<std::string, std::pair<float*, size_t>> t;
   std::vector<void*> allocs;
-  mutable WImgCache wimg;           // operand images of this net's weights (GLAMR_NET_WIMG=1), built on first use
 };
 
 namespace {
@@ -798,11 +643,11 @@ int mha(cudaStream_t s, Arena& A, const AttnW& w, int B, int Sq, int Sk, const f
   float* att = A.take((size_t)Mq * 256);
   if (!q || !kv || !att) return GLAMR_ENOSPACE;
   int rc;
-  if ((rc = gemm(s, Mq, 256, 256, q_src, 256, w.in_w, w.in_b, nullptr, q, 256, 0))) return rc;
-  if ((rc = gemm(s, Mk, 512, 256, kv_src, 256, w.in_w + 256 * 256, w.in_b + 256, nullptr, kv, 512, 0))) return rc;
+  if ((rc = gemm(s, kTf32x3, Mq, 256, 256, q_src, 256, w.in_w, w.in_b, nullptr, q, 256, 0))) return rc;
+  if ((rc = gemm(s, kTf32x3, Mk, 512, 256, kv_src, 256, w.in_w + 256 * 256, w.in_b + 256, nullptr, kv, 512, 0))) return rc;
   attention_kernel<<<dim3(B, 8, (Sq + kAttnQChunk - 1) / kAttnQChunk), 128, 0, s>>>(B, Sq, Sk, q, 256, kv, kv + 256, 512, mask, att, 256);
   GLAMR_LAUNCH_CHECK();
-  if ((rc = gemm(s, Mq, 256, 256, att, 256, w.out_w, w.out_b, nullptr, out, 256, 0))) return rc;
+  if ((rc = gemm(s, kTf32x3, Mq, 256, 256, att, 256, w.out_w, w.out_b, nullptr, out, 256, 0))) return rc;
   A.used = mark;
   return GLAMR_OK;
 }
@@ -812,8 +657,8 @@ int ffn(cudaStream_t s, Arena& A, int M, const float* x, const float* l1w, const
   float* h = A.take((size_t)M * 512);
   if (!h) return GLAMR_ENOSPACE;
   int rc;
-  if ((rc = gemm(s, M, 512, 256, x, 256, l1w, l1b, nullptr, h, 512, 1))) return rc;
-  if ((rc = gemm(s, M, 256, 512, h, 512, l2w, l2b, nullptr, out, 256, 0))) return rc;
+  if ((rc = gemm(s, kTf32x3, M, 512, 256, x, 256, l1w, l1b, nullptr, h, 512, 1))) return rc;
+  if ((rc = gemm(s, kTf32x3, M, 256, 512, h, 512, l2w, l2b, nullptr, out, 256, 0))) return rc;
   A.used = mark;
   return GLAMR_OK;
 }
@@ -852,31 +697,10 @@ int decoder_layer(cudaStream_t s, Arena& A, const DecLayer& L, int B, int S, int
 
 // Y[M,N] = act(X[M,K] W[N,K]^T + bias) -- stand-alone entry for the GEMM used by every Linear of the prior networks
 // (nn.Linear in lib/models/mlp.py:32-41, nn.MultiheadAttention projections, FFN).  mode: 1 wgmma 3xTF32, 0 FP32 SIMT.
-// W is the caller's and may be rewritten between calls, so a weight image (GLAMR_NET_WIMG=1) is built for this call only; the
-// call then waits for its stream before it frees the image.
 extern "C" int glamr_linear_forward(int M, int N, int K, const float* X, const float* W, const float* bias, int relu, float* Y, int mode,
                                     void* stream) {
   if (M <= 0 || N <= 0 || K <= 0 || !X || !W || !Y) return GLAMR_EINVAL;
-  const int saved = g_gemm_mode;
-  g_gemm_mode = mode;
-  WImgCache images;
-  int rc;
-  {
-    ScopedWImgCache scope(&images);
-    rc = gemm((cudaStream_t)stream, M, N, K, X, K, W, bias, nullptr, Y, N, relu ? 1 : 0);
-  }
-  g_gemm_mode = saved;
-  if (!images.empty()) {
-    const cudaError_t e = cudaStreamSynchronize((cudaStream_t)stream);
-    wimg_free(images);
-    if (!rc && e != cudaSuccess) rc = (int)e;
-  }
-  return rc;
-}
-extern "C" int glamr_net_set_gemm_mode(int mode) {
-  if (mode != 0 && mode != 1) return GLAMR_EINVAL;
-  g_gemm_mode = mode;
-  return GLAMR_OK;
+  return gemm((cudaStream_t)stream, mode == 1 ? kTf32x3 : kFp32, M, N, K, X, K, W, bias, nullptr, Y, N, relu ? 1 : 0);
 }
 
 extern "C" int glamr_net_create(glamr_net** out) {
@@ -887,7 +711,6 @@ extern "C" int glamr_net_create(glamr_net** out) {
 extern "C" int glamr_net_destroy(glamr_net* n) {
   if (!n) return GLAMR_OK;
   cudaDeviceSynchronize();
-  wimg_free(n->wimg);
   for (void* p : n->allocs) cudaFree(p);
   delete n;
   return GLAMR_OK;
@@ -899,7 +722,6 @@ extern "C" int glamr_net_set_tensor(glamr_net* n, const char* name, const float*
   GLAMR_CUDA_TRY(cudaMalloc(&p, numel * sizeof(float)));
   GLAMR_CUDA_TRY(cudaMemcpy(p, host, numel * sizeof(float), cudaMemcpyHostToDevice));
   n->allocs.push_back(p);
-  if (n->t.count(name)) { cudaDeviceSynchronize(); wimg_free(n->wimg); }      // a weight was replaced: this net's images are stale
   n->t[name] = {(float*)p, numel};
   return GLAMR_OK;
 }
@@ -930,7 +752,6 @@ extern "C" int glamr_infiller_window_forward(const glamr_net* n, int B, const fl
   const float* pmw = W(n, dd + "p_z_mu_net.weight", 128 * 256, &e), * pmb = W(n, dd + "p_z_mu_net.bias", 128, &e);
   const float* plw = W(n, dd + "p_z_logvar_net.weight", 128 * 256, &e), * plb = W(n, dd + "p_z_logvar_net.bias", 128, &e);
   if (e) return GLAMR_EINVAL;
-  ScopedWImgCache images(&n->wimg);
   Arena A{workspace, workspace_floats, 0};
   const int S = 50, Sc = 30, M = S * B, Mc = Sc * B;
   float* x = A.take((size_t)M * 256);
@@ -947,10 +768,10 @@ extern "C" int glamr_infiller_window_forward(const glamr_net* n, int B, const fl
   if (!dec_out) return GLAMR_ENOSPACE;
   int rc;
   // ---- context encoder (motion_infiller_vae.py:92-123)
-  if ((rc = gemm(s, M, 256, 69, in_pose, 69, in_fc_w, in_fc_b, nullptr, x, 256, 0))) return rc;
+  if ((rc = gemm(s, kTf32x3, M, 256, 69, in_pose, 69, in_fc_w, in_fc_b, nullptr, x, 256, 0))) return rc;
   pe_concat_kernel<<<M, 128, 0, s>>>(M, B, 256, x, 256, 0, 0, 0, cat);
   GLAMR_LAUNCH_CHECK();
-  if ((rc = gemm(s, M, 256, 512, cat, 512, cpe_w, cpe_b, nullptr, x, 256, 0))) return rc;
+  if ((rc = gemm(s, kTf32x3, M, 256, 512, cat, 512, cpe_w, cpe_b, nullptr, x, 256, 0))) return rc;
   for (int l = 0; l < 2; ++l)
     if ((rc = encoder_layer(s, A, enc[l], B, S, x, key_pad_mask))) return rc;
   // ---- learned prior over z (:354-362): two tokens attend to the context
@@ -958,21 +779,21 @@ extern "C" int glamr_infiller_window_forward(const glamr_net* n, int B, const fl
   GLAMR_CUDA_TRY(cudaMemcpyAsync(tok + 256, lv_tok, 256 * sizeof(float), cudaMemcpyDeviceToDevice, s));
   pe_concat_kernel<<<2 * B, 128, 0, s>>>(2 * B, B, 256, tok, 256, 0, 1, 0, cat);
   GLAMR_LAUNCH_CHECK();
-  if ((rc = gemm(s, 2 * B, 256, 512, cat, 512, ppe_w, ppe_b, nullptr, px, 256, 0))) return rc;
+  if ((rc = gemm(s, kTf32x3, 2 * B, 256, 512, cat, 512, ppe_w, ppe_b, nullptr, px, 256, 0))) return rc;
   if ((rc = decoder_layer(s, A, pri, B, 2, S, px, x, key_pad_mask))) return rc;
-  if ((rc = gemm(s, B, 128, 256, px, 256, pmw, pmb, nullptr, mu, 128, 0))) return rc;
-  if ((rc = gemm(s, B, 128, 256, px + (size_t)B * 256, 256, plw, plb, nullptr, lv, 128, 0))) return rc;
+  if ((rc = gemm(s, kTf32x3, B, 128, 256, px, 256, pmw, pmb, nullptr, mu, 128, 0))) return rc;
+  if ((rc = gemm(s, kTf32x3, B, 128, 256, px + (size_t)B * 256, 256, plw, plb, nullptr, lv, 128, 0))) return rc;
   sample_z_kernel<<<(B * 128 + 127) / 128, 128, 0, s>>>(B, 128, mu, 128, lv, 128, eps, eps_rows == 1 ? 0 : 128, z);
   GLAMR_LAUNCH_CHECK();
   // ---- decoder (:383-395): z repeated over the 30 current frames, PE offset 10
   pe_concat_kernel<<<Mc, 128, 0, s>>>(Mc, B, 128, z, 128, 1, 0, 10, cat);
   GLAMR_LAUNCH_CHECK();
-  if ((rc = gemm(s, Mc, 256, 384, cat, 384, dpe_w, dpe_b, nullptr, dx, 256, 0))) return rc;
+  if ((rc = gemm(s, kTf32x3, Mc, 256, 384, cat, 384, dpe_w, dpe_b, nullptr, dx, 256, 0))) return rc;
   for (int l = 0; l < 2; ++l)
     if ((rc = decoder_layer(s, A, dec[l], B, Sc, S, dx, x, key_pad_mask))) return rc;
-  if ((rc = gemm(s, Mc, 512, 256, dx, 256, om0w, om0b, nullptr, h1, 512, 1))) return rc;
-  if ((rc = gemm(s, Mc, 256, 512, h1, 512, om1w, om1b, nullptr, h2, 256, 1))) return rc;
-  if ((rc = gemm(s, Mc, 69, 256, h2, 256, ofw, ofb, nullptr, dec_out, 69, 0))) return rc;
+  if ((rc = gemm(s, kTf32x3, Mc, 512, 256, dx, 256, om0w, om0b, nullptr, h1, 512, 1))) return rc;
+  if ((rc = gemm(s, kTf32x3, Mc, 256, 512, h1, 512, om1w, om1b, nullptr, h2, 256, 1))) return rc;
+  if ((rc = gemm(s, kTf32x3, Mc, 69, 256, h2, 256, ofw, ofb, nullptr, dec_out, 69, 0))) return rc;
   concat_time_kernel<<<64, 256, 0, s>>>(10, Sc, B, 69, in_pose, dec_out, out_pose);
   GLAMR_LAUNCH_CHECK();
   return GLAMR_OK;
@@ -1042,10 +863,10 @@ extern "C" int glamr_traj_local2global(int T, int B, const float* local_traj, in
 // The trajectory predictor's network for R independent rows of T frames (traj_pred_vae.py:72-92 context encoder, :281-297
 // prior + z, :298-333 decoder up to out_fc): in [T,R,69] -> raw [T,R,11], the decoder output before any frame-0 override.
 // eps [R or 1,128] (eps_rows = R or 1) or NULL (-> z = mu).  Scratch comes from A.  The single-pass and the windowed entry
-// points both run the network through here.
+// points both run the network through here.  Its Linears stay on the FP32 GEMMs: their matrices are launch-latency sized, and the
+// per-frame heading error accumulates through the codec's prefix sum.
 static int trajpred_network(const glamr_net* n, int T, int R, const float* in, const float* eps, int eps_rows, float* raw, Arena& A,
                             cudaStream_t s) {
-  ScopedFp32Gemm fp32_only;
   int e = 0;
   const std::string ce = "context_encoder.", dd = "data_decoder.";
   const float* im0w = W(n, ce + "in_mlp.affine_layers.0.weight", 512 * 69, &e), * im0b = W(n, ce + "in_mlp.affine_layers.0.bias", 512, &e);
@@ -1086,31 +907,31 @@ static int trajpred_network(const glamr_net* n, int T, int R, const float* in, c
     attr = true;
   }
   // ---- context encoder (traj_pred_vae.py:72-92)
-  if ((rc = gemm(s, M, 512, 69, in, 69, im0w, im0b, nullptr, h512, 512, 1))) return rc;
-  if ((rc = gemm(s, M, 256, 512, h512, 512, im1w, im1b, nullptr, x, 256, 1))) return rc;
+  if ((rc = gemm(s, kFp32, M, 512, 69, in, 69, im0w, im0b, nullptr, h512, 512, 1))) return rc;
+  if ((rc = gemm(s, kFp32, M, 256, 512, h512, 512, im1w, im1b, nullptr, x, 256, 1))) return rc;
   for (int l = 0; l < 2; ++l) {
     for (int d = 0; d < 2; ++d)   // xproj[t][b][d][:] = W_ih x + b_ih + b_hh
-      if ((rc = gemm(s, M, 512, 256, x, 256, wih[l][d], bih[l][d], bhh[l][d], xp + d * 512, 1024, 0))) return rc;
+      if ((rc = gemm(s, kFp32, M, 512, 256, x, 256, wih[l][d], bih[l][d], bhh[l][d], xp + d * 512, 1024, 0))) return rc;
     lstm_recurrence_kernel<<<dim3(R, 2), LG, lstm_smem, s>>>(T, R, xp, whh[l][0], whh[l][1], y);
     GLAMR_LAUNCH_CHECK();
     float* tmp = x; x = y; y = tmp;
   }
-  if ((rc = gemm(s, M, 512, 256, x, 256, cm0w, cm0b, nullptr, h512, 512, 1))) return rc;
-  if ((rc = gemm(s, M, 256, 512, h512, 512, cm1w, cm1b, nullptr, y, 256, 1))) return rc;      // y = context
+  if ((rc = gemm(s, kFp32, M, 512, 256, x, 256, cm0w, cm0b, nullptr, h512, 512, 1))) return rc;
+  if ((rc = gemm(s, kFp32, M, 256, 512, h512, 512, cm1w, cm1b, nullptr, y, 256, 1))) return rc;      // y = context
   // ---- prior + z (:281-297)
   mean_time_kernel<<<(R * 256 + 127) / 128, 128, 0, s>>>(T, R, 256, y, hm);
   GLAMR_LAUNCH_CHECK();
-  if ((rc = gemm(s, R, 512, 256, hm, 256, pm0w, pm0b, nullptr, hp, 512, 1))) return rc;
-  if ((rc = gemm(s, R, 256, 512, hp, 512, pm1w, pm1b, nullptr, hq, 256, 1))) return rc;
-  if ((rc = gemm(s, R, 256, 256, hq, 256, pzw, pzb, nullptr, pz, 256, 0))) return rc;
+  if ((rc = gemm(s, kFp32, R, 512, 256, hm, 256, pm0w, pm0b, nullptr, hp, 512, 1))) return rc;
+  if ((rc = gemm(s, kFp32, R, 256, 512, hp, 512, pm1w, pm1b, nullptr, hq, 256, 1))) return rc;
+  if ((rc = gemm(s, kFp32, R, 256, 256, hq, 256, pzw, pzb, nullptr, pz, 256, 0))) return rc;
   sample_z_kernel<<<(R * 128 + 127) / 128, 128, 0, s>>>(R, 128, pz, 256, pz + 128, 256, eps, eps_rows == 1 ? 0 : 128, z);
   GLAMR_LAUNCH_CHECK();
   // ---- decoder (:298-333)
   concat_z_kernel<<<256, 256, 0, s>>>(M, R, 128, 256, z, y, cat);
   GLAMR_LAUNCH_CHECK();
-  if ((rc = gemm(s, M, 512, 384, cat, 384, dm0w, dm0b, nullptr, h512, 512, 1))) return rc;
-  if ((rc = gemm(s, M, 256, 512, h512, 512, dm1w, dm1b, nullptr, x, 256, 1))) return rc;
-  return gemm(s, M, 11, 256, x, 256, ofw, ofb, nullptr, raw, 11, 0);
+  if ((rc = gemm(s, kFp32, M, 512, 384, cat, 384, dm0w, dm0b, nullptr, h512, 512, 1))) return rc;
+  if ((rc = gemm(s, kFp32, M, 256, 512, h512, 512, dm1w, dm1b, nullptr, x, 256, 1))) return rc;
+  return gemm(s, kFp32, M, 11, 256, x, 256, ofw, ofb, nullptr, raw, 11, 0);
 }
 
 // TrajPredVAE.inference (multi_step False, sample_num 1): joint positions -> local trajectory -> global trajectory.

@@ -107,11 +107,11 @@ int glamr_net_destroy(glamr_net_t* n);
 /* upload one named float32 parameter from a HOST pointer */
 int glamr_net_set_tensor(glamr_net_t* n, const char* name, const float* host, size_t numel);
 /* Y[M,N] = act(X[M,K] W[N,K]^T + bias): the GEMM behind every nn.Linear / attention projection / FFN of the prior
- * networks.  mode 1 (default inside the networks): tcgen05.mma.kind::tf32 with a 3xTF32 split (FP32-accurate), TMEM
- * accumulator; mode 0: FP32 SIMT kernel kept for A/B verification.  bias may be NULL. */
+ * networks.  M <= 256 runs an exact FP32 kernel in both modes.  Above that, mode 1 (the infiller's transformer) runs
+ * wgmma tf32 with a 3xTF32 split (FP32-accurate), its partial sums folded in FP32 at every K step of 32; mode 0 runs the
+ * FP32 SIMT tile kernel that the trajectory predictor uses.  bias may be NULL. */
 int glamr_linear_forward(int M, int N, int K, const float* X, const float* W, const float* bias, int relu, float* Y, int mode,
                          void* stream);
-int glamr_net_set_gemm_mode(int mode);
 size_t glamr_infiller_workspace_floats(int B);
 size_t glamr_trajpred_workspace_floats(int T, int B);
 /* One 50-frame window (past 10 | current 30 | future 10), B sequences, seq-first buffers:

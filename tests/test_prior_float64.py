@@ -19,9 +19,9 @@ term exceeds by orders of magnitude.
 C = 4, R = 8, FLOOR = 2^-24, ORIENT_FLOOR = 2^-20 (rotation-matrix elements) and C_LIN = 16 were set from measurements on an
 H100 80GB HBM3 at a 700 W power limit.  Worst measured |got - o64| / bound over the cases of each test:
 
-    linear layers, every variant       tensor cores 0.13, FP32 kernels 0.078 (a weight rewritten in place: 0.034)
+    linear layers                      tensor cores 0.13, FP32 kernels 0.077 (a weight rewritten in place: 0.034)
     one infiller window                0.14 at B <= 5 (FP32 skinny GEMMs), 0.32 at B >= 6 (tensor cores);
-                                       0.32 on the weight-image path with a second net destroyed between calls
+                                       0.30 with a second net destroyed between calls
     infiller sweep                     0.15 at B <= 3, 0.39 at 64 x 71
     trajectory predictor               local 0.36, trans 0.49, orient 0.25
     codec alone                        trans 0.011 / 7.9e-5, orient 0.33 / 0.0053 (local_heading 0 / 1)
@@ -37,10 +37,8 @@ eps 1e-6) and 2.5x (the encoder's first FFN layer as 2xTF32); the rest break it 
 The CPU tests apply the modelled bugs to the float32 oracle and print the factor by which each breaks the bound.
 """
 import gc
-import json
 import math
 import os
-import subprocess
 import sys
 
 import numpy as np
@@ -450,7 +448,7 @@ def run_linear_sweep():
     return res
 
 
-def run_stale_image():
+def run_weight_rewrite():
     """glamr_linear_forward, W rewritten in place between two calls: the second result must follow the new W"""
     lib = _lib()
     res = {}
@@ -490,7 +488,7 @@ WINDOW_B = (1, 5, 6, 9, 64)
 
 def run_window_cases(cases, net=None, between=None):
     """glamr_infiller_window_forward vs MotionInfiller.window in float64, per (B, mask, eps mode) case -> worst ratio per case.
-    between: called after each library call (the image-ownership check destroys another net there)"""
+    between: called after each library call (the two-nets check destroys another net there)"""
     from glamr_b200 import motion_traj as mt
     lib = _lib()
     if net is None:
@@ -525,13 +523,13 @@ def window_cases():
     return [(B, n, modes[(i + j) % 3]) for i, B in enumerate(WINDOW_B) for j, n in enumerate(names)]
 
 
-def run_image_ownership():
-    """the image path of the infiller window with two nets alive, one destroyed between calls: results must not change"""
+def run_two_nets():
+    """the infiller window with two nets alive, one destroyed between calls: results must not change"""
     from glamr_b200 import motion_traj as mt
     net = mt._Net(states()[0], torch.device(DEV))
     other = [mt._Net(states()[0], torch.device(DEV))]
     cases = [(1, 'random', 'rowsB'), (6, 'past_only', 'null'), (64, 'alternating', 'rows1')]
-    warm = run_window_cases(cases[:1], net=other[0])           # `other` builds images of its own weights
+    warm = run_window_cases(cases[:1], net=other[0])           # `other` runs once before it is destroyed
 
     def destroy_other():
         if other:
@@ -542,47 +540,28 @@ def run_image_ownership():
     return {**{'other ' + k: v for k, v in warm.items()}, **first, **{'again ' + k: v for k, v in again.items()}}
 
 
-def _child(what, env):
-    """run one of the variant functions in a fresh python process (the dispatch switches are read once per process)"""
-    e = dict(os.environ, **env)
-    e['PYTHONPATH'] = os.pathsep.join([REPO, os.path.join(REPO, 'tests')] + ([e['PYTHONPATH']] if e.get('PYTHONPATH') else []))
-    p = subprocess.run([sys.executable, os.path.abspath(__file__), what], env=e, capture_output=True, text=True, timeout=900)
-    assert p.returncode == 0, p.stdout[-3000:] + p.stderr[-3000:]
-    return json.loads(p.stdout.strip().splitlines()[-1])
-
-
-LINEAR_VARIANTS = {
-    'default': {},                                               # skinny (VEC and not) at M <= 256, wgmma NT=128 / FP32 tile above
-    'tiles': {'GLAMR_NET_SKINNY': '0'},                          # wgmma NT=32 at M <= 128, NT=128 above; FP32 tile everywhere
-    'nt32': {'GLAMR_NET_SKINNY': '0', 'GLAMR_TC_NTILE': '32'},
-    'nt128': {'GLAMR_NET_SKINNY': '0', 'GLAMR_TC_NTILE': '128'},
-    'wimg': {'GLAMR_NET_SKINNY': '0', 'GLAMR_NET_WIMG': '1'},     # pre-split weight image by bulk copy, NT=32 and 128
-}
-
-
 @pytest.mark.gpu
-@pytest.mark.parametrize('variant', list(LINEAR_VARIANTS))
-def test_linear_layers_match_float64(variant):
-    """every dispatch variant of the prior's Linear at shapes across every tile edge; Y is NaN before each call"""
-    res = _child('linear', LINEAR_VARIANTS[variant])
-    print(variant, res)
-    for k, v in res.items():
-        assert v <= 1.0, f'{variant} {k}: worst |y - y64| / bound = {v}'
-
-
-@pytest.mark.gpu
-def test_linear_weight_rewritten_in_place_is_not_served_stale():
-    """GLAMR_NET_WIMG=1: the weight image of a caller's buffer must not outlive the call"""
-    res = _child('stale', {'GLAMR_NET_SKINNY': '0', 'GLAMR_NET_WIMG': '1'})
+def test_linear_layers_match_float64():
+    """the prior's Linear at shapes across every dispatch edge, tensor cores and FP32; Y is NaN before each call"""
+    res = run_linear_sweep()
     print(res)
     for k, v in res.items():
         assert v <= 1.0, f'{k}: worst |y - y64| / bound = {v}'
 
 
 @pytest.mark.gpu
-def test_weight_images_belong_to_their_net():
-    """GLAMR_NET_WIMG=1: destroying one net leaves another net's images (and results) intact"""
-    res = _child('images', {'GLAMR_NET_SKINNY': '0', 'GLAMR_NET_WIMG': '1'})
+def test_linear_weight_rewritten_in_place_is_not_served_stale():
+    """W is the caller's buffer: a call must read the values W holds at that call"""
+    res = run_weight_rewrite()
+    print(res)
+    for k, v in res.items():
+        assert v <= 1.0, f'{k}: worst |y - y64| / bound = {v}'
+
+
+@pytest.mark.gpu
+def test_destroying_one_net_leaves_another_intact():
+    """destroying one net leaves another net's weights (and results) intact"""
+    res = run_two_nets()
     print(res)
     for k, v in res.items():
         assert v <= 1.0, f'{k}: worst |o - o64| / bound = {v}'
@@ -760,9 +739,3 @@ def test_graph_replay_is_bit_identical_to_eager(cuda_prior):
             assert all(e['graph'] is not None for e in list(mf.graphs.entries.values()) + list(tp.graphs.entries.values()))
     finally:
         mf.graphs, tp.graphs = saved
-
-
-if __name__ == '__main__':          # the variants that need their own process (dispatch switches in the environment)
-    torch.set_num_threads(max(1, min(8, os.cpu_count() or 1)))
-    fn = {'linear': run_linear_sweep, 'stale': run_stale_image, 'images': run_image_ownership}[sys.argv[1]]
-    print(json.dumps(fn()))

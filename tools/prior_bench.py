@@ -1,7 +1,6 @@
 """BASELINE config 3: motion_infiller + traj_pred inference, batch 64 x 120-frame sequences, 1 GPU (ms per batch)."""
-import ctypes, os, sys, time, torch
+import os, sys, time, torch
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
-from glamr_b200 import lib as L
 from glamr_b200.motion_traj import MotionTrajJointModel
 from glamr_b200.smpl import SMPL
 from glamr_b200.synthetic import make_smpl_assets
@@ -13,12 +12,8 @@ g = torch.Generator().manual_seed(0)
 pose = (torch.randn(B, T, 69, generator=g) * 0.3).to(dev); mask = torch.ones(B, T, device=dev); mask[:, 40:70] = 0
 nw = -(-(T - 10) // 30)
 batch = {'in_body_pose': pose * mask[..., None], 'frame_mask': mask, 'in_motion_latent': torch.randn(nw, 128, generator=g).to(dev), 'in_traj_latent': torch.randn(1, 128, generator=g).to(dev)}
-res = {}
-for mode in (1, 0):
-    L.load().glamr_net_set_gemm_mode(mode)
-    for _ in range(3): out = m.inference(batch)
-    torch.cuda.synchronize(); t0 = time.perf_counter()
-    for _ in range(10): out = m.inference(batch)
-    torch.cuda.synchronize(); res[mode] = ((time.perf_counter() - t0) / 10 * 1e3, out)
-d = (res[1][1]['infer_out_body_pose'] - res[0][1]['infer_out_body_pose']).abs().max().item()
-print(f'B={B} T={T}: wgmma 3xTF32 {res[1][0]:.2f} ms/batch, FP32 SIMT {res[0][0]:.2f} ms/batch, max |pose diff| {d:.2e}')
+for _ in range(3): m.inference(batch)
+torch.cuda.synchronize(); t0 = time.perf_counter()
+for _ in range(10): m.inference(batch)
+torch.cuda.synchronize()
+print(f'B={B} T={T}: {(time.perf_counter() - t0) / 10 * 1e3:.2f} ms/batch')
