@@ -61,7 +61,8 @@ NITERS = 4                      # Adam steps per stage before the second check p
 DEV = 'cuda:0'
 WHOLE = {'traj_local_xy', 'traj_local_heading', 'cam_rot_6d_fix', 'cam_trans_fix'}
 PERSON_VARS = ['traj_local_xy', 'traj_local_heading', 'traj_local_dxy', 'traj_local_dheading', 'traj_local_z', 'traj_local_rot',
-               'smpl_orient_world_res', 'root_trans_world_res', 'world_dheading', 'world_dxy']
+               'smpl_orient_world_res', 'root_trans_world_res', 'world_dheading', 'world_dxy', 'person2cam_res_rot',
+               'person2cam_res_trans']
 GLOBAL_ROWS = {'smpl_orient_world_res', 'root_trans_world_res', 'world_dheading', 'world_dxy'}   # rows are frames t of the sequence
 
 GOLDEN = ['dynamic_p1_t300', 'static_multi_p4_t300', '3dpw_p1_t600_gaps']
@@ -87,10 +88,22 @@ def _is_vec(cfg):
 
 def oracle_for(cfg):
     from oracle.global_opt import OracleGlobalRecon
+    g = cfg.grecon_model_specs
     if _is_vec(cfg) or any('world_dxy' in st['opt_variables'] for st in cfg.opt_stage_specs.values()):
         from traj_variable_cases import oracle_class
         return oracle_class()
+    if g.get('flag_traj_from_cam', False):
+        import traj_source_cases
+        return traj_source_cases.oracle_class()
+    if g.get('flag_opt_person2cam_rot', False) or g.get('flag_opt_person2cam_trans', False):
+        import person2cam_cases
+        return person2cam_cases.oracle_class()
     return OracleGlobalRecon
+
+
+def p2c_flags(model):
+    """(flag_opt_person2cam_rot, flag_opt_person2cam_trans) of an oracle or GlobalReconOptimizer"""
+    return (getattr(model, 'flag_opt_person2cam_rot', False), getattr(model, 'flag_opt_person2cam_trans', False))
 
 
 def synthetic_in_dict(assets, name):
@@ -126,8 +139,9 @@ def case(name, assets):
     return cfg, in_dict, make_prior
 
 
-def param_order(opt_variables, P, fixed_cam, opt_traj=True):
-    """(person or None, name) of every tensor get_parameter returns, in its order (global_recon_model.py:591-633)"""
+def param_order(opt_variables, P, fixed_cam, opt_traj=True, p2c=(False, False)):
+    """(person or None, name) of every tensor get_parameter returns, in its order (global_recon_model.py:591-633); p2c: the
+    person2cam flags (p2c_flags), a residual being returned when its flag is set and the stage lists it"""
     if 'cam' not in opt_variables:
         order = [(None, 'cam_inv_rot_residual'), (None, 'cam_inv_trans_residual')]
     elif fixed_cam:
@@ -141,6 +155,9 @@ def param_order(opt_variables, P, fixed_cam, opt_traj=True):
                     order += [(p, 'smpl_orient_world_res'), (p, 'root_trans_world_res')]
                 if 'local' in key:
                     order.append((p, f'traj_{key}'))
+        for flag, key in zip(p2c, ('rot', 'trans')):
+            if flag and f'person2cam_{key}' in opt_variables:
+                order.append((p, f'person2cam_res_{key}'))
         if 'world_dheading' in opt_variables:
             order.append((p, 'world_dheading'))
         if 'world_dxy' in opt_variables:
@@ -185,7 +202,7 @@ def oracle_closure(Oracle, cfg, assets, state, specs, stage, lay, theta, dtype):
         data = ora.to_float64(data)
     variables = specs['opt_variables']
     params = ora.get_parameter(data, variables)
-    order = param_order(variables, len(data['person_data']), ora.flag_fixed_cam, ora.flag_opt_traj)
+    order = param_order(variables, len(data['person_data']), ora.flag_fixed_cam, ora.flag_opt_traj, p2c_flags(ora))
     assert len(order) == len(params)
     th = theta.detach().cpu()
     with torch.no_grad():
@@ -286,6 +303,9 @@ def check_terms(what, terms, ref, report=None):
 
 # ------------------------------------------------------------------------------------------------ CPU: host emulator
 def _emu_runner(ora, data):
+    if any(p2c_flags(ora)):
+        from test_person2cam import _emu_runner as make
+        return make(ora, data)
     if not hasattr(ora, 'heading_type'):
         from emu_runner import EmuRunner
         return EmuRunner(ora, data)
@@ -293,11 +313,12 @@ def _emu_runner(ora, data):
     return make(ora, data)
 
 
-def emulator_records(name, assets):
+def emulator_records(name, assets, setup=case):
     """the host-compiled frame functions (tests/emu_runner.py) from the oracle's float32 init: first closure of every stage
-    and the closure after the stage's Adam steps, each with the oracle's float64 / float32 gradients at the same state"""
+    and the closure after the stage's Adam steps, each with the oracle's float64 / float32 gradients at the same state (kept as
+    r['state']); setup(name, assets) -> (cfg, in_dict, prior factory) of the case"""
     from glamr_b200 import lib as L
-    cfg, in_dict, make_prior = case(name, assets)
+    cfg, in_dict, make_prior = setup(name, assets)
     Oracle = oracle_for(cfg)
     ora_t = Oracle(copy.deepcopy(cfg), assets, mt_model=make_prior('cpu'))
     template = ora_t.init_data(copy.deepcopy(in_dict))
@@ -310,7 +331,7 @@ def emulator_records(name, assets):
     recs = []
     for stage, specs in cfg.opt_stage_specs.items():
         variables = specs['opt_variables']
-        order = param_order(variables, P, ora_e.flag_fixed_cam, ora_e.flag_opt_traj)
+        order = param_order(variables, P, ora_e.flag_fixed_cam, ora_e.flag_opt_traj, p2c_flags(ora_e))
         run.set_stage(variables, specs['loss_cfg'], stage)
         for point in ('first', 'stepped'):
             if point == 'stepped':
@@ -323,7 +344,8 @@ def emulator_records(name, assets):
             ref = references(Oracle, cfg, assets, state, specs, stage, run.layout, run.theta)
             recs.append({'stage': stage, 'point': point, 'order': order,
                          'grads': [view(run.layout, grad, p, n).numpy().astype(np.float64) for p, n in order],
-                         'terms': {k: float(terms[L.TERM_INDEX[k]]) for k in specs['loss_cfg']}, 'ref': ref,
+                         'terms': {k: float(terms[L.TERM_INDEX[k]]) for k in specs['loss_cfg']}, 'ref': ref, 'state': state,
+                         'specs': specs, 'layout': run.layout, 'theta': run.theta.clone(),
                          'starts': [int(d['fr_start']) for d in data_e['person_data'].values()],
                          'lens': [int(d['exist_len']) for d in data_e['person_data'].values()]})
         cam = run.buffer(L.R_CAM_POSE).view(T, 3, 4)
@@ -540,11 +562,11 @@ def _snapshot(data):
     return out
 
 
-def gpu_run(name, assets):
+def gpu_run(name, assets, setup=case):
     """first closure of every stage and the closure after its Adam steps on the CUDA path: packed gradients, term values,
     theta and the state the oracle needs"""
     from glamr_b200 import lib as L
-    cfg, in_dict, make_prior = case(name, assets)
+    cfg, in_dict, make_prior = setup(name, assets)
     model = _make_model(cfg, assets, make_prior(DEV))
     data = _init(model, in_dict)
     P = len(data['person_data'])
@@ -559,7 +581,7 @@ def gpu_run(name, assets):
                 model._set_stage(data, variables, specs['loss_cfg'], stage, reset_adam=False)
             grad, terms = _closure(model)
             recs.append({'stage': stage, 'point': point, 'specs': specs,
-                         'order': param_order(variables, P, model.flag_fixed_cam, model.flag_opt_traj),
+                         'order': param_order(variables, P, model.flag_fixed_cam, model.flag_opt_traj, p2c_flags(model)),
                          'grad': grad[:model._layout.n_params].cpu(), 'sums': grad[model._layout.n_params:].cpu(),
                          'terms': {k: float(terms[L.TERM_INDEX[k]]) for k in specs['loss_cfg']},
                          'theta': model._theta.detach().cpu().clone(), 'state': _snapshot(data)})
@@ -570,10 +592,10 @@ def gpu_run(name, assets):
     return model, cfg, recs
 
 
-def _references_of(name, cfg, assets, lay, recs, template=None):
+def _references_of(name, cfg, assets, lay, recs, template=None, setup=case):
     """the oracle's float64 / float32 references at the theta and state of each record (r['ref']), and the record's gradient
     split into its variables (r['grads']); -> the oracle's init data, re-usable as `template`"""
-    _, in_dict, make_prior = case(name, assets)
+    _, in_dict, make_prior = setup(name, assets)
     Oracle = oracle_for(cfg)
     if template is None:
         template = Oracle(copy.deepcopy(cfg), assets, mt_model=make_prior('cpu')).init_data(copy.deepcopy(in_dict))
