@@ -17,7 +17,7 @@ REL_SO_PATH = os.path.join(HERE, 'libglamr_b200.so')
 SO_PATH = os.environ.get('GLAMR_B200_SO') or REL_SO_PATH
 EXP_SO_PATH = os.path.join(HERE, 'libglamr_b200_exp.so')
 CSRC = os.path.join(HERE, 'csrc')
-SOURCES = ['smpl_kernels.cu', 'globalopt_kernels.cu', 'c_api.cu', 'nets_kernels.cu', 'eval_kernels.cu']
+SOURCES = ['smpl_kernels.cu', 'globalopt_kernels.cu', 'c_api.cu', 'nets_kernels.cu', 'eval_kernels.cu', 'init_kernels.cu']
 NUM_TERMS = 21
 
 TERM_INDEX = {
@@ -37,6 +37,8 @@ TRAJ_PREDICTED, TRAJ_BASE = 0, 1          # enum glamr_traj_source
  ROP_QUAT_MUL, ROP_ROTMAT_TO_AA, ROP_QUAT_TO_ROTMAT, ROP_SAFE_ATAN2, ROP_PROJECT, ROP_MAT3_MUL) = range(12)
 ROP_DIMS = {0: (3, 0, 9), 1: (3, 0, 9), 2: (6, 0, 9), 3: (9, 0, 4), 4: (4, 0, 3), 5: (3, 0, 4), 6: (4, 4, 4), 7: (9, 0, 3),
             8: (4, 0, 9), 9: (2, 0, 1), 10: (3, 9, 2), 11: (9, 9, 9)}
+
+FILL_F32, FILL_F64, FILL_F32_W64 = 0, 1, 2   # GLAMR_FILL_*
 
 _fp = ctypes.POINTER(ctypes.c_float)
 _vp = ctypes.c_void_p
@@ -68,6 +70,10 @@ class Problem(ctypes.Structure):
                [(n, _vp) for n in
                 ['persons', 'groups', 'smpl_pose_all', 'smpl_beta_all', 'scale_all', 'cam_pose_const', 'empty_index', 'fill_src',
                  'inv_num_persons', 'rel_target', 'rel_w', 'rel_wt', 'active']]
+
+
+class FillJob(ctypes.Structure):
+    _fields_ = [('src', _vp), ('dst', _vp)] + [(n, ctypes.c_int32) for n in ['person', 'C', 'src_stride', 'src_col0', 'kind', 'interp', 'rows']]
 
 
 class GlamrError(RuntimeError):
@@ -121,6 +127,7 @@ def load():
     lib.glamr_smpl_fk_workspace_bytes.restype = ctypes.c_size_t
     lib.glamr_sizeof_person.restype = ctypes.c_size_t
     lib.glamr_sizeof_problem.restype = ctypes.c_size_t
+    lib.glamr_sizeof_fill_job.restype = ctypes.c_size_t
     lib.glamr_opt_reduce_count.restype = ctypes.c_size_t
     lib.glamr_opt_peer_bytes.restype = ctypes.c_size_t
     lib.glamr_fp32_probe.argtypes = [ctypes.c_int, _vp, ctypes.c_size_t, _vp, _vp]
@@ -134,7 +141,13 @@ def load():
     lib.glamr_allreduce_inplace.argtypes = [_vp, _vp, ctypes.c_size_t, _vp]
     lib.glamr_opt_apply.argtypes = [_vp, _vp, _vp, ctypes.c_double, _vp, ctypes.c_int, _vp]
     lib.glamr_opt_iterate.argtypes = [_vp, _vp, _vp, ctypes.c_double, _vp, ctypes.c_int, ctypes.c_int, ctypes.c_int, _vp]
-    if lib.glamr_sizeof_person() != ctypes.sizeof(Person) or lib.glamr_sizeof_problem() != ctypes.sizeof(Problem):
+    lib.glamr_init_rotvec.argtypes = [ctypes.c_int, _vp, ctypes.c_int, _vp, _vp, _vp, _vp]
+    lib.glamr_init_vis_tables.argtypes = [ctypes.c_int, ctypes.c_int, _vp, _vp, _vp, _vp, _vp, _vp]
+    lib.glamr_init_fill.argtypes = [ctypes.c_int, _vp, ctypes.c_int, ctypes.c_int, _vp, _vp, _vp, _vp]
+    lib.glamr_init_filter_pose.argtypes = [ctypes.c_int, ctypes.c_int, ctypes.c_int, _vp, _vp, _vp, _vp, ctypes.c_double, ctypes.c_double,
+                                           _vp, _vp]
+    if lib.glamr_sizeof_person() != ctypes.sizeof(Person) or lib.glamr_sizeof_problem() != ctypes.sizeof(Problem) or \
+            lib.glamr_sizeof_fill_job() != ctypes.sizeof(FillJob):
         raise GlamrError('struct layout mismatch between include/glamr_b200.h and glamr_b200/lib.py')
     _lib = lib
     return lib

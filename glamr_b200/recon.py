@@ -6,9 +6,11 @@ Same constructor, ``optimize(in_dict, continue_opt=False) -> dict`` (numpy), ``i
 ``optimize_seeds(in_dict, seeds) -> [dict]`` runs several seeds of one sequence as one problem, and
 ``optimize_batch(in_dicts, seeds) -> [[dict]]`` every (sequence, seed) pair of several sequences (groups, see glamr_b200/problem.py):
 every pair's result is the one ``optimize`` gives for that sequence and seed.
-Host Python does what the reference does on the host (dict bookkeeping, SciPy rotation-vector conversion and linear
-gap interpolation, log lines); every formula of the per-iteration path -- trajectory codec, camera, SMPL, projection,
-residuals, analytic backward, Adam -- is a kernel of glamr_b200/csrc.  No autograd, no CPU fallback.
+Every array of an ``in_dict['est']`` pose_dict (bboxes_dict.exist, smpl_pose_quat_wroot, smpl_beta, root_trans, kp_2d, cam_K) may be
+a numpy array or a torch tensor on the CPU or a GPU; the data dict and the output are the same for either.  ``init_data``'s per-frame
+work (rotation vectors, gap interpolation, filter_pose) runs in kernels for all persons at once, after one upload and with one
+read-back; host Python keeps the dict bookkeeping and the log lines.  Every formula of the per-iteration path -- trajectory codec,
+camera, SMPL, projection, residuals, analytic backward, Adam -- is a kernel of glamr_b200/csrc.  No autograd, no CPU fallback.
 """
 import copy
 import ctypes
@@ -16,7 +18,6 @@ import time
 
 import numpy as np
 import torch
-from scipy.interpolate import interp1d
 
 from . import geometry as G
 from . import lib as L
@@ -153,6 +154,77 @@ def rotmats_to_rotvec(mats):
     return np.ascontiguousarray((scale * q[:3]).T)
 
 
+class _Slot:
+    def __init__(self, i):
+        self.i = i
+
+
+def _torch_dtype(np_dtype):
+    return torch.from_numpy(np.zeros(0, np_dtype)).dtype
+
+
+class _Upload:
+    """Host arrays packed into one pinned buffer and sent to the device with one non-blocking copy; CUDA tensors are used
+    where they are.  source() returns the tensor or a slot; get() the device tensor of either once allocate() ran."""
+
+    def __init__(self):
+        self._host, self._nbytes, self._views, self._dev = [], 0, None, None
+
+    def source(self, x, device):
+        if isinstance(x, torch.Tensor):
+            if x.is_cuda:
+                return x.detach().to(device)
+            x = x.detach().numpy()
+        return self._add(np.ascontiguousarray(x))
+
+    def _add(self, a):
+        off = (self._nbytes + 15) // 16 * 16
+        self._host.append((a, off))
+        self._nbytes = off + a.nbytes
+        return _Slot(len(self._host) - 1)
+
+    def reserve(self, nbytes):
+        return self._add(np.zeros(nbytes, np.uint8))
+
+    def host(self, h):
+        return self._host[h.i][0]
+
+    def shape(self, h):
+        return tuple(h.shape) if isinstance(h, torch.Tensor) else self._host[h.i][0].shape
+
+    def dtype(self, h):
+        return h.dtype if isinstance(h, torch.Tensor) else _torch_dtype(self._host[h.i][0].dtype)
+
+    def numel(self, h):
+        return h.numel() if isinstance(h, torch.Tensor) else self._host[h.i][0].size
+
+    def allocate(self, device):
+        self._dev = torch.empty(max(self._nbytes, 16), dtype=torch.uint8, device=device)
+        self._views = [self._dev[off:off + a.nbytes].view(_torch_dtype(a.dtype)).view(a.shape) for a, off in self._host]
+
+    def get(self, h):
+        return h if isinstance(h, torch.Tensor) else self._views[h.i]
+
+    def fill(self, h, data):
+        self._host[h.i][0][:] = np.frombuffer(data, np.uint8)
+
+    def send(self):
+        buf = torch.empty(self._dev.shape, dtype=torch.uint8, pin_memory=True)
+        hb = buf.numpy()
+        for a, off in self._host:
+            hb[off:off + a.nbytes] = a.reshape(-1).view(np.uint8)
+        self._dev.copy_(buf, non_blocking=True)
+
+
+def _upload_index(arrays, device):
+    """int64 index arrays -> device tensors with one pinned non-blocking copy"""
+    up = _Upload()
+    slots = [up.source(np.asarray(a, np.int64), device) for a in arrays]
+    up.allocate(device)
+    up.send()
+    return [up.get(h) for h in slots]
+
+
 def _sec_to_time(secs):
     secs = int(secs)
     return f'{secs // 3600}:{(secs % 3600) // 60:02d}:{secs % 60:02d}'
@@ -228,6 +300,7 @@ class GlobalReconOptimizer:
             self.load_model()
         self._lib = L.load()
         self._opt = None
+        self._consts = {}
         self.iter_ms = []              # (stage, niters, ms per iteration) of every optimize_main call
 
     def load_model(self):
@@ -243,76 +316,175 @@ class GlobalReconOptimizer:
                                               'flag_opt_person2cam_trans']}
 
     # ------------------------------------------------------------------------------------------------ init_data
-    def _person_from_estimate(self, est, gt_entry):
-        """global_recon_model.py:88-137 (host side, numpy/SciPy exactly as the reference)"""
-        d = {}
-        visible = est['bboxes_dict']['exist'].copy()
-        d['visible'] = visible
-        d['visible_orig'] = visible.copy()
-        where = np.where(visible)[0]
-        start, end = where[0], where[-1] + 1
-        d['fr_start'], d['fr_end'] = start, end
-        exist = visible == 1
-        exist[start:end] = True
-        d['exist_frames'] = exist
-        d['exist_len'] = end - start
-        d['max_len'] = n = visible.shape[0]
-        d['frames'] = np.arange(n)
-        d['vis_frames'] = vis = visible == 1
-        d['invis_frames'] = visible == 0
-        d['frame2ind'] = {f: i for i, f in enumerate(d['frames'])}
-        d['scale'] = None
-        rotmats = est['smpl_pose_quat_wroot']
-        nv = rotmats.shape[0]
-        aa = rotmats_to_rotvec(rotmats).reshape(nv, -1, 3).astype(np.float32)
-        d['smpl_pose'] = aa[:, 1:].reshape(-1, 69)
-        if gt_entry is not None:
-            d['smpl_pose_gt'] = gt_entry['pose'][:, 3:]
-        d['smpl_beta'] = est['smpl_beta']
-        d['smpl_orient_cam'] = aa[:, 0]
-        d['root_trans_cam'] = est['root_trans']
-        j2d = est['kp_2d'][:, :24]
-        j2d = np.concatenate([j2d, np.ones_like(j2d[:, :, :1])], axis=-1)
-        kp = np.zeros((int(vis.sum()), 26, 3))
-        kp[:, SMPL_TO_BODY26FK[:, 0]] = j2d[:, SMPL_TO_BODY26FK[:, 1]]
-        d['kp_2d'], d['kp_2d_score'] = kp[:, :, :2], kp[:, :, 2]
-        d['kp_2d_aligned'] = d['kp_2d'].copy()
-        d['cam_K'] = est['cam_K'].astype(np.float32)
-        if not np.all(visible):
-            for key in ['kp_2d', 'kp_2d_score', 'kp_2d_aligned', 'cam_K']:
-                full = np.zeros((n,) + d[key].shape[1:], dtype=d[key].dtype)
-                full[vis] = d[key]
-                d[key] = full
-            vis_ind = np.where(visible)[0].astype(np.float32)
-            for key in ['smpl_pose', 'smpl_beta', 'root_trans_cam', 'smpl_orient_cam']:
-                f = interp1d(vis_ind, d[key], axis=0, assume_sorted=True, fill_value='extrapolate')
-                d[key] = f(np.arange(n, dtype=np.float32))
-        return tensor_to(d, self.device)
+    def _const(self, key, values):
+        """small constant tensor on the device, uploaded once per optimiser"""
+        c = self._consts.get(key)
+        if c is None:
+            c = self._consts[key] = torch.tensor(values, device=self.device)
+        return c
 
-    def filter_pose(self, d):
-        """:250-271"""
-        visible = d['visible']
-        q = G.angle_axis_to_quaternion(d['smpl_orient_cam'].float())
-        jump = G.quat_angle_diff(q[1:], q[:-1])
-        ind = (torch.where((jump > np.pi / 3) & visible[1:].bool())[0] + 1).tolist()
-        for i in ind:
-            if visible[i - 1]:
-                if i + 1 < q.shape[0] and visible[i + 1] and (i + 1) not in ind:
-                    visible[i - 1] = 0
-                else:
-                    visible[i] = 0
-        if self.flag_make_invis_with_keypoint:
-            vis_ind = torch.where(visible == 1.0)[0]
-            nvalid = (d['kp_2d_score'][vis_ind] > self.make_invis_keypoint_min_score).sum(dim=1)
-            visible[vis_ind[nvalid < self.make_invis_keypoint_min_num]] = 0.0
-        d['vis_frames'] = visible == 1
-        d['invis_frames'] = visible == 0
+    def _persons_from_estimates(self, in_dict, num_fr):
+        """global_recon_model.py:88-137 and filter_pose (:250-271) for every person of the sequence on the device: the host
+        arrays of all persons go up in one pinned copy, the rotation vectors, gap fill and filter_pose run as one launch each
+        for all persons, and one read-back brings the visibility the host needs for its index tables.  Estimates may be
+        numpy arrays or torch tensors (CPU or CUDA); the person dicts equal those of the numpy path."""
+        dev, T = self.device, num_fr
+        keys = list(in_dict['est'].keys())
+        P = len(keys)
+        up = _Upload()
+        srcs = []
+        for idx in keys:
+            est = in_dict['est'][idx]
+            gt = in_dict['gt'].get(idx)
+            s = {n: up.source(x, dev) for n, x in [('exist', est['bboxes_dict']['exist']), ('rot', est['smpl_pose_quat_wroot']),
+                                                    ('beta', est['smpl_beta']), ('trans', est['root_trans']), ('kp', est['kp_2d']),
+                                                    ('K', est['cam_K'])]}
+            if gt is not None:
+                s['gt'] = up.source(gt['pose'][:, 3:], dev)
+            srcs.append(s)
+        for idx, s in zip(keys, srcs):
+            nv = up.shape(s['rot'])[0]
+            if up.shape(s['exist'])[0] != T:
+                raise ValueError(f'person {idx}: bboxes_dict.exist has {up.shape(s["exist"])[0]} frames, person 0 has {T}')
+            if nv == 0 or (nv < T and nv < 2):
+                raise ValueError(f'person {idx}: {nv} visible frames; filling the invisible frames needs at least two')
+            ex = s['exist']
+            if not isinstance(ex, torch.Tensor) and np.count_nonzero(up.host(ex)) != nv:
+                raise ValueError(f'person {idx}: bboxes_dict.exist marks {np.count_nonzero(up.host(ex))} frames visible, the estimates have {nv} rows')
+            for n in ('beta', 'trans'):
+                if up.dtype(s[n]) not in (torch.float32, torch.float64):
+                    raise TypeError(f'person {idx}: {n} must be float32 or float64, got {up.dtype(s[n])}')
+        nvs = [up.shape(s['rot'])[0] for s in srcs]
+        s0 = np.concatenate([[0], np.cumsum(nvs)]).astype(np.int64)
+        J = up.numel(srcs[0]['rot']) // (nvs[0] * 9)
+        jobs_slot = up.reserve(8 * P * ctypes.sizeof(L.FillJob))
+        up.allocate(dev)
+        get = up.get
+        f32, f64 = torch.float32, torch.float64
+        exists = [get(s['exist']) for s in srcs]
+        rot_dt = f64 if any(get(s['rot']).dtype != f32 for s in srcs) else f32
+        N = int(s0[-1]) * J
+        rot_all = torch.empty((N, 9), dtype=rot_dt, device=dev)
+        after_send = [lambda: [rot_all[s0[p] * J:s0[p + 1] * J].copy_(get(s['rot']).reshape(-1, 9)) for p, s in enumerate(srcs)]]
+        aa_all = torch.empty((N, 3), device=dev)
+        flags = torch.empty(N, dtype=torch.uint8, device=dev)
+        rb = torch.zeros(1 + 3 * P + P * T, dtype=torch.int32, device=dev)
+        pose_all = torch.empty((P, T, (J - 1) * 3), device=dev)
+        orient_all = torch.empty((P, T, 3), device=dev)
+        kp_all = torch.empty((P, T, 26, 2), dtype=f64, device=dev)
+        score_all = torch.empty((P, T, 26), dtype=f64, device=dev)
+        aligned_all = torch.empty((P, T, 26, 2), dtype=f64, device=dev)
+        K_all = torch.empty((P, T) + tuple(up.shape(srcs[0]['K'])[1:]), device=dev)
+        m0, m1 = self._const('kp_dst', SMPL_TO_BODY26FK[:, 0].tolist()), self._const('kp_src', SMPL_TO_BODY26FK[:, 1].tolist())
+        keep, jobs, outs = [], [], []
+        for p, s in enumerate(srcs):
+            nv, gaps = nvs[p], int(nvs[p] < T)
+            o = {}
+            aa_p = aa_all[s0[p] * J:s0[p + 1] * J]
+            jobs.append((aa_p, pose_all[p], p, (J - 1) * 3, J * 3, 3, L.FILL_F32, gaps))
+            jobs.append((aa_p, orient_all[p], p, 3, J * 3, 0, L.FILL_F32, gaps))
+            for n in ('beta', 'trans'):
+                x = get(s[n])                       # only its pointer is read before the upload: host arrays arrive contiguous
+                o[n] = torch.empty((T,) + tuple(x.shape[1:]), dtype=x.dtype, device=dev)
+                C = x.numel() // nv
+                jobs.append((x.contiguous(), o[n], p, C, C, 0, L.FILL_F32 if x.dtype == f32 else L.FILL_F64, gaps))
+            kp2 = torch.zeros((nv, 26, 2), dtype=f64, device=dev)
+            score = torch.zeros((nv, 26), dtype=f64, device=dev).index_fill_(1, m0, 1.0)
+            camk = torch.empty(up.shape(s['K']), device=dev)
+            after_send.append(lambda kp2=kp2, camk=camk, s=s: (kp2.index_copy_(1, m0, get(s['kp'])[:, :24].index_select(1, m1).to(f64)),
+                                                              camk.copy_(get(s['K']))))
+            jobs += [(kp2, kp_all[p], p, 52, 52, 0, L.FILL_F64, 0), (score, score_all[p], p, 26, 26, 0, L.FILL_F64, 0),
+                     (kp2, aligned_all[p], p, 52, 52, 0, L.FILL_F64, 0), (camk, K_all[p], p, camk[0].numel(), camk[0].numel(), 0, L.FILL_F32, 0)]
+            keep += [kp2, score, camk]
+            outs.append(o)
+        table = (L.FillJob * len(jobs))(*[L.FillJob(src.data_ptr(), dst.data_ptr(), p, C, stride, col0, kind, interp, nvs[p])
+                                            for src, dst, p, C, stride, col0, kind, interp in jobs])
+        up.fill(jobs_slot, bytes(table))
+        up.send()
+        for f in after_send:
+            f()
+        jobs_dev = up.get(jobs_slot)
+        vis_orig = torch.stack([e.to(f32) for e in exists]).contiguous()
+        before = torch.empty((P, T), dtype=torch.int32, device=dev)
+        frames = torch.empty((P, T), dtype=torch.int32, device=dev)
+        exist_all = torch.empty((P, T), dtype=torch.bool, device=dev)
+        jump = torch.empty((P, T), dtype=torch.uint8, device=dev)
+        info, visf_dev = rb[1:1 + 3 * P], rb[1 + 3 * P:]
+        lib = self._lib
+        with torch.cuda.device(dev):
+            st = L.stream_ptr()
+            L.check(lib.glamr_init_rotvec(N, L.ptr(rot_all), int(rot_dt == f64), L.ptr(aa_all), L.ptr(flags), L.ptr(rb), st), 'glamr_init_rotvec')
+            L.check(lib.glamr_init_vis_tables(P, T, L.ptr(vis_orig), L.ptr(before), L.ptr(frames), L.ptr(info), L.ptr(exist_all), st),
+                    'glamr_init_vis_tables')
+        max_cols = max(j[3] for j in jobs)
+        kp_rule = self.flag_filter_pose and self.flag_make_invis_with_keypoint
+
+        def fill_and_filter():
+            vis = vis_orig.clone()
+            with torch.cuda.device(dev):
+                L.check(lib.glamr_init_fill(len(jobs), L.ptr(jobs_dev), T, max_cols, L.ptr(before), L.ptr(frames), L.ptr(info), L.stream_ptr()),
+                        'glamr_init_fill')
+                L.check(lib.glamr_init_filter_pose(P, T, int(self.flag_filter_pose), L.ptr(orient_all), L.ptr(vis), L.ptr(jump),
+                                                   L.ptr(score_all) if kp_rule else None, ctypes.c_double(self.make_invis_keypoint_min_score),
+                                                   ctypes.c_double(self.make_invis_keypoint_min_num), L.ptr(visf_dev), L.stream_ptr()),
+                        'glamr_init_filter_pose')
+            host = torch.empty(rb.shape, dtype=torch.int32, pin_memory=True)
+            host.copy_(rb, non_blocking=True)
+            torch.cuda.current_stream(dev).synchronize()                 # the one read-back of init_data
+            return vis, host.numpy()
+        vis32, rb_h = fill_and_filter()
+        if rb_h[0] > 0:
+            # rows the Newton steps could not bring onto SO(3) (not HybrIK's float32 rotations): SciPy's projection, as
+            # rotmats_to_rotvec does, then the fill and the filter again
+            bad = torch.nonzero(flags).reshape(-1)
+            aa_all[bad] = torch.from_numpy(rotmats_to_rotvec(rot_all[bad].cpu().numpy()).astype(np.float32)).to(dev)
+            vis32, rb_h = fill_and_filter()
+        info_h = rb_h[1:1 + 3 * P].reshape(P, 3)
+        visf_h = rb_h[1 + 3 * P:].reshape(P, T).astype(bool)
+        self._init_host = {}
+        persons = {}
+        for p, (idx, s) in enumerate(zip(keys, srcs)):
+            if info_h[p, 0] != nvs[p]:
+                raise ValueError(f'person {idx}: bboxes_dict.exist marks {info_h[p, 0]} frames visible, the estimates have {nvs[p]} rows')
+            ex = exists[p]
+            visible = vis32[p].to(ex.dtype) if self.flag_filter_pose else ex.clone()
+            start, end = np.int64(info_h[p, 1]), np.int64(info_h[p, 2] + 1)
+            d = {'visible': visible, 'visible_orig': ex.clone(), 'fr_start': start, 'fr_end': end, 'exist_frames': exist_all[p],
+                 'exist_len': end - start, 'max_len': T, 'frames': torch.arange(T, device=dev), 'vis_frames': visible == 1,
+                 'invis_frames': visible == 0, 'frame2ind': {f: i for i, f in enumerate(np.arange(T))}, 'scale': None,
+                 'smpl_pose': pose_all[p]}
+            if 'gt' in s:
+                gt = get(s['gt'])          # a caller's CUDA tensor is copied, as the numpy path copies
+                d['smpl_pose_gt'] = gt.clone(memory_format=torch.contiguous_format) if isinstance(s['gt'], torch.Tensor) else gt
+            d['smpl_beta'] = outs[p]['beta']
+            d['smpl_orient_cam'] = orient_all[p]
+            d['root_trans_cam'] = outs[p]['trans']
+            d['kp_2d'], d['kp_2d_score'], d['kp_2d_aligned'], d['cam_K'] = kp_all[p], score_all[p], aligned_all[p], K_all[p]
+            persons[idx] = d
+            self._init_host[idx] = {'p': p, 'vis': visf_h[p], 'start': int(start), 'end': int(end)}
+        self._init_visf = (visf_h, visf_dev.view(P, T))
+        self._init_tables_f = None
+        return persons
+
+    def _filtered_tables(self):
+        """sample tables (glamr_init_vis_tables) of the filtered visibility: the heading interpolants' samples"""
+        if self._init_tables_f is None:
+            visf_h, visf_dev = self._init_visf
+            P, T = visf_h.shape
+            vis = visf_dev.to(torch.float32)
+            t = tuple(torch.empty((P, T), dtype=torch.int32, device=self.device) for _ in range(2)) + \
+                (torch.empty((P, 3), dtype=torch.int32, device=self.device),)
+            with torch.cuda.device(self.device):
+                L.check(self._lib.glamr_init_vis_tables(P, T, L.ptr(vis), L.ptr(t[0]), L.ptr(t[1]), L.ptr(t[2]), None, L.stream_ptr()),
+                        'glamr_init_vis_tables')
+            self._init_tables_f = t
+        return self._init_tables_f
 
     def infer_motion_traj(self, d):
         """:353-392"""
         if self.mt_model is None:
             return
-        ex = d['exist_frames']
+        ex = _exist_range(d)
         batch = {'in_body_pose': d['smpl_pose_nofill'][ex].unsqueeze(0).clone(), 'frame_mask': d['visible'][ex].unsqueeze(0).clone()}
         out = self.mt_model.inference(batch, sample_num=1)
         self._take_prior_output(d, out, 0)
@@ -326,8 +498,8 @@ class GlobalReconOptimizer:
         ds = list(persons.values())
         lens = {int(d['exist_len']) for d in ds}
         if len(ds) > 1 and len(lens) == 1 and getattr(self.mt_model, 'supports_person_batch', False):
-            batch = {'in_body_pose': torch.stack([d['smpl_pose_nofill'][d['exist_frames']] for d in ds]),
-                     'frame_mask': torch.stack([d['visible'][d['exist_frames']] for d in ds])}
+            batch = {'in_body_pose': torch.stack([d['smpl_pose_nofill'][_exist_range(d)] for d in ds]),
+                     'frame_mask': torch.stack([d['visible'][_exist_range(d)] for d in ds])}
             out = self.mt_model.inference(batch, sample_num=1)
             for b, d in enumerate(ds):
                 self._take_prior_output(d, out, b)
@@ -337,7 +509,7 @@ class GlobalReconOptimizer:
 
     def _take_prior_output(self, d, out, b):
         """:368-392 for batch row b of the prior's output"""
-        ex = d['exist_frames']
+        ex = _exist_range(d)
         if self.flag_infill_motion:
             d['infilled'] = True
             d['smpl_pose'] = d['smpl_pose'].detach().clone()
@@ -357,8 +529,8 @@ class GlobalReconOptimizer:
 
     def init_default_traj(self, d):
         """:319-323"""
-        d['root_trans_world_base'][:] = torch.tensor([0.0, 0.0, 0.8], device=self.device)
-        d['smpl_orient_world_base'][:] = G.quaternion_to_angle_axis(torch.tensor([[0.0, 0.0, 0.7071, 0.7071]], device=self.device))[0]
+        d['root_trans_world_base'][:] = self._const('default_trans', [0.0, 0.0, 0.8])
+        d['smpl_orient_world_base'][:] = G.quaternion_to_angle_axis(self._const('default_q', [[0.0, 0.0, 0.7071, 0.7071]]))[0]
         d['root_trans_world'] = d['root_trans_world_base']
         d['smpl_orient_world'] = d['smpl_orient_world_base']
 
@@ -366,110 +538,143 @@ class GlobalReconOptimizer:
         """:325-351 -- the world trajectory seen through the initial camera: translation as observed (the estimate is
         already interpolated over gaps), orientation interpolated with separate heading ('linear_interp') or both held at
         the last visible frame over the exist range ('last_pose', which also holds the body pose unless the prior infilled it)."""
-        for d in data['person_data'].values():
+        ds = data['person_data']
+        trans, orient_q = {}, {}
+        for key, d in ds.items():
             d['person_transform_world'] = torch.matmul(data['cam_pose_inv'], d['person_transform_cam'])
-            trans = d['person_transform_world'][:, :3, 3]
-            orient_q = G.rotation_matrix_to_quaternion(d['person_transform_world'][:, :3, :3].contiguous())
-            vis = d['vis_frames']
-            if self.traj_interp_method == 'linear_interp':
-                orient_q = self._interp_orient_q_sep_heading(orient_q[vis], vis)
-            else:
-                # forward fill from the last visible frame, over the exist range only (its first frame is visible); the
-                # source frames are visible, so one gather reproduces the reference's frame-by-frame loop
-                vis_h, ex_h = vis.cpu().numpy(), d['exist_frames'].cpu().numpy()
-                idx = np.arange(len(vis_h))
-                src = np.maximum.accumulate(np.where(vis_h, idx, 0))
-                fill = np.where(ex_h & ~vis_h)[0]
+            trans[key] = d['person_transform_world'][:, :3, 3]
+            orient_q[key] = G.rotation_matrix_to_quaternion(d['person_transform_world'][:, :3, :3].contiguous())
+        if self.traj_interp_method == 'linear_interp':
+            orient_q = self._interp_orient_q_sep_heading(orient_q)
+        else:
+            # forward fill from the last visible frame, over the exist range only (its first frame is visible); the
+            # source frames are visible, so one gather reproduces the reference's frame-by-frame loop.  One upload for all persons.
+            fills = {}
+            for key in ds:
+                h = self._init_host[key]
+                vis_h = h['vis']
+                src = np.maximum.accumulate(np.where(vis_h, np.arange(len(vis_h)), 0))
+                fill = np.nonzero(~vis_h[h['start']:h['end']])[0] + h['start']
                 if fill.size:
-                    dst_t, src_t = torch.as_tensor(fill, device=self.device), torch.as_tensor(src[fill], device=self.device)
-                    trans[dst_t] = trans[src_t]
-                    orient_q[dst_t] = orient_q[src_t]
+                    fills[key] = (fill, src[fill])
+            idx = iter(_upload_index([a for f in fills.values() for a in f], self.device)) if fills else None
+            for key, d in ds.items():
+                if key in fills:
+                    dst_t, src_t = next(idx), next(idx)
+                    trans[key][dst_t] = trans[key][src_t]
+                    orient_q[key][dst_t] = orient_q[key][src_t]
                     if not (self.flag_infer_motion_traj and self.flag_infill_motion):
                         d['smpl_pose'][dst_t] = d['smpl_pose'][src_t]
-            d['root_trans_world'] = d['root_trans_world_base'] = trans
-            d['smpl_orient_world'] = d['smpl_orient_world_base'] = G.quaternion_to_angle_axis(orient_q)
+        for key, d in ds.items():
+            d['root_trans_world'] = d['root_trans_world_base'] = trans[key]
+            d['smpl_orient_world'] = d['smpl_orient_world_base'] = G.quaternion_to_angle_axis(orient_q[key])
 
     def init_cam_pose(self, data, all_frames=False):
         """:294-317"""
-        cands = [torch.matmul(d['person_transform_world'], d['person2cam']) * d['vis_frames'][:, None, None]
-                 for d in data['person_data'].values()]
-        npers = data['fr_num_persons']
-        has = npers > 0
-        start = torch.where(has)[0][0]
-        inv = torch.zeros_like(data['cam_pose'])
-        inv[has] = cands[0][has]
+        d0 = next(iter(data['person_data'].values()))          # the reference builds every person's candidate and takes person 0's
+        cand = torch.matmul(d0['person_transform_world'], d0['person2cam']) * d0['vis_frames'][:, None, None]
+        has = data['fr_num_persons'] > 0
+        start = int(np.nonzero(self._init_visf[0].any(axis=0))[0][0])
+        inv = torch.where(has[:, None, None], cand, torch.zeros_like(data['cam_pose']))
         data['pose_infer_cam_pose_inv'] = inv
-        if all_frames:
-            if not torch.all(has):
-                last = inv[start]
-                for i in range(len(npers)):
-                    if npers[i] == 0:
-                        data['cam_pose_inv'][i] = last
-                    else:
-                        last = data['cam_pose_inv'][i]
-        else:
+        # all_frames: the reference's forward fill over frames without persons writes into the data['cam_pose_inv'] that
+        # the assignment below replaces, so the frames without persons keep zeros
+        if not all_frames:
             inv[...] = inv[start].clone()
         inv[:, :3, :3] = G.rot6d_to_rotmat(G.rotmat_to_rot6d(inv[:, :3, :3]))
         data['cam_pose_inv'] = inv
         data['cam_pose'] = G.inverse_transform(inv)
 
-    def _traj_local2global(self, local, local_heading=True):
-        """traj_pred/utils/traj_utils.py:65-88 for one sequence [T,11] -> trans [T,3], orient_q [T,4]"""
-        T = local.shape[0]
-        loc = local.reshape(T, 1, 11).contiguous().float()
-        trans = torch.empty((T, 1, 3), device=self.device)
-        oq = torch.empty((T, 1, 4), device=self.device)
-        scratch = torch.empty(T * 3, device=self.device)
-        with torch.cuda.device(self.device):
-            L.check(self._lib.glamr_traj_local2global(T, 1, L.ptr(loc), int(local_heading), L.ptr(trans), L.ptr(oq), L.ptr(scratch),
-                                                      L.stream_ptr()), 'glamr_traj_local2global')
-        return trans[:, 0], oq[:, 0]
+    def _traj_local2global(self, locals_, local_heading=True):
+        """traj_pred/utils/traj_utils.py:65-88 for a list of sequences [L_i,11] -> [(trans [L_i,3], orient_q [L_i,4])], one launch
+        per distinct length (the kernel runs one CTA per sequence)"""
+        out = [None] * len(locals_)
+        by_len = {}
+        for i, l in enumerate(locals_):
+            by_len.setdefault(l.shape[0], []).append(i)
+        for T, idx in by_len.items():
+            B = len(idx)
+            loc = torch.stack([locals_[i].float() for i in idx], dim=1).contiguous()        # time-major [T,B,11]
+            trans = torch.empty((T, B, 3), device=self.device)
+            oq = torch.empty((T, B, 4), device=self.device)
+            scratch = torch.empty(B * T * 3, device=self.device)
+            with torch.cuda.device(self.device):
+                L.check(self._lib.glamr_traj_local2global(T, B, L.ptr(loc), int(local_heading), L.ptr(trans), L.ptr(oq), L.ptr(scratch),
+                                                          L.stream_ptr()), 'glamr_traj_local2global')
+            for b, i in enumerate(idx):
+                out[i] = (trans[:, b], oq[:, b])
+        return out
 
     def _traj_global2local(self, trans, orient_q):
-        """traj_pred/utils/traj_utils.py:44-62 (init only)"""
-        base = torch.tensor([0.5, 0.5, 0.5, 0.5], device=self.device)
+        """traj_pred/utils/traj_utils.py:44-62 (init only) for [..., T, 3] / [..., T, 4]"""
+        base = self._const('base_q', [0.5, 0.5, 0.5, 0.5])
         xy, z = trans[..., :2], trans[..., 2]
         q = G.quat_mul(orient_q, G.quat_conjugate(base).expand_as(orient_q))
         heading = G.get_heading(q)
         d6 = G.quat_to_rot6d(G.deheading_quat(q, G.get_heading_q(q)))
-        d_heading = torch.cat([heading[:1], heading[1:] - heading[:-1]])
+        d_heading = torch.cat([heading[..., :1], heading[..., 1:] - heading[..., :-1]], dim=-1)
         hvec = G.heading_to_vec(d_heading)
-        dxy = xy[1:] - xy[:-1]
-        th = -heading[:-1]
+        dxy = xy[..., 1:, :] - xy[..., :-1, :]
+        th = -heading[..., :-1]
         c, s = torch.cos(th), torch.sin(th)
-        dxy_h = torch.stack([dxy[:, 0] * c - dxy[:, 1] * s, dxy[:, 0] * s + dxy[:, 1] * c], dim=-1)
-        return torch.cat([torch.cat([xy[:1], dxy_h]), z.unsqueeze(-1), d6, hvec], dim=-1)
+        dxy_h = torch.stack([dxy[..., 0] * c - dxy[..., 1] * s, dxy[..., 0] * s + dxy[..., 1] * c], dim=-1)
+        return torch.cat([torch.cat([xy[..., :1, :], dxy_h], dim=-2), z.unsqueeze(-1), d6, hvec], dim=-1)
 
-    def _interp_orient_q_sep_heading(self, orient_q_vis, vis_frames):
-        """traj_pred/utils/traj_utils.py:120-142 (SciPy linear interpolation on the host, as the reference)"""
-        base = torch.tensor([0.5, 0.5, 0.5, 0.5], device=self.device)
-        q = G.quat_mul(orient_q_vis, G.quat_conjugate(base).expand_as(orient_q_vis))
+    def _interp_orient_q_sep_heading(self, orient_q):
+        """traj_pred/utils/traj_utils.py:120-142 for every person: orient_q {key: [T,4]} -> {key: [T,4]}.  The heading vectors
+        and 6d rotations of each person's visible frames are linearly interpolated over the invisible ones (glamr_init_fill,
+        SciPy's operation order), all persons in one upload and one launch."""
+        before, frames, info = self._filtered_tables()
+        visf_h = self._init_visf[0]
+        keys = list(orient_q)
+        ps = [self._init_host[k]['p'] for k in keys]
+        T = visf_h.shape[1]
+        ns = [int(visf_h[p].sum()) for p in ps]
+        for k, n in zip(keys, ns):
+            if n < T and n < 2:              # filter_pose can leave fewer samples than the estimates had
+                raise ValueError(f'x and y arrays must have at least 2 entries: {n} frames of person {k} stay visible after '
+                                 'filter_pose, too few to interpolate the orientation over the others')
+        rows = np.concatenate([np.nonzero(visf_h[p])[0] + i * T for i, p in enumerate(ps)])
+        offs = np.concatenate([[0], np.cumsum(ns)])
+        packed = torch.empty((int(offs[-1]), 8), device=self.device)
+        both = torch.empty((len(keys), T, 8), device=self.device)
+        # a person whose every frame is a sample copies its samples, as the reference skips the interpolation
+        table = (L.FillJob * len(keys))(*[L.FillJob(packed[offs[i]:].data_ptr() if ns[i] else packed.data_ptr(), both[i].data_ptr(), p, 8, 8, 0,
+                                                    L.FILL_F32_W64, int(ns[i] < T), ns[i]) for i, p in enumerate(ps)])
+        up = _Upload()
+        rows_slot = up.source(rows.astype(np.int64), self.device)
+        job_slot = up.source(np.frombuffer(bytes(table), np.uint8), self.device)
+        up.allocate(self.device)
+        up.send()
+        q_all = torch.stack([orient_q[k] for k in keys]).reshape(-1, 4)
+        q_vis = q_all.index_select(0, up.get(rows_slot))
+        base = self._const('base_q', [0.5, 0.5, 0.5, 0.5])
+        q = G.quat_mul(q_vis, G.quat_conjugate(base).expand_as(q_vis))
         hq = G.get_heading_q(q)
-        hvec = G.heading_to_vec(G.get_heading(q))
-        d6 = G.quat_to_rot6d(G.deheading_quat(q, hq))
-        n = vis_frames.shape[0]
-        if int(vis_frames.sum()) == n:
-            hvec_i, d6_i = hvec, d6             # every frame is a sample point: linear interpolation returns the samples
-        else:
-            packed = torch.cat([hvec, d6], dim=-1).cpu().numpy()          # one device->host copy for both interpolants
-            vis_ind = np.where(vis_frames.cpu().numpy())[0]
-            f = interp1d(vis_ind, packed, axis=0, assume_sorted=True, fill_value='extrapolate')
-            both = torch.tensor(f(np.arange(n, dtype=np.float32)), device=self.device, dtype=torch.float32)
-            hvec_i, d6_i = both[:, :2].contiguous(), both[:, 2:].contiguous()
+        torch.cat([G.heading_to_vec(G.get_heading(q)), G.quat_to_rot6d(G.deheading_quat(q, hq))], dim=-1, out=packed)
+        with torch.cuda.device(self.device):
+            L.check(self._lib.glamr_init_fill(len(keys), L.ptr(up.get(job_slot)), T, 8, L.ptr(before), L.ptr(frames), L.ptr(info),
+                                              L.stream_ptr()), 'glamr_init_fill')
+        hvec_i, d6_i = both[..., :2].contiguous(), both[..., 2:].contiguous()
         out = G.quat_mul(G.heading_to_quat(G.vec_to_heading(hvec_i)), G.rot6d_to_quat(d6_i))
-        return G.quat_mul(out, base.expand_as(out))
+        out = G.quat_mul(out, base.expand_as(out))
+        return {k: out[i] for i, k in enumerate(keys)}
 
     def init_traj_heading_from_cam(self, data):
-        """:273-292"""
-        for d in data['person_data'].values():
-            world = torch.matmul(data['cam_pose_inv'], d['person_transform_cam'])
-            q = G.rotation_matrix_to_quaternion(world[:, :3, :3].contiguous())
-            q_interp = self._interp_orient_q_sep_heading(q[d['vis_frames']], d['vis_frames'])
-            local = self._traj_global2local(world[:, :3, 3], q_interp)
+        """:273-292 for every person: the interpolation and global->local conversion over [P, T], the codec per exist length"""
+        ds = data['person_data']
+        world = {key: torch.matmul(data['cam_pose_inv'], d['person_transform_cam']) for key, d in ds.items()}
+        q = {key: G.rotation_matrix_to_quaternion(w[:, :3, :3].contiguous()) for key, w in world.items()}
+        q_interp = self._interp_orient_q_sep_heading(q)
+        keys = list(ds)
+        local = self._traj_global2local(torch.stack([world[k][:, :3, 3] for k in keys]), torch.stack([q_interp[k] for k in keys]))
+        for i, (key, d) in enumerate(ds.items()):
+            ex = _exist_range(d)
             for (s, e) in self.cam_fix_frames:
-                d['traj_local_pred'][s:e, -2:] = local[d['exist_frames']][s:e, -2:]
-            trans, oq = self._traj_local2global(d['traj_local_pred'])
-            ex = d['exist_frames']
+                d['traj_local_pred'][s:e, -2:] = local[i][ex][s:e, -2:]
+        codec = self._traj_local2global([d['traj_local_pred'] for d in ds.values()])
+        for (trans, oq), d in zip(codec, ds.values()):
+            ex = _exist_range(d)
             d['smpl_orient_world_base'] = d['smpl_orient_world_base'].detach().clone()
             d['root_trans_world_base'] = d['root_trans_world_base'].detach().clone()
             d['smpl_orient_world_base'][ex] = G.quaternion_to_angle_axis(oq)
@@ -485,18 +690,15 @@ class GlobalReconOptimizer:
         num_fr = len(in_dict['est'][0]['bboxes_dict']['exist'])
         cam_pose = torch.eye(4, device=dev).repeat(num_fr, 1, 1)
         cam_pose_inv = G.inverse_transform(cam_pose)
-        persons = {}
-        for idx, est in in_dict['est'].items():
-            d = self._person_from_estimate(est, in_dict['gt'].get(idx))
-            if self.flag_filter_pose:
-                self.filter_pose(d)
+        persons = self._persons_from_estimates(in_dict, num_fr)
+        for d in persons.values():
             d['root_trans_world'] = G.transform_trans(cam_pose_inv, d['root_trans_cam'].float())
             d['smpl_orient_world'] = G.transform_rot(cam_pose_inv, d['smpl_orient_cam'].float())
             d['root_trans_world_base'] = d['root_trans_world'].clone()
             d['smpl_orient_world_base'] = d['smpl_orient_world'].clone()
             d['smpl_pose_nofill'] = d['smpl_pose'].clone()
-            d['smpl_pose_nofill'][~d['exist_frames']] = 0.0
-            persons[idx] = d
+            d['smpl_pose_nofill'][:int(d['fr_start'])] = 0.0
+            d['smpl_pose_nofill'][int(d['fr_end']):] = 0.0
         if self.flag_infer_motion_traj:
             self.infer_motion_traj_all(persons)
         if not (self.flag_infer_motion_traj and self.flag_pred_traj):
@@ -511,7 +713,7 @@ class GlobalReconOptimizer:
             last = d
             for d in persons.values():
                 if self.flag_opt_person2cam_rot or self.flag_opt_person2cam_trans:        # identity 6d, zero translation (:173-175)
-                    d['person2cam_res_rot'] = torch.tensor([1., 0., 0., 0., 1., 0.], device=dev).repeat(num_fr, 1)
+                    d['person2cam_res_rot'] = self._const('p2c_rot', [1., 0., 0., 0., 1., 0.]).repeat(num_fr, 1)
                     d['person2cam_res_trans'] = torch.zeros(num_fr, 3, device=dev)
                 d['smpl_orient_world_res'] = torch.zeros_like(last['smpl_orient_world'])
                 d['root_trans_world_res'] = torch.zeros_like(last['root_trans_world'])
@@ -536,7 +738,7 @@ class GlobalReconOptimizer:
                     d['root_trans_world_base'][:] = d['root_trans_world_base'][0].clone()
                     d['smpl_orient_world_base'][:] = d['smpl_orient_world_base'][0].clone()
         fr_num_persons = sum(d['vis_frames'] for d in persons.values())
-        n_empty = int((fr_num_persons == 0).sum())
+        n_empty = int((~self._init_visf[0].any(axis=0)).sum())
         data = {
             'seq_name': in_dict['seq_name'], 'person_data': persons, 'seq_len': num_fr, 'fr_num_persons': fr_num_persons,
             'cam_pose': cam_pose, 'cam_pose_inv': cam_pose_inv,
@@ -939,6 +1141,11 @@ class GlobalReconOptimizer:
         lh, S = self.loss_history, len(batch[0])
         hists = [lh] if len(datas) == 1 else [lh[:, g] for g in range(len(datas))]
         self.batch_loss_histories = [hists[i * S:(i + 1) * S] for i in range(len(batch))]
+
+
+def _exist_range(d):
+    """the exist frames of a person dict as a slice: they run from the first to the last visible frame"""
+    return slice(int(d['fr_start']), int(d['fr_end']))
 
 
 def _device_view(addr, count, device):

@@ -94,6 +94,44 @@ int glamr_traj_local2global(int T, int B, const float* local_traj, int local_hea
                             float* scratch, void* stream);
 
 /* ------------------------------------------------------------------------------------------------------------
+ * init_data on the device  --  global_recon/models/global_recon_model.py:88-137, :250-271 (glamr_b200/recon.py).
+ * All P persons of a T-frame sequence in one launch per entry point.
+ *
+ * glamr_init_rotvec: n rotation matrices [n,9] (float64 if f64, else float32) -> float32 rotation vectors [n,3] by
+ *   recon.rotmats_to_rotvec's float64 algorithm.  flags[i] = 1 (and *n_flagged += 1, int32, zeroed by the caller)
+ *   where the two Newton steps do not reach a proper rotation; those rows of rotvec hold zeros and belong to SciPy.
+ * glamr_init_vis_tables: per person p, from vis [P,T] (a frame is a sample where vis != 0): before [P,T] = samples
+ *   at earlier frames, frames [P,T] = frame of each sample (first `count` entries), info [P,3] = (count, first
+ *   sample frame, last sample frame; T and -1 without samples), exist [P,T] (uint8 0/1, may be NULL) = vis == 1 or
+ *   first <= t <= last.
+ * glamr_init_fill: job j of `jobs` (device array) writes jobs[j].dst [T, C] from the sample rows of person
+ *   jobs[j].person: with `interp`, scipy interp1d(kind='linear', fill_value='extrapolate') over the sample frames
+ *   (SciPy 1.18 operation order); without, the samples at their frames and zeros elsewhere.  max_cols >= every C.
+ *   Only the first min(count, rows) samples are read; an interpolating job with fewer than two leaves dst untouched
+ *   (the caller rejects that input, as interp1d does).
+ * glamr_init_filter_pose: with do_filter, recon.filter_pose on vis [P,T] in place (orient_cam [P,T,3] float32; jump
+ *   [P,T] uint8 scratch; kp_score [P,T,26] float64 or NULL for no keypoint rule); then vis_frames [P,T] int32 =
+ *   (vis == 1).
+ * ---------------------------------------------------------------------------------------------------------- */
+#define GLAMR_FILL_F32 0        /* float32 abscissae and rows (interp1d of float32 samples at float32 frames) */
+#define GLAMR_FILL_F64 1        /* float32 abscissae, float64 rows */
+#define GLAMR_FILL_F32_W64 2    /* float64 abscissae (integer frame indices), float32 rows, computed in float64, float32 out */
+typedef struct {
+  const void* src;      /* sample k of the person at src + (k * src_stride + src_col0) elements */
+  void* dst;            /* [T, C] */
+  int32_t person, C, src_stride, src_col0, kind, interp;
+  int32_t rows;         /* sample rows at src */
+} glamr_fill_job;
+size_t glamr_sizeof_fill_job(void);
+int glamr_init_rotvec(int n, const void* mats, int f64, float* rotvec, uint8_t* flags, int32_t* n_flagged, void* stream);
+int glamr_init_vis_tables(int P, int T, const float* vis, int32_t* before, int32_t* frames, int32_t* info, uint8_t* exist,
+                          void* stream);
+int glamr_init_fill(int n_jobs, const glamr_fill_job* jobs, int T, int max_cols, const int32_t* before, const int32_t* frames,
+                    const int32_t* info, void* stream);
+int glamr_init_filter_pose(int P, int T, int do_filter, const float* orient_cam, float* vis, uint8_t* jump, const double* kp_score,
+                           double min_score, double min_num, int32_t* vis_frames, void* stream);
+
+/* ------------------------------------------------------------------------------------------------------------
  * Learned prior (inference only)  --  stands behind MotionTrajJointModel.inference
  * (motion_infiller/models/motion_traj_joint_model.py:141-145): MotionInfillerVAE.inference_one_step
  * (motion_infiller/models/motion_infiller_vae.py:551-562 with ContextEncoder :92-123, DataDecoder :345-421) and

@@ -61,7 +61,7 @@ def wrap(obj, name, label=None):
     setattr(obj, name, timed)
 
 
-for n in ['_person_from_estimate', 'filter_pose', 'infer_motion_traj_all', 'init_cam_pose', 'init_traj_heading_from_cam', '_attach', 'forward', '_take_prior_output']:
+for n in ['_persons_from_estimates', '_interp_orient_q_sep_heading', 'infer_motion_traj_all', 'init_cam_pose', 'init_traj_heading_from_cam', '_attach', 'forward', '_take_prior_output']:
     wrap(model, n)
 wrap(mt, 'inference', 'mt_model.inference')
 REP = 5
