@@ -30,23 +30,20 @@ __global__ void rowop_vjp_kernel(int op, int n, int d0, int d1, int dout, const 
   if (gin1) for (int k = 0; k < d1; ++k) gin1[(size_t)i * d1 + k] = gb[k];
 }
 
-// traj_pred/utils/traj_utils.py:65-88 for sequence b (time-major [T,B,*]); one CTA per sequence.
-__global__ void __launch_bounds__(kScanThreads) traj_local2global_kernel(int T, int B, const float* __restrict__ local, int local_heading,
-                                                                        float* __restrict__ trans, float* __restrict__ orient_q,
-                                                                        float* __restrict__ scratch /*[B][T][3]*/) {
-  __shared__ float sm[kScanThreads / 32 + 1];
-  const int b = blockIdx.x;
-  float* head = scratch + (size_t)b * T * 3;
-  float* xy = head + T;
+// traj_pred/utils/traj_utils.py:65-88 for one sequence of T frames whose frame t sits at row t * ld (local, trans, orient_q
+// already offset to the sequence); head [T] and xy [2T] are its scratch.  One CTA.
+__device__ __forceinline__ void traj_local2global_seq(int T, int ld, const float* __restrict__ local, int local_heading,
+                                                      float* __restrict__ trans, float* __restrict__ orient_q, float* __restrict__ head,
+                                                      float* __restrict__ xy, float* sm) {
   for (int t = threadIdx.x; t < T; t += kScanThreads) {
-    const float* l = local + ((size_t)t * B + b) * 11;
+    const float* l = local + (size_t)t * ld * 11;
     head[t] = safe_atan2(l[10], l[9]);
   }
   __syncthreads();
   if (local_heading) block_scan_inplace(head, T, 1, false, sm);
   __syncthreads();
   for (int t = threadIdx.x; t < T; t += kScanThreads) {
-    const float* l = local + ((size_t)t * B + b) * 11;
+    const float* l = local + (size_t)t * ld * 11;
     float x = l[0], y = l[1];
     if (t > 0) {
       const float h = head[t - 1];
@@ -61,7 +58,7 @@ __global__ void __launch_bounds__(kScanThreads) traj_local2global_kernel(int T, 
   block_scan_inplace(xy + 1, T, 2, false, sm);
   __syncthreads();
   for (int t = threadIdx.x; t < T; t += kScanThreads) {
-    const float* l = local + ((size_t)t * B + b) * 11;
+    const float* l = local + (size_t)t * ld * 11;
     float R[9], lq[4], hq[4], q1[4], q[4];
     rot6d_to_rotmat(l + 3, R);
     rotmat_to_quat(R, lq);
@@ -70,11 +67,32 @@ __global__ void __launch_bounds__(kScanThreads) traj_local2global_kernel(int T, 
     quat_mul(hq, lq, q1);
     const float base[4] = {0.5f, 0.5f, 0.5f, 0.5f};
     quat_mul(q1, base, q);
-    float* tr = trans + ((size_t)t * B + b) * 3;
+    float* tr = trans + (size_t)t * ld * 3;
     tr[0] = xy[2 * t]; tr[1] = xy[2 * t + 1]; tr[2] = l[2];
-    float* oq = orient_q + ((size_t)t * B + b) * 4;
+    float* oq = orient_q + (size_t)t * ld * 4;
     oq[0] = q[0]; oq[1] = q[1]; oq[2] = q[2]; oq[3] = q[3];
   }
+}
+
+// B sequences, time-major [T,B,*]; one CTA per sequence
+__global__ void __launch_bounds__(kScanThreads) traj_local2global_kernel(int T, int B, const float* __restrict__ local, int local_heading,
+                                                                        float* __restrict__ trans, float* __restrict__ orient_q,
+                                                                        float* __restrict__ scratch /*[B][T][3]*/) {
+  __shared__ float sm[kScanThreads / 32 + 1];
+  const int b = blockIdx.x;
+  float* head = scratch + (size_t)b * T * 3;
+  traj_local2global_seq(T, B, local + (size_t)b * 11, local_heading, trans + (size_t)b * 3, orient_q + (size_t)b * 4, head, head + T, sm);
+}
+
+// B sequences of their own length, packed: sequence b holds rows offsets[b] .. offsets[b+1] - 1 of every array (scratch [rows][3]).
+// Sequence b gets exactly the arithmetic of a T = offsets[b+1] - offsets[b] call: the scan's chunking follows its own length.
+__global__ void __launch_bounds__(kScanThreads) traj_local2global_ragged_kernel(const int* __restrict__ offsets, const float* __restrict__ local,
+                                                                               int local_heading, float* __restrict__ trans,
+                                                                               float* __restrict__ orient_q, float* __restrict__ scratch) {
+  __shared__ float sm[kScanThreads / 32 + 1];
+  const int b = blockIdx.x, o = offsets[b], T = offsets[b + 1] - o;
+  float* head = scratch + (size_t)o * 3;
+  traj_local2global_seq(T, 1, local + (size_t)o * 11, local_heading, trans + (size_t)o * 3, orient_q + (size_t)o * 4, head, head + T, sm);
 }
 
 // Register-resident FFMA loop: what the FP32 pipe of this GPU sustains at its current clocks (bench.py quotes the LBS kernel,
@@ -138,3 +156,13 @@ extern "C" int glamr_traj_local2global(int T, int B, const float* local_traj, in
   GLAMR_LAUNCH_CHECK();
   return GLAMR_OK;
 }
+
+namespace glamr {
+// the codec over packed sequences of their own length (nets_kernels.cu's ragged trajectory predictor); offsets [B+1] on the device
+int traj_local2global_ragged(int B, const int* offsets, const float* local_traj, float* trans, float* orient_q, float* scratch,
+                             cudaStream_t stream) {
+  traj_local2global_ragged_kernel<<<B, kScanThreads, 0, stream>>>(offsets, local_traj, 1, trans, orient_q, scratch);
+  GLAMR_LAUNCH_CHECK();
+  return GLAMR_OK;
+}
+}  // namespace glamr

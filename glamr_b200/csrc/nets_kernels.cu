@@ -351,9 +351,8 @@ static int gemm_skinny_launch(cudaStream_t s, int M, int N, int K, const float* 
 
 // Arithmetic of a Linear with more than kSkinnyMaxM rows; smaller ones run the exact FP32 skinny kernel either way.
 enum GemmPrec { kTf32x3, kFp32 };
-static int gemm(cudaStream_t s, GemmPrec prec, int M, int N, int K, const float* X, int ldx, const float* W, const float* b, const float* b2,
-                float* Y, int ldy, int act) {
-  if (M <= kSkinnyMaxM) return gemm_skinny_launch(s, M, N, K, X, ldx, W, b, b2, Y, ldy, act);
+static int gemm_large(cudaStream_t s, GemmPrec prec, int M, int N, int K, const float* X, int ldx, const float* W, const float* b,
+                      const float* b2, float* Y, int ldy, int act) {
   if (prec == kTf32x3) return gemm_tc_launch(s, M, N, K, X, ldx, W, b, b2, Y, ldy, act);
   dim3 grid((N + GT - 1) / GT, (M + GT - 1) / GT);
   if (act == 1)
@@ -361,6 +360,22 @@ static int gemm(cudaStream_t s, GemmPrec prec, int M, int N, int K, const float*
   else
     gemm_bias_act_kernel<0><<<grid, 256, 0, s>>>(M, N, K, X, ldx, W, b, b2, Y, ldy);
   GLAMR_LAUNCH_CHECK();
+  return GLAMR_OK;
+}
+static int gemm(cudaStream_t s, GemmPrec prec, int M, int N, int K, const float* X, int ldx, const float* W, const float* b, const float* b2,
+                float* Y, int ldy, int act) {
+  if (M <= kSkinnyMaxM) return gemm_skinny_launch(s, M, N, K, X, ldx, W, b, b2, Y, ldy, act);
+  return gemm_large(s, prec, M, N, K, X, ldx, W, b, b2, Y, ldy, act);
+}
+// The ragged entry points: rows [0, split) run on the kernel a call of at most kSkinnyMaxM rows selects, rows [split, M) on the one a
+// larger call selects, so that each row gets the arithmetic of the single-track call it reproduces (every kernel computes an output row
+// from its X row and W alone).  X + split * ldx keeps the 16-byte alignment the vector paths test whenever ldx % 4 == 0, and with
+// ldx % 4 != 0 both the sub-range and the full call take the scalar path.
+static int gemm_split(cudaStream_t s, GemmPrec prec, int split, int M, int N, int K, const float* X, int ldx, const float* W, const float* b,
+                      const float* b2, float* Y, int ldy, int act) {
+  int rc;
+  if (split > 0 && (rc = gemm_skinny_launch(s, split, N, K, X, ldx, W, b, b2, Y, ldy, act))) return rc;
+  if (split < M) return gemm_large(s, prec, M - split, N, K, X + (size_t)split * ldx, ldx, W, b, b2, Y + (size_t)split * ldy, ldy, act);
   return GLAMR_OK;
 }
 
@@ -391,10 +406,12 @@ __global__ void __launch_bounds__(128) add_layernorm_kernel(int M, const float* 
 }
 
 // ------------------------------------------------------------------------------------------------ attention, head dim 32
-// Q rows (tq * B + b), K/V rows (tk * B + b); row strides ldq / ldkv; 8 heads of 32.  key_mask [B,Sk] (1 = ignore) or NULL.
+// Q rows (tq * B + b), K/V rows (tk * B + b) -- or batch-major (BM) rows b * Sq + tq, b * Sk + tk; row strides ldq / ldkv; 8 heads of
+// 32.  key_mask [B,Sk] (1 = ignore) or NULL.
 // grid (B, 8 heads, ceil(Sq / 8)): a CTA stages the head's K / V once and its 4 warps take 2 queries each, so that the kernel is
 // one short dependent chain deep at the batch sizes of the inference (B = 1-4) instead of Sq / 4 of them.
 constexpr int kAttnQChunk = 8;
+template <bool BM>
 __global__ void __launch_bounds__(128) attention_kernel(int B, int Sq, int Sk, const float* __restrict__ Q, int ldq,
                                                         const float* __restrict__ K, const float* __restrict__ V, int ldkv,
                                                         const uint8_t* __restrict__ key_mask, float* __restrict__ O, int ldo) {
@@ -405,14 +422,16 @@ __global__ void __launch_bounds__(128) attention_kernel(int B, int Sq, int Sk, c
   const int tid = threadIdx.x, lane = tid & 31, w = tid >> 5;
   for (int e = tid; e < Sk * 32; e += 128) {
     const int j = e >> 5, d = e & 31;
-    Ks[j][d] = K[((size_t)j * B + b) * ldkv + h * 32 + d];
-    Vs[j][d] = V[((size_t)j * B + b) * ldkv + h * 32 + d];
+    const size_t kr = BM ? (size_t)b * Sk + j : (size_t)j * B + b;
+    Ks[j][d] = K[kr * ldkv + h * 32 + d];
+    Vs[j][d] = V[kr * ldkv + h * 32 + d];
   }
   __syncthreads();
   const float scale = 0.17677669529663687f;   // 1/sqrt(32)
   const int q_end = min(Sq, ((int)blockIdx.z + 1) * kAttnQChunk);
   for (int q = blockIdx.z * kAttnQChunk + w; q < q_end; q += 4) {
-    const float qd = Q[((size_t)q * B + b) * ldq + h * 32 + lane] * scale;   // torch scales q before q k^T
+    const size_t qr = BM ? (size_t)b * Sq + q : (size_t)q * B + b;
+    const float qd = Q[qr * ldq + h * 32 + lane] * scale;   // torch scales q before q k^T
     float sc[2];
 #pragma unroll
     for (int r = 0; r < 2; ++r) {
@@ -433,19 +452,22 @@ __global__ void __launch_bounds__(128) attention_kernel(int B, int Sq, int Sk, c
     __syncwarp();
     float o = 0.0f;
     for (int j = 0; j < Sk; ++j) o = fmaf(Ps[w][j], Vs[j][lane], o);      // in key order (the reference's softmax(QK^T) V row sum)
-    O[((size_t)q * B + b) * ldo + h * 32 + lane] = o;
+    O[qr * ldo + h * 32 + lane] = o;
     __syncwarp();
   }
 }
 
 // ------------------------------------------------------------------------------------------------ positional encoding
 // out[row] = [ src_row (in_dim) | PE(pos) (256) ] with the 'original' sinusoid (lib/models/pos_encoding.py:27-32);
-// row = t * B + b, pos = t + pos_offset; src row = (src_bcast_t ? b : row) -> lets z be repeated over time.
-__global__ void pe_concat_kernel(int rows, int B, int in_dim, const float* __restrict__ src, int src_ld, int src_bcast_t,
+// row = t * B + b (or, batch-major, row = b * S + t with per = S; else per = B), pos = t + pos_offset; src row = (src_bcast_t ? b : row)
+// -> lets z be repeated over time.
+template <bool BM>
+__global__ void pe_concat_kernel(int rows, int per, int in_dim, const float* __restrict__ src, int src_ld, int src_bcast_t,
                                  int token_mode, int pos_offset, float* __restrict__ out) {
   const int row = blockIdx.x;
   if (row >= rows) return;
-  const int t = row / B, b = row - t * B;
+  const int q = row / per, r = row - q * per;
+  const int t = BM ? r : q, b = BM ? q : r;
   const int od = in_dim + 256;
   const float* s = token_mode ? (src + (size_t)t * src_ld) : (src + (size_t)(src_bcast_t ? b : row) * src_ld);
   for (int c = threadIdx.x; c < od; c += blockDim.x) {
@@ -491,6 +513,39 @@ __global__ void mean_time_kernel(int T, int B, int D, const float* __restrict__ 
   out[e] = s / (float)T;
 }
 
+// ---- packed sequences of their own length: sequence b holds rows off[b] .. off[b+1] - 1 (off == NULL: every sequence has T rows)
+__device__ __forceinline__ int seq_off(const int* off, int T, int b) { return off ? off[b] : b * T; }
+// the sequence that packed row `row` belongs to
+__device__ __forceinline__ int seq_of_row(const int* __restrict__ off, int B, int row) {
+  int lo = 0, hi = B - 1;
+  while (lo < hi) {
+    const int mid = (lo + hi + 1) >> 1;
+    if (off[mid] <= row) lo = mid; else hi = mid - 1;
+  }
+  return lo;
+}
+// mean_time_kernel of each sequence over its own frames, in the same order
+__global__ void mean_time_ragged_kernel(int B, int T, const int* __restrict__ off, int D, const float* __restrict__ X, float* __restrict__ out) {
+  const int e = blockIdx.x * blockDim.x + threadIdx.x;
+  if (e >= B * D) return;
+  const int b = e / D, k = e - b * D;
+  const int o = seq_off(off, T, b), n = seq_off(off, T, b + 1) - o;
+  float s = 0.0f;
+  for (int t = 0; t < n; ++t) s += X[((size_t)o + t) * D + k];
+  out[e] = s / (float)n;
+}
+// concat_z_kernel with each packed row's own sequence
+__global__ void concat_z_ragged_kernel(int rows, int B, int T, const int* __restrict__ off, int nz, int D, const float* __restrict__ z,
+                                       const float* __restrict__ ctx, float* __restrict__ out) {
+  const size_t total = (size_t)rows * (nz + D);
+  for (size_t e = (size_t)blockIdx.x * blockDim.x + threadIdx.x; e < total; e += (size_t)gridDim.x * blockDim.x) {
+    const size_t row = e / (nz + D);
+    const int c = (int)(e - row * (nz + D));
+    const int b = off ? seq_of_row(off, B, (int)row) : (int)(row / T);
+    out[e] = (c < nz) ? z[(size_t)b * nz + c] : ctx[row * D + (c - nz)];
+  }
+}
+
 // [z (nz, per batch) | context row] -> rows of width nz + D
 __global__ void concat_z_kernel(int rows, int B, int nz, int D, const float* __restrict__ z, const float* __restrict__ ctx,
                                 float* __restrict__ out) {
@@ -516,6 +571,18 @@ __global__ void traj_first_frame_kernel(int B, float* __restrict__ local /*[T,B,
   l[10] = init_heading ? sinf(init_heading[b]) : 1.0f;
 }
 
+// traj_first_frame_kernel on frame 0 of each packed sequence
+__global__ void traj_first_frame_ragged_kernel(int B, const int* __restrict__ off, float* __restrict__ local /*[rows,11]*/,
+                                               const float* __restrict__ init_xy, const float* __restrict__ init_heading) {
+  const int b = blockIdx.x * blockDim.x + threadIdx.x;
+  if (b >= B) return;
+  float* l = local + (size_t)off[b] * 11;
+  l[0] = init_xy ? init_xy[b * 2] : 0.0f;
+  l[1] = init_xy ? init_xy[b * 2 + 1] : 0.0f;
+  l[9] = init_heading ? cosf(init_heading[b]) : 0.0f;
+  l[10] = init_heading ? sinf(init_heading[b]) : 1.0f;
+}
+
 __global__ void quat_rows_to_aa_kernel(int n, const float* __restrict__ q, float* __restrict__ aa) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= n) return;
@@ -529,8 +596,11 @@ __global__ void quat_rows_to_aa_kernel(int n, const float* __restrict__ q, float
 // grid (B, 2 directions), 512 threads = one gate row each.  The recurrent matrix W_hh [512,128] lives on chip for the
 // whole sequence: columns 0..63 of a thread's row in registers, columns 64..127 in shared memory ([k][row], conflict
 // free).  xproj [T,B,2,512] already holds W_ih x_t + b_ih + b_hh.  out [T,B,256] = [h_fwd | h_bwd].
+// PACKED: sequence b is rows seq_off(off, T, b) .. of its own length (xproj [rows,2,512], out [rows,256]); the backward direction starts
+// at its own last frame.
 constexpr int LH = 128, LG = 4 * LH, LREG = 64;
-__global__ void __launch_bounds__(LG, 1) lstm_recurrence_kernel(int T, int B, const float* __restrict__ xproj,
+template <bool PACKED>
+__global__ void __launch_bounds__(LG, 1) lstm_recurrence_kernel(int T, int B, const int* __restrict__ off, const float* __restrict__ xproj,
                                                                 const float* __restrict__ whh_f, const float* __restrict__ whh_b,
                                                                 float* __restrict__ out) {
   extern __shared__ float smem[];
@@ -538,6 +608,8 @@ __global__ void __launch_bounds__(LG, 1) lstm_recurrence_kernel(int T, int B, co
   float* hs = Wsm + (LH - LREG) * LG;      // [LH]
   float* gs = hs + LH;                     // [LG]
   const int b = blockIdx.x, dir = blockIdx.y, r = threadIdx.x;
+  const int o = PACKED ? seq_off(off, T, b) : 0;
+  const int n = PACKED ? seq_off(off, T, b + 1) - o : T;
   const float* W = (dir == 0 ? whh_f : whh_b) + (size_t)r * LH;
   float wreg[LREG];
 #pragma unroll
@@ -546,9 +618,10 @@ __global__ void __launch_bounds__(LG, 1) lstm_recurrence_kernel(int T, int B, co
   float c = 0.0f;
   if (r < LH) hs[r] = 0.0f;
   __syncthreads();
-  for (int step = 0; step < T; ++step) {
-    const int t = dir == 0 ? step : T - 1 - step;
-    float a = xproj[(((size_t)t * B + b) * 2 + dir) * LG + r];
+  for (int step = 0; step < n; ++step) {
+    const int t = dir == 0 ? step : n - 1 - step;
+    const size_t row = PACKED ? (size_t)o + t : (size_t)t * B + b;
+    float a = xproj[(row * 2 + dir) * LG + r];
 #pragma unroll
     for (int k4 = 0; k4 < LREG / 4; ++k4) {
       const float4 h4 = *reinterpret_cast<const float4*>(hs + 4 * k4);
@@ -569,7 +642,7 @@ __global__ void __launch_bounds__(LG, 1) lstm_recurrence_kernel(int T, int B, co
       c = fg * c + ig * gg;
       const float h = og * tanhf(c);
       hs[r] = h;
-      out[((size_t)t * B + b) * (2 * LH) + dir * LH + r] = h;
+      out[row * (2 * LH) + dir * LH + r] = h;
     }
     __syncthreads();
   }
@@ -626,6 +699,21 @@ struct Arena {
   float* take(size_t n) { size_t o = used; used += (n + 63) & ~(size_t)63; return used <= cap ? base + o : nullptr; }
 };
 
+// How the Linears of an infiller window choose their kernel.  rb == NULL: by the launch's own M (B sequences, time-major rows t * B + b).
+// Otherwise the rows are batch-major (b * S + t) and slot b reproduces a call of rb[b] sequences (host array); the slots are ordered so
+// that S * rb[b] > kSkinnyMaxM holds on a suffix of them for every S, and a Linear over S rows per slot runs as two row ranges.
+struct WinDisp {
+  int B;
+  const int* rb;
+};
+int lin(cudaStream_t s, const WinDisp& d, int S, int N, int K, const float* X, int ldx, const float* W, const float* b, float* Y, int ldy,
+        int act) {
+  if (!d.rb) return gemm(s, kTf32x3, S * d.B, N, K, X, ldx, W, b, nullptr, Y, ldy, act);
+  int j = 0;
+  while (j < d.B && S * d.rb[j] <= kSkinnyMaxM) ++j;
+  return gemm_split(s, kTf32x3, j * S, S * d.B, N, K, X, ldx, W, b, nullptr, Y, ldy, act);
+}
+
 int layernorm(cudaStream_t s, int M, const float* X, const float* R, const float* g, const float* b, float* Y) {
   add_layernorm_kernel<<<(M + 3) / 4, 128, 0, s>>>(M, X, R, g, b, Y);
   GLAMR_LAUNCH_CHECK();
@@ -633,62 +721,66 @@ int layernorm(cudaStream_t s, int M, const float* X, const float* R, const float
 }
 
 // multi-head attention block: out = out_proj(attn(q_src, kv_src)); q_src [Sq*B,256], kv_src [Sk*B,256]
-int mha(cudaStream_t s, Arena& A, const AttnW& w, int B, int Sq, int Sk, const float* q_src, const float* kv_src, const uint8_t* mask,
-        float* out) {
+int mha(cudaStream_t s, Arena& A, const WinDisp& d, const AttnW& w, int Sq, int Sk, const float* q_src, const float* kv_src,
+        const uint8_t* mask, float* out) {
   if (Sk > 64) return GLAMR_EUNSUPPORTED;
-  const int Mq = Sq * B, Mk = Sk * B;
+  const int B = d.B, Mq = Sq * B, Mk = Sk * B;
   const size_t mark = A.used;
   float* q = A.take((size_t)Mq * 256);
   float* kv = A.take((size_t)Mk * 512);
   float* att = A.take((size_t)Mq * 256);
   if (!q || !kv || !att) return GLAMR_ENOSPACE;
   int rc;
-  if ((rc = gemm(s, kTf32x3, Mq, 256, 256, q_src, 256, w.in_w, w.in_b, nullptr, q, 256, 0))) return rc;
-  if ((rc = gemm(s, kTf32x3, Mk, 512, 256, kv_src, 256, w.in_w + 256 * 256, w.in_b + 256, nullptr, kv, 512, 0))) return rc;
-  attention_kernel<<<dim3(B, 8, (Sq + kAttnQChunk - 1) / kAttnQChunk), 128, 0, s>>>(B, Sq, Sk, q, 256, kv, kv + 256, 512, mask, att, 256);
+  if ((rc = lin(s, d, Sq, 256, 256, q_src, 256, w.in_w, w.in_b, q, 256, 0))) return rc;
+  if ((rc = lin(s, d, Sk, 512, 256, kv_src, 256, w.in_w + 256 * 256, w.in_b + 256, kv, 512, 0))) return rc;
+  const dim3 grid(B, 8, (Sq + kAttnQChunk - 1) / kAttnQChunk);
+  if (d.rb) attention_kernel<true><<<grid, 128, 0, s>>>(B, Sq, Sk, q, 256, kv, kv + 256, 512, mask, att, 256);
+  else attention_kernel<false><<<grid, 128, 0, s>>>(B, Sq, Sk, q, 256, kv, kv + 256, 512, mask, att, 256);
   GLAMR_LAUNCH_CHECK();
-  if ((rc = gemm(s, kTf32x3, Mq, 256, 256, att, 256, w.out_w, w.out_b, nullptr, out, 256, 0))) return rc;
+  if ((rc = lin(s, d, Sq, 256, 256, att, 256, w.out_w, w.out_b, out, 256, 0))) return rc;
   A.used = mark;
   return GLAMR_OK;
 }
 
-int ffn(cudaStream_t s, Arena& A, int M, const float* x, const float* l1w, const float* l1b, const float* l2w, const float* l2b, float* out) {
+int ffn(cudaStream_t s, Arena& A, const WinDisp& d, int S, const float* x, const float* l1w, const float* l1b, const float* l2w,
+        const float* l2b, float* out) {
   const size_t mark = A.used;
-  float* h = A.take((size_t)M * 512);
+  float* h = A.take((size_t)S * d.B * 512);
   if (!h) return GLAMR_ENOSPACE;
   int rc;
-  if ((rc = gemm(s, kTf32x3, M, 512, 256, x, 256, l1w, l1b, nullptr, h, 512, 1))) return rc;
-  if ((rc = gemm(s, kTf32x3, M, 256, 512, h, 512, l2w, l2b, nullptr, out, 256, 0))) return rc;
+  if ((rc = lin(s, d, S, 512, 256, x, 256, l1w, l1b, h, 512, 1))) return rc;
+  if ((rc = lin(s, d, S, 256, 512, h, 512, l2w, l2b, out, 256, 0))) return rc;
   A.used = mark;
   return GLAMR_OK;
 }
 
 // nn.TransformerEncoderLayer, post-norm, relu, eval mode (dropout = identity); x updated in place
-int encoder_layer(cudaStream_t s, Arena& A, const EncLayer& L, int B, int S, float* x, const uint8_t* mask) {
-  const int M = S * B;
+int encoder_layer(cudaStream_t s, Arena& A, const WinDisp& d, const EncLayer& L, int S, float* x, const uint8_t* mask) {
+  const int M = S * d.B;
   const size_t mark = A.used;
   float* t = A.take((size_t)M * 256);
   if (!t) return GLAMR_ENOSPACE;
   int rc;
-  if ((rc = mha(s, A, L.sa, B, S, S, x, x, mask, t))) return rc;
+  if ((rc = mha(s, A, d, L.sa, S, S, x, x, mask, t))) return rc;
   if ((rc = layernorm(s, M, x, t, L.n1g, L.n1b, x))) return rc;
-  if ((rc = ffn(s, A, M, x, L.l1w, L.l1b, L.l2w, L.l2b, t))) return rc;
+  if ((rc = ffn(s, A, d, S, x, L.l1w, L.l1b, L.l2w, L.l2b, t))) return rc;
   if ((rc = layernorm(s, M, x, t, L.n2g, L.n2b, x))) return rc;
   A.used = mark;
   return GLAMR_OK;
 }
 // nn.TransformerDecoderLayer (no tgt mask), memory [Sm*B,256] with key padding mask
-int decoder_layer(cudaStream_t s, Arena& A, const DecLayer& L, int B, int S, int Sm, float* x, const float* mem, const uint8_t* mem_mask) {
-  const int M = S * B;
+int decoder_layer(cudaStream_t s, Arena& A, const WinDisp& d, const DecLayer& L, int S, int Sm, float* x, const float* mem,
+                  const uint8_t* mem_mask) {
+  const int M = S * d.B;
   const size_t mark = A.used;
   float* t = A.take((size_t)M * 256);
   if (!t) return GLAMR_ENOSPACE;
   int rc;
-  if ((rc = mha(s, A, L.sa, B, S, S, x, x, nullptr, t))) return rc;
+  if ((rc = mha(s, A, d, L.sa, S, S, x, x, nullptr, t))) return rc;
   if ((rc = layernorm(s, M, x, t, L.n1g, L.n1b, x))) return rc;
-  if ((rc = mha(s, A, L.ca, B, S, Sm, x, mem, mem_mask, t))) return rc;
+  if ((rc = mha(s, A, d, L.ca, S, Sm, x, mem, mem_mask, t))) return rc;
   if ((rc = layernorm(s, M, x, t, L.n2g, L.n2b, x))) return rc;
-  if ((rc = ffn(s, A, M, x, L.l1w, L.l1b, L.l2w, L.l2b, t))) return rc;
+  if ((rc = ffn(s, A, d, S, x, L.l1w, L.l1b, L.l2w, L.l2b, t))) return rc;
   if ((rc = layernorm(s, M, x, t, L.n3g, L.n3b, x))) return rc;
   A.used = mark;
   return GLAMR_OK;
@@ -728,14 +820,12 @@ extern "C" int glamr_net_set_tensor(glamr_net* n, const char* name, const float*
 
 extern "C" size_t glamr_infiller_workspace_floats(int B) { return (size_t)B * 50 * 256 * 16 + 65536; }
 
-// One 50-frame window of MotionInfillerVAE.inference_one_step (mode 'infer', sample_num 1), B sequences.
-//   in_pose [50,B,69]  key_pad_mask [B,50] (1 = frame not usable as key)  eps [B or 1,128] (eps_rows = B or 1) or NULL
-//   out_pose [40,B,69] = [first 10 input frames | 30 decoded frames]
-extern "C" int glamr_infiller_window_forward(const glamr_net* n, int B, const float* in_pose, const uint8_t* key_pad_mask,
-                                             const float* eps, int eps_rows, float* out_pose, float* workspace,
-                                             size_t workspace_floats, void* stream) {
-  if (!n || B <= 0 || !in_pose || !key_pad_mask || !out_pose || !workspace) return GLAMR_EINVAL;
-  cudaStream_t s = (cudaStream_t)stream;
+// One 50-frame window of MotionInfillerVAE.inference_one_step for d.B sequences (layout and kernel choice: WinDisp) -> *dec_out, the
+// 30 decoded frames [30 B, 69] (arena memory).  in_pose [50 B, 69]  key_pad_mask [B,50]  eps rows eps_ld apart (0: one row for all) or NULL
+static int infiller_window(const glamr_net* n, const WinDisp& d, const float* in_pose, const uint8_t* key_pad_mask, const float* eps,
+                           int eps_ld, float** dec_out_p, Arena& A, cudaStream_t s) {
+  const int B = d.B;
+  const bool bm = d.rb != nullptr;
   int e = 0;
   const std::string ce = "context_encoder.", dd = "data_decoder.";
   const float* in_fc_w = W(n, ce + "in_fc.weight", 256 * 69, &e), * in_fc_b = W(n, ce + "in_fc.bias", 256, &e);
@@ -752,7 +842,6 @@ extern "C" int glamr_infiller_window_forward(const glamr_net* n, int B, const fl
   const float* pmw = W(n, dd + "p_z_mu_net.weight", 128 * 256, &e), * pmb = W(n, dd + "p_z_mu_net.bias", 128, &e);
   const float* plw = W(n, dd + "p_z_logvar_net.weight", 128 * 256, &e), * plb = W(n, dd + "p_z_logvar_net.bias", 128, &e);
   if (e) return GLAMR_EINVAL;
-  Arena A{workspace, workspace_floats, 0};
   const int S = 50, Sc = 30, M = S * B, Mc = Sc * B;
   float* x = A.take((size_t)M * 256);
   float* cat = A.take((size_t)M * 512);
@@ -767,34 +856,58 @@ extern "C" int glamr_infiller_window_forward(const glamr_net* n, int B, const fl
   float* dec_out = A.take((size_t)Mc * 69);
   if (!dec_out) return GLAMR_ENOSPACE;
   int rc;
+  auto pe_concat = [&](int rows, int per_tm, int per_bm, int in_dim, const float* src, int src_bcast_t, int token_mode, int pos_offset) {
+    if (bm) pe_concat_kernel<true><<<rows, 128, 0, s>>>(rows, per_bm, in_dim, src, in_dim, src_bcast_t, token_mode, pos_offset, cat);
+    else pe_concat_kernel<false><<<rows, 128, 0, s>>>(rows, per_tm, in_dim, src, in_dim, src_bcast_t, token_mode, pos_offset, cat);
+  };
   // ---- context encoder (motion_infiller_vae.py:92-123)
-  if ((rc = gemm(s, kTf32x3, M, 256, 69, in_pose, 69, in_fc_w, in_fc_b, nullptr, x, 256, 0))) return rc;
-  pe_concat_kernel<<<M, 128, 0, s>>>(M, B, 256, x, 256, 0, 0, 0, cat);
+  if ((rc = lin(s, d, S, 256, 69, in_pose, 69, in_fc_w, in_fc_b, x, 256, 0))) return rc;
+  pe_concat(M, B, S, 256, x, 0, 0, 0);
   GLAMR_LAUNCH_CHECK();
-  if ((rc = gemm(s, kTf32x3, M, 256, 512, cat, 512, cpe_w, cpe_b, nullptr, x, 256, 0))) return rc;
+  if ((rc = lin(s, d, S, 256, 512, cat, 512, cpe_w, cpe_b, x, 256, 0))) return rc;
   for (int l = 0; l < 2; ++l)
-    if ((rc = encoder_layer(s, A, enc[l], B, S, x, key_pad_mask))) return rc;
+    if ((rc = encoder_layer(s, A, d, enc[l], S, x, key_pad_mask))) return rc;
   // ---- learned prior over z (:354-362): two tokens attend to the context
   GLAMR_CUDA_TRY(cudaMemcpyAsync(tok, mu_tok, 256 * sizeof(float), cudaMemcpyDeviceToDevice, s));
   GLAMR_CUDA_TRY(cudaMemcpyAsync(tok + 256, lv_tok, 256 * sizeof(float), cudaMemcpyDeviceToDevice, s));
-  pe_concat_kernel<<<2 * B, 128, 0, s>>>(2 * B, B, 256, tok, 256, 0, 1, 0, cat);
+  pe_concat(2 * B, B, 2, 256, tok, 0, 1, 0);
   GLAMR_LAUNCH_CHECK();
-  if ((rc = gemm(s, kTf32x3, 2 * B, 256, 512, cat, 512, ppe_w, ppe_b, nullptr, px, 256, 0))) return rc;
-  if ((rc = decoder_layer(s, A, pri, B, 2, S, px, x, key_pad_mask))) return rc;
-  if ((rc = gemm(s, kTf32x3, B, 128, 256, px, 256, pmw, pmb, nullptr, mu, 128, 0))) return rc;
-  if ((rc = gemm(s, kTf32x3, B, 128, 256, px + (size_t)B * 256, 256, plw, plb, nullptr, lv, 128, 0))) return rc;
-  sample_z_kernel<<<(B * 128 + 127) / 128, 128, 0, s>>>(B, 128, mu, 128, lv, 128, eps, eps_rows == 1 ? 0 : 128, z);
+  if ((rc = lin(s, d, 2, 256, 512, cat, 512, ppe_w, ppe_b, px, 256, 0))) return rc;
+  if ((rc = decoder_layer(s, A, d, pri, 2, S, px, x, key_pad_mask))) return rc;
+  // the mu token's rows, then the logvar token's: rows 0 .. B-1 and B .. 2B-1 time-major, every other row batch-major
+  const float* pmu = px;
+  const float* plv = bm ? px + 256 : px + (size_t)B * 256;
+  const int ldp = bm ? 512 : 256;
+  if ((rc = lin(s, d, 1, 128, 256, pmu, ldp, pmw, pmb, mu, 128, 0))) return rc;
+  if ((rc = lin(s, d, 1, 128, 256, plv, ldp, plw, plb, lv, 128, 0))) return rc;
+  sample_z_kernel<<<(B * 128 + 127) / 128, 128, 0, s>>>(B, 128, mu, 128, lv, 128, eps, eps_ld, z);
   GLAMR_LAUNCH_CHECK();
   // ---- decoder (:383-395): z repeated over the 30 current frames, PE offset 10
-  pe_concat_kernel<<<Mc, 128, 0, s>>>(Mc, B, 128, z, 128, 1, 0, 10, cat);
+  pe_concat(Mc, B, Sc, 128, z, 1, 0, 10);
   GLAMR_LAUNCH_CHECK();
-  if ((rc = gemm(s, kTf32x3, Mc, 256, 384, cat, 384, dpe_w, dpe_b, nullptr, dx, 256, 0))) return rc;
+  if ((rc = lin(s, d, Sc, 256, 384, cat, 384, dpe_w, dpe_b, dx, 256, 0))) return rc;
   for (int l = 0; l < 2; ++l)
-    if ((rc = decoder_layer(s, A, dec[l], B, Sc, S, dx, x, key_pad_mask))) return rc;
-  if ((rc = gemm(s, kTf32x3, Mc, 512, 256, dx, 256, om0w, om0b, nullptr, h1, 512, 1))) return rc;
-  if ((rc = gemm(s, kTf32x3, Mc, 256, 512, h1, 512, om1w, om1b, nullptr, h2, 256, 1))) return rc;
-  if ((rc = gemm(s, kTf32x3, Mc, 69, 256, h2, 256, ofw, ofb, nullptr, dec_out, 69, 0))) return rc;
-  concat_time_kernel<<<64, 256, 0, s>>>(10, Sc, B, 69, in_pose, dec_out, out_pose);
+    if ((rc = decoder_layer(s, A, d, dec[l], Sc, S, dx, x, key_pad_mask))) return rc;
+  if ((rc = lin(s, d, Sc, 512, 256, dx, 256, om0w, om0b, h1, 512, 1))) return rc;
+  if ((rc = lin(s, d, Sc, 256, 512, h1, 512, om1w, om1b, h2, 256, 1))) return rc;
+  if ((rc = lin(s, d, Sc, 69, 256, h2, 256, ofw, ofb, dec_out, 69, 0))) return rc;
+  *dec_out_p = dec_out;
+  return GLAMR_OK;
+}
+
+// One 50-frame window of MotionInfillerVAE.inference_one_step (mode 'infer', sample_num 1), B sequences.
+//   in_pose [50,B,69]  key_pad_mask [B,50] (1 = frame not usable as key)  eps [B or 1,128] (eps_rows = B or 1) or NULL
+//   out_pose [40,B,69] = [first 10 input frames | 30 decoded frames]
+extern "C" int glamr_infiller_window_forward(const glamr_net* n, int B, const float* in_pose, const uint8_t* key_pad_mask,
+                                             const float* eps, int eps_rows, float* out_pose, float* workspace,
+                                             size_t workspace_floats, void* stream) {
+  if (!n || B <= 0 || !in_pose || !key_pad_mask || !out_pose || !workspace) return GLAMR_EINVAL;
+  cudaStream_t s = (cudaStream_t)stream;
+  Arena A{workspace, workspace_floats, 0};
+  float* dec_out = nullptr;
+  const int rc = infiller_window(n, WinDisp{B, nullptr}, in_pose, key_pad_mask, eps, eps_rows == 1 ? 0 : 128, &dec_out, A, s);
+  if (rc) return rc;
+  concat_time_kernel<<<64, 256, 0, s>>>(10, 30, B, 69, in_pose, dec_out, out_pose);
   GLAMR_LAUNCH_CHECK();
   return GLAMR_OK;
 }
@@ -855,6 +968,115 @@ extern "C" int glamr_infiller_forward(const glamr_net* n, int T, int B, float* p
   return GLAMR_OK;
 }
 
+// ------------------------------------------------------------------------------------------------ tracks of their own length
+// The ragged entry points take B tracks packed without padding: track b is rows offsets[b] .. offsets[b+1] - 1 (offsets [B+1] on the
+// device, lens [B] and row_batch [B] on the host).  Row b reproduces the single-track entry called for a batch of row_batch[b] tracks of
+// its length (1 for a lone track, P for a block of P equal-length tracks): each Linear of that call picks its kernel by M, so the rows are
+// ordered by the kernel each Linear runs for them, and every Linear runs as at most two launches over contiguous rows (gemm_split).
+
+// The infiller's kernel choice for a call of rb tracks: which of its Linears (50, 30, 2 and 1 rows per track) exceed kSkinnyMaxM rows.
+static int infiller_class(int rb) {
+  const int S[4] = {50, 30, 2, 1};
+  int c = 0;
+  for (int i = 0; i < 4; ++i) c += S[i] * rb > kSkinnyMaxM;
+  return c;
+}
+static int infiller_windows(int T) { return (T - 10 + 29) / 30; }
+
+// Window slots -> tracks.  The tracks are ordered by infiller class and, within a class, by decreasing length, so the tracks that still
+// have window i form a prefix of each class: slot j of segment g (slot0[g] <= j < slot0[g+1]) is track row0[g] + j - slot0[g].
+constexpr int kMaxInfillerClasses = 5;
+struct SlotMap {
+  int nseg;
+  int slot0[kMaxInfillerClasses + 1], row0[kMaxInfillerClasses];
+};
+__device__ __forceinline__ int slot_track(const SlotMap& m, int j) {
+  int g = 0;
+  while (g + 1 < m.nseg && j >= m.slot0[g + 1]) ++g;
+  return m.row0[g] + j - m.slot0[g];
+}
+// window_prep_kernel for the Bi active slots (batch-major window [Bi,50,69], key mask [Bi,50]), plus each slot's eps of window `wi`
+__global__ void window_prep_ragged_kernel(int Bi, SlotMap m, int wi, int s0, int eps_windows, const int* __restrict__ off,
+                                          const float* __restrict__ pose, const uint8_t* __restrict__ key_pad, const float* __restrict__ eps,
+                                          float* __restrict__ win, uint8_t* __restrict__ kp, float* __restrict__ epsw) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i < Bi * 50 * 69) {
+    const int j = i / (50 * 69), t = (i - j * 50 * 69) / 69, k = i - (j * 50 + t) * 69;
+    const int r = slot_track(m, j), o = off[r], T = off[r + 1] - o;
+    win[i] = (s0 + t < T) ? pose[((size_t)o + s0 + t) * 69 + k] : 0.0f;
+  }
+  if (i < Bi * 50) {
+    const int j = i / 50, t = i - j * 50;
+    const int r = slot_track(m, j), o = off[r], T = off[r + 1] - o;
+    kp[i] = t < 10 ? 0 : ((s0 + t < T) ? key_pad[(size_t)o + s0 + t] : 1);
+  }
+  if (i < Bi * 128) {
+    const int j = i / 128, k = i - j * 128;
+    epsw[i] = eps[((size_t)slot_track(m, j) * eps_windows + wi) * 128 + k];
+  }
+}
+// window_commit_kernel: the first min(40, T - s0) frames of [10 input frames | 30 decoded frames] replace the track's running pose
+__global__ void window_commit_ragged_kernel(int Bi, SlotMap m, int s0, const int* __restrict__ off, const float* __restrict__ win,
+                                            const float* __restrict__ dec, float* __restrict__ pose) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= Bi * 40 * 69) return;
+  const int j = i / (40 * 69), t = (i - j * 40 * 69) / 69, k = i - (j * 40 + t) * 69;
+  const int r = slot_track(m, j), o = off[r], T = off[r + 1] - o;
+  if (t < min(40, T - s0)) pose[((size_t)o + s0 + t) * 69 + k] = t < 10 ? win[((size_t)j * 50 + t) * 69 + k] : dec[((size_t)j * 30 + t - 10) * 69 + k];
+}
+
+extern "C" size_t glamr_infiller_ragged_workspace_floats(int B) {
+  if (B <= 0) return 0;
+  return glamr_infiller_workspace_floats(B) + (size_t)50 * B * 69 + (size_t)B * 128 + (size_t)(B * 50 + 3) / 4 + 256;
+}
+
+extern "C" int glamr_infiller_forward_ragged(const glamr_net* n, int B, const int* lens, const int* row_batch, const int* offsets,
+                                             float* pose_io, const uint8_t* key_pad, const float* eps, int eps_windows, float* workspace,
+                                             size_t workspace_floats, void* stream) {
+  if (!n || B <= 0 || !lens || !row_batch || !offsets || !pose_io || !key_pad || !eps || !workspace) return GLAMR_EINVAL;
+  int nmax = 0;
+  for (int b = 0; b < B; ++b) {
+    if (lens[b] <= 10 || row_batch[b] <= 0) return GLAMR_EINVAL;
+    if (b > 0) {
+      const int c0 = infiller_class(row_batch[b - 1]), c1 = infiller_class(row_batch[b]);
+      if (c1 < c0 || (c1 == c0 && lens[b] > lens[b - 1])) return GLAMR_EINVAL;
+    }
+    nmax = max(nmax, infiller_windows(lens[b]));
+  }
+  if (eps_windows < nmax) return GLAMR_EINVAL;
+  if (workspace_floats < glamr_infiller_ragged_workspace_floats(B)) return GLAMR_ENOSPACE;
+  cudaStream_t s = (cudaStream_t)stream;
+  float* win = workspace;
+  float* epsw = win + (size_t)50 * B * 69;
+  uint8_t* kp = reinterpret_cast<uint8_t*>(epsw + (size_t)B * 128);
+  float* rest = reinterpret_cast<float*>((reinterpret_cast<uintptr_t>(kp + (size_t)B * 50) + 255) & ~(uintptr_t)255);
+  const size_t rest_floats = workspace_floats - (size_t)(rest - workspace);
+  std::vector<int> rb_slot(B);
+  for (int i = 0; i < nmax; ++i) {
+    SlotMap m{};
+    int Bi = 0;
+    for (int b0 = 0; b0 < B;) {
+      int b1 = b0;
+      while (b1 < B && infiller_class(row_batch[b1]) == infiller_class(row_batch[b0])) ++b1;
+      m.slot0[m.nseg] = Bi;
+      m.row0[m.nseg++] = b0;
+      for (int b = b0; b < b1 && infiller_windows(lens[b]) > i; ++b) rb_slot[Bi++] = row_batch[b];
+      b0 = b1;
+    }
+    m.slot0[m.nseg] = Bi;
+    const int s0 = i * 30;
+    window_prep_ragged_kernel<<<(Bi * 50 * 69 + 255) / 256, 256, 0, s>>>(Bi, m, i, s0, eps_windows, offsets, pose_io, key_pad, eps, win, kp, epsw);
+    GLAMR_LAUNCH_CHECK();
+    Arena A{rest, rest_floats, 0};
+    float* dec = nullptr;
+    const int rc = infiller_window(n, WinDisp{Bi, rb_slot.data()}, win, kp, epsw, 128, &dec, A, s);
+    if (rc) return rc;
+    window_commit_ragged_kernel<<<(Bi * 40 * 69 + 255) / 256, 256, 0, s>>>(Bi, m, s0, offsets, win, dec, pose_io);
+    GLAMR_LAUNCH_CHECK();
+  }
+  return GLAMR_OK;
+}
+
 extern "C" size_t glamr_trajpred_workspace_floats(int T, int B) { return (size_t)T * B * (512 + 256 + 2 * 512 + 256 + 384 + 512 + 256 + 64) + (size_t)B * 2048 + 65536; }
 
 extern "C" int glamr_traj_local2global(int T, int B, const float* local_traj, int local_heading, float* trans, float* orient_q,
@@ -865,8 +1087,14 @@ extern "C" int glamr_traj_local2global(int T, int B, const float* local_traj, in
 // eps [R or 1,128] (eps_rows = R or 1) or NULL (-> z = mu).  Scratch comes from A.  The single-pass and the windowed entry
 // points both run the network through here.  Its Linears stay on the FP32 GEMMs: their matrices are launch-latency sized, and the
 // per-frame heading error accumulates through the codec's prefix sum.
-static int trajpred_network(const glamr_net* n, int T, int R, const float* in, const float* eps, int eps_rows, float* raw, Arena& A,
-                            cudaStream_t s) {
+// Packed rows (the ragged entries): sequence b of the R holds frames seq_off(off, T, b) .. of its own length, M frames in all; frames
+// [0, fsplit) and sequences [0, rsplit) run their Linears on the kernel a call of at most kSkinnyMaxM rows selects, the rest on the larger one.
+struct Packed {
+  const int* off;
+  int M, fsplit, rsplit;
+};
+static int trajpred_network(const glamr_net* n, int T, int R, const Packed* pk, const float* in, const float* eps, int eps_rows, float* raw,
+                            Arena& A, cudaStream_t s) {
   int e = 0;
   const std::string ce = "context_encoder.", dd = "data_decoder.";
   const float* im0w = W(n, ce + "in_mlp.affine_layers.0.weight", 512 * 69, &e), * im0b = W(n, ce + "in_mlp.affine_layers.0.bias", 512, &e);
@@ -887,7 +1115,13 @@ static int trajpred_network(const glamr_net* n, int T, int R, const float* in, c
   const float* dm1w = W(n, dd + "out_mlp.affine_layers.1.weight", 256 * 512, &e), * dm1b = W(n, dd + "out_mlp.affine_layers.1.bias", 256, &e);
   const float* ofw = W(n, dd + "out_fc.weight", 11 * 256, &e), * ofb = W(n, dd + "out_fc.bias", 11, &e);
   if (e) return GLAMR_EINVAL;
-  const int M = T * R;
+  const int M = pk ? pk->M : T * R;
+  auto flin = [&](int N, int K, const float* X, int ldx, const float* Wt, const float* b, const float* b2, float* Y, int ldy, int act) {
+    return pk ? gemm_split(s, kFp32, pk->fsplit, M, N, K, X, ldx, Wt, b, b2, Y, ldy, act) : gemm(s, kFp32, M, N, K, X, ldx, Wt, b, b2, Y, ldy, act);
+  };
+  auto rlin = [&](int N, int K, const float* X, int ldx, const float* Wt, const float* b, float* Y, int ldy, int act) {
+    return pk ? gemm_split(s, kFp32, pk->rsplit, R, N, K, X, ldx, Wt, b, nullptr, Y, ldy, act) : gemm(s, kFp32, R, N, K, X, ldx, Wt, b, nullptr, Y, ldy, act);
+  };
   float* h512 = A.take((size_t)M * 512);
   float* x = A.take((size_t)M * 256);
   float* xp = A.take((size_t)M * 2 * 512);
@@ -903,35 +1137,39 @@ static int trajpred_network(const glamr_net* n, int T, int R, const float* in, c
   static bool attr = false;
   const size_t lstm_smem = ((size_t)(LH - LREG) * LG + LH + LG) * sizeof(float);
   if (!attr) {
-    GLAMR_CUDA_TRY(cudaFuncSetAttribute(lstm_recurrence_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)lstm_smem));
+    GLAMR_CUDA_TRY(cudaFuncSetAttribute(lstm_recurrence_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)lstm_smem));
+    GLAMR_CUDA_TRY(cudaFuncSetAttribute(lstm_recurrence_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)lstm_smem));
     attr = true;
   }
   // ---- context encoder (traj_pred_vae.py:72-92)
-  if ((rc = gemm(s, kFp32, M, 512, 69, in, 69, im0w, im0b, nullptr, h512, 512, 1))) return rc;
-  if ((rc = gemm(s, kFp32, M, 256, 512, h512, 512, im1w, im1b, nullptr, x, 256, 1))) return rc;
+  if ((rc = flin(512, 69, in, 69, im0w, im0b, nullptr, h512, 512, 1))) return rc;
+  if ((rc = flin(256, 512, h512, 512, im1w, im1b, nullptr, x, 256, 1))) return rc;
   for (int l = 0; l < 2; ++l) {
     for (int d = 0; d < 2; ++d)   // xproj[t][b][d][:] = W_ih x + b_ih + b_hh
-      if ((rc = gemm(s, kFp32, M, 512, 256, x, 256, wih[l][d], bih[l][d], bhh[l][d], xp + d * 512, 1024, 0))) return rc;
-    lstm_recurrence_kernel<<<dim3(R, 2), LG, lstm_smem, s>>>(T, R, xp, whh[l][0], whh[l][1], y);
+      if ((rc = flin(512, 256, x, 256, wih[l][d], bih[l][d], bhh[l][d], xp + d * 512, 1024, 0))) return rc;
+    if (pk) lstm_recurrence_kernel<true><<<dim3(R, 2), LG, lstm_smem, s>>>(T, R, pk->off, xp, whh[l][0], whh[l][1], y);
+    else lstm_recurrence_kernel<false><<<dim3(R, 2), LG, lstm_smem, s>>>(T, R, nullptr, xp, whh[l][0], whh[l][1], y);
     GLAMR_LAUNCH_CHECK();
     float* tmp = x; x = y; y = tmp;
   }
-  if ((rc = gemm(s, kFp32, M, 512, 256, x, 256, cm0w, cm0b, nullptr, h512, 512, 1))) return rc;
-  if ((rc = gemm(s, kFp32, M, 256, 512, h512, 512, cm1w, cm1b, nullptr, y, 256, 1))) return rc;      // y = context
+  if ((rc = flin(512, 256, x, 256, cm0w, cm0b, nullptr, h512, 512, 1))) return rc;
+  if ((rc = flin(256, 512, h512, 512, cm1w, cm1b, nullptr, y, 256, 1))) return rc;      // y = context
   // ---- prior + z (:281-297)
-  mean_time_kernel<<<(R * 256 + 127) / 128, 128, 0, s>>>(T, R, 256, y, hm);
+  if (pk) mean_time_ragged_kernel<<<(R * 256 + 127) / 128, 128, 0, s>>>(R, T, pk->off, 256, y, hm);
+  else mean_time_kernel<<<(R * 256 + 127) / 128, 128, 0, s>>>(T, R, 256, y, hm);
   GLAMR_LAUNCH_CHECK();
-  if ((rc = gemm(s, kFp32, R, 512, 256, hm, 256, pm0w, pm0b, nullptr, hp, 512, 1))) return rc;
-  if ((rc = gemm(s, kFp32, R, 256, 512, hp, 512, pm1w, pm1b, nullptr, hq, 256, 1))) return rc;
-  if ((rc = gemm(s, kFp32, R, 256, 256, hq, 256, pzw, pzb, nullptr, pz, 256, 0))) return rc;
+  if ((rc = rlin(512, 256, hm, 256, pm0w, pm0b, hp, 512, 1))) return rc;
+  if ((rc = rlin(256, 512, hp, 512, pm1w, pm1b, hq, 256, 1))) return rc;
+  if ((rc = rlin(256, 256, hq, 256, pzw, pzb, pz, 256, 0))) return rc;
   sample_z_kernel<<<(R * 128 + 127) / 128, 128, 0, s>>>(R, 128, pz, 256, pz + 128, 256, eps, eps_rows == 1 ? 0 : 128, z);
   GLAMR_LAUNCH_CHECK();
   // ---- decoder (:298-333)
-  concat_z_kernel<<<256, 256, 0, s>>>(M, R, 128, 256, z, y, cat);
+  if (pk) concat_z_ragged_kernel<<<256, 256, 0, s>>>(M, R, T, pk->off, 128, 256, z, y, cat);
+  else concat_z_kernel<<<256, 256, 0, s>>>(M, R, 128, 256, z, y, cat);
   GLAMR_LAUNCH_CHECK();
-  if ((rc = gemm(s, kFp32, M, 512, 384, cat, 384, dm0w, dm0b, nullptr, h512, 512, 1))) return rc;
-  if ((rc = gemm(s, kFp32, M, 256, 512, h512, 512, dm1w, dm1b, nullptr, x, 256, 1))) return rc;
-  return gemm(s, kFp32, M, 11, 256, x, 256, ofw, ofb, nullptr, raw, 11, 0);
+  if ((rc = flin(512, 384, cat, 384, dm0w, dm0b, nullptr, h512, 512, 1))) return rc;
+  if ((rc = flin(256, 512, h512, 512, dm1w, dm1b, nullptr, x, 256, 1))) return rc;
+  return flin(11, 256, x, 256, ofw, ofb, nullptr, raw, 11, 0);
 }
 
 // TrajPredVAE.inference (multi_step False, sample_num 1): joint positions -> local trajectory -> global trajectory.
@@ -945,7 +1183,7 @@ extern "C" int glamr_trajpred_forward(const glamr_net* n, int T, int B, const fl
   Arena A{workspace, workspace_floats, 0};
   const int M = T * B;
   int rc;
-  if ((rc = trajpred_network(n, T, B, in_joint_pos, eps, eps_rows, out_local_traj, A, s))) return rc;
+  if ((rc = trajpred_network(n, T, B, nullptr, in_joint_pos, eps, eps_rows, out_local_traj, A, s))) return rc;
   float* oq = A.take((size_t)M * 4);
   float* sc = A.take((size_t)M * 3);
   if (!sc) return GLAMR_ENOSPACE;
@@ -982,12 +1220,9 @@ __global__ void traj_window_gather_kernel(int T, int B, int W, int C, const floa
 // xy = 0, heading vector (0, 1): no init_xy / init_heading reaches a window, :319-327); window c >= 1 its raw output with
 // frame 0's heading vector replaced by heading_to_vec(get_heading(rot6d_to_quat(.))) of global frame c W - 1's columns 3:9.
 // Padded frames are dropped.  One thread per output row.
-__global__ void traj_window_stitch_kernel(int T, int B, int W, int C, const float* __restrict__ raw, float* __restrict__ local) {
-  const int i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= T * B) return;
-  const int t = i / B, b = i - t * B;
-  const int c = t / W, tw = t - c * W;
-  const float* src = raw + ((size_t)tw * C * B + (size_t)c * B + b) * 11;
+// src: the frame's raw row; prev: raw row W - 1 of window c - 1
+__device__ __forceinline__ void traj_window_stitch_row(int c, int tw, const float* __restrict__ src, const float* __restrict__ prev,
+                                                       float* __restrict__ dst) {
   float l[11];
 #pragma unroll
   for (int k = 0; k < 11; ++k) l[k] = src[k];
@@ -995,7 +1230,6 @@ __global__ void traj_window_stitch_kernel(int T, int B, int W, int C, const floa
     if (c == 0) {
       l[0] = 0.0f; l[1] = 0.0f; l[9] = 0.0f; l[10] = 1.0f;
     } else {
-      const float* prev = raw + ((size_t)(W - 1) * C * B + (size_t)(c - 1) * B + b) * 11;
       float R[9], q[4];
       rot6d_to_rotmat(prev + 3, R);
       rotmat_to_quat(R, q);
@@ -1003,9 +1237,16 @@ __global__ void traj_window_stitch_kernel(int T, int B, int W, int C, const floa
       l[9] = cosf(h); l[10] = sinf(h);
     }
   }
-  float* dst = local + (size_t)i * 11;
 #pragma unroll
   for (int k = 0; k < 11; ++k) dst[k] = l[k];
+}
+__global__ void traj_window_stitch_kernel(int T, int B, int W, int C, const float* __restrict__ raw, float* __restrict__ local) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= T * B) return;
+  const int t = i / B, b = i - t * B;
+  const int c = t / W, tw = t - c * W;
+  traj_window_stitch_row(c, tw, raw + ((size_t)tw * C * B + (size_t)c * B + b) * 11,
+                         c > 0 ? raw + ((size_t)(W - 1) * C * B + (size_t)(c - 1) * B + b) * 11 : nullptr, local + (size_t)i * 11);
 }
 
 extern "C" size_t glamr_trajpred_windows_workspace_floats(int T, int B, int W) {
@@ -1033,11 +1274,148 @@ extern "C" int glamr_trajpred_windows_forward(const glamr_net* n, int T, int B, 
   traj_window_gather_kernel<<<1024, 256, 0, s>>>(T, B, W, C, in_joint_pos, win);
   GLAMR_LAUNCH_CHECK();
   int rc;
-  if ((rc = trajpred_network(n, W, R, win, eps, R, raw, A, s))) return rc;
+  if ((rc = trajpred_network(n, W, R, nullptr, win, eps, R, raw, A, s))) return rc;
   traj_window_stitch_kernel<<<(T * B + 127) / 128, 128, 0, s>>>(T, B, W, C, raw, out_local_traj);
   GLAMR_LAUNCH_CHECK();
   if ((rc = glamr_traj_local2global(T, B, out_local_traj, 1, out_trans, oq, sc, stream))) return rc;
   quat_rows_to_aa_kernel<<<(T * B + 127) / 128, 128, 0, s>>>(T * B, oq, out_orient_aa);
+  GLAMR_LAUNCH_CHECK();
+  return GLAMR_OK;
+}
+
+// ------------------------------------------------------------------------------------------------ ragged trajectory predictor
+extern "C" int glamr_traj_local2global(int T, int B, const float* local_traj, int local_heading, float* trans, float* orient_q,
+                                       float* scratch, void* stream);
+namespace glamr {
+int traj_local2global_ragged(int B, const int* offsets, const float* local_traj, float* trans, float* orient_q, float* scratch,
+                             cudaStream_t stream);
+}
+
+// The predictor's kernel choice for a call whose Linears have `frames` rows per frame-wise layer and `rows` per sequence-wise layer
+static int trajpred_class(long long frames, long long rows) { return (frames > kSkinnyMaxM) + (rows > kSkinnyMaxM); }
+
+static int ragged_total(int B, const int* lens) {
+  long long M = 0;
+  for (int b = 0; b < B; ++b) {
+    if (lens[b] <= 0) return -1;
+    M += lens[b];
+  }
+  return M > INT_MAX / 1024 ? -1 : (int)M;
+}
+
+extern "C" size_t glamr_trajpred_ragged_workspace_floats(int B, const int* lens) {
+  const int M = (B > 0 && lens) ? ragged_total(B, lens) : -1;
+  return M < 0 ? 0 : glamr_trajpred_workspace_floats(M, 1) + (size_t)B * 2048;
+}
+
+extern "C" int glamr_trajpred_forward_ragged(const glamr_net* n, int B, const int* lens, const int* row_batch, const int* offsets,
+                                             const float* in_joint_pos, const float* eps, const float* init_xy, const float* init_heading,
+                                             float* out_local_traj, float* out_trans, float* out_orient_aa, float* workspace,
+                                             size_t workspace_floats, void* stream) {
+  if (!n || B <= 0 || !lens || !row_batch || !offsets || !in_joint_pos || !out_local_traj || !out_trans || !out_orient_aa || !workspace)
+    return GLAMR_EINVAL;
+  const int M = ragged_total(B, lens);
+  if (M < 0) return GLAMR_EINVAL;
+  Packed pk{offsets, M, 0, 0};
+  for (int b = 0; b < B; ++b) {
+    if (row_batch[b] <= 0) return GLAMR_EINVAL;
+    const int c = trajpred_class((long long)lens[b] * row_batch[b], row_batch[b]);
+    if (b > 0 && c < trajpred_class((long long)lens[b - 1] * row_batch[b - 1], row_batch[b - 1])) return GLAMR_EINVAL;
+    if (c == 0) pk.fsplit += lens[b];
+    if (c < 2) ++pk.rsplit;
+  }
+  if (workspace_floats < glamr_trajpred_ragged_workspace_floats(B, lens)) return GLAMR_ENOSPACE;
+  cudaStream_t s = (cudaStream_t)stream;
+  Arena A{workspace, workspace_floats, 0};
+  int rc;
+  if ((rc = trajpred_network(n, 0, B, &pk, in_joint_pos, eps, B, out_local_traj, A, s))) return rc;
+  float* oq = A.take((size_t)M * 4);
+  float* sc = A.take((size_t)M * 3);
+  if (!sc) return GLAMR_ENOSPACE;
+  traj_first_frame_ragged_kernel<<<(B + 127) / 128, 128, 0, s>>>(B, offsets, out_local_traj, init_xy, init_heading);
+  GLAMR_LAUNCH_CHECK();
+  if ((rc = traj_local2global_ragged(B, offsets, out_local_traj, out_trans, oq, sc, s))) return rc;
+  quat_rows_to_aa_kernel<<<(M + 127) / 128, 128, 0, s>>>(M, oq, out_orient_aa);
+  GLAMR_LAUNCH_CHECK();
+  return GLAMR_OK;
+}
+
+// window row w (window c of track b, w = win_offsets[b] + c), frame tw = global frame c W + tw of track b, zero past its end
+__global__ void traj_window_gather_ragged_kernel(int B, int W, int Rw, const int* __restrict__ off, const int* __restrict__ woff,
+                                                 const float* __restrict__ jp, float* __restrict__ win) {
+  const size_t total = (size_t)Rw * W * 69;
+  for (size_t e = (size_t)blockIdx.x * blockDim.x + threadIdx.x; e < total; e += (size_t)gridDim.x * blockDim.x) {
+    const size_t row = e / 69;
+    const int k = (int)(e - row * 69);
+    const int w = (int)(row / W), tw = (int)(row - (size_t)w * W);
+    const int b = seq_of_row(woff, B, w);
+    const int t = (w - woff[b]) * W + tw, o = off[b];
+    win[e] = t < off[b + 1] - o ? jp[((size_t)o + t) * 69 + k] : 0.0f;
+  }
+}
+__global__ void traj_window_stitch_ragged_kernel(int B, int W, int M, const int* __restrict__ off, const int* __restrict__ woff,
+                                                 const float* __restrict__ raw, float* __restrict__ local) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= M) return;
+  const int b = seq_of_row(off, B, i);
+  const int t = i - off[b], c = t / W, tw = t - c * W;
+  const size_t w = (size_t)woff[b] + c;
+  traj_window_stitch_row(c, tw, raw + (w * W + tw) * 11, c > 0 ? raw + ((w - 1) * W + W - 1) * 11 : nullptr, local + (size_t)i * 11);
+}
+
+static long long ragged_windows(int B, const int* lens, int W) {
+  long long C = 0;
+  for (int b = 0; b < B; ++b) C += (lens[b] + W - 1) / W;
+  return C;
+}
+
+extern "C" size_t glamr_trajpred_windows_ragged_workspace_floats(int B, const int* lens, int W) {
+  const int M = (B > 0 && lens && W > 0) ? ragged_total(B, lens) : -1;
+  if (M < 0) return 0;
+  const long long Rw = ragged_windows(B, lens, W);
+  if (Rw * W > INT_MAX / 1024) return 0;
+  return (size_t)W * Rw * (69 + 11) + (size_t)M * 7 + 4 * 64 + glamr_trajpred_workspace_floats(W, (int)Rw);
+}
+
+extern "C" int glamr_trajpred_windows_forward_ragged(const glamr_net* n, int B, int W, const int* lens, const int* row_batch,
+                                                     const int* offsets, const int* win_offsets, const float* in_joint_pos, const float* eps,
+                                                     float* out_local_traj, float* out_trans, float* out_orient_aa, float* workspace,
+                                                     size_t workspace_floats, void* stream) {
+  if (!n || B <= 0 || W <= 0 || !lens || !row_batch || !offsets || !win_offsets || !in_joint_pos || !out_local_traj || !out_trans ||
+      !out_orient_aa || !workspace)
+    return GLAMR_EINVAL;
+  const size_t need = glamr_trajpred_windows_ragged_workspace_floats(B, lens, W);
+  if (need == 0) return GLAMR_EINVAL;
+  const int M = ragged_total(B, lens), Rw = (int)ragged_windows(B, lens, W);
+  // window rows inherit their track's class: a single-track call of rb tracks runs C rb windows of W frames as one batch
+  Packed pk{nullptr, Rw * W, 0, 0};
+  for (int b = 0; b < B; ++b) {
+    if (row_batch[b] <= 0) return GLAMR_EINVAL;
+    const long long C = (lens[b] + W - 1) / W, r = C * row_batch[b];
+    const int c = trajpred_class(r * W, r);
+    if (b > 0) {
+      const long long rp = (long long)((lens[b - 1] + W - 1) / W) * row_batch[b - 1];
+      if (c < trajpred_class(rp * W, rp)) return GLAMR_EINVAL;
+    }
+    if (c == 0) pk.fsplit += (int)C * W;
+    if (c < 2) pk.rsplit += (int)C;
+  }
+  if (workspace_floats < need) return GLAMR_ENOSPACE;
+  cudaStream_t s = (cudaStream_t)stream;
+  Arena A{workspace, workspace_floats, 0};
+  float* win = A.take((size_t)W * Rw * 69);
+  float* raw = A.take((size_t)W * Rw * 11);
+  float* oq = A.take((size_t)M * 4);
+  float* sc = A.take((size_t)M * 3);
+  if (!sc) return GLAMR_ENOSPACE;
+  traj_window_gather_ragged_kernel<<<1024, 256, 0, s>>>(B, W, Rw, offsets, win_offsets, in_joint_pos, win);
+  GLAMR_LAUNCH_CHECK();
+  int rc;
+  if ((rc = trajpred_network(n, W, Rw, &pk, win, eps, Rw, raw, A, s))) return rc;
+  traj_window_stitch_ragged_kernel<<<(M + 127) / 128, 128, 0, s>>>(B, W, M, offsets, win_offsets, raw, out_local_traj);
+  GLAMR_LAUNCH_CHECK();
+  if ((rc = traj_local2global_ragged(B, offsets, out_local_traj, out_trans, oq, sc, s))) return rc;
+  quat_rows_to_aa_kernel<<<(M + 127) / 128, 128, 0, s>>>(M, oq, out_orient_aa);
   GLAMR_LAUNCH_CHECK();
   return GLAMR_OK;
 }

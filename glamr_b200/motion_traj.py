@@ -21,6 +21,7 @@ from . import lib as L
 PAST, CUR, FUT, NZ = 10, 30, 10, 128
 TRAJ_WINDOW = 100        # seq_len of traj_pred/cfg/traj_pred_demo.yml: the window of multi-step trajectory prediction
 PRIOR_GRAPH_DEFAULT = '0'
+SKINNY_MAX_M = 256       # nets_kernels.cu kSkinnyMaxM: Linears of at most this many rows run the exact FP32 skinny GEMM
 WINDOW = PAST + CUR + FUT
 
 
@@ -40,7 +41,90 @@ def _declare(lib):
     lib.glamr_trajpred_windows_workspace_floats.restype = ctypes.c_size_t
     lib.glamr_trajpred_windows_workspace_floats.argtypes = [ctypes.c_int] * 3
     lib.glamr_trajpred_windows_forward.argtypes = [ctypes.c_void_p] + [ctypes.c_int] * 3 + [ctypes.c_void_p] * 6 + [ctypes.c_size_t, ctypes.c_void_p]
+    vp, sz = ctypes.c_void_p, ctypes.c_size_t
+    lib.glamr_infiller_ragged_workspace_floats.restype = sz
+    lib.glamr_infiller_ragged_workspace_floats.argtypes = [ctypes.c_int]
+    lib.glamr_infiller_forward_ragged.argtypes = [vp, ctypes.c_int] + [vp] * 6 + [ctypes.c_int, vp, sz, vp]
+    lib.glamr_trajpred_ragged_workspace_floats.restype = sz
+    lib.glamr_trajpred_ragged_workspace_floats.argtypes = [ctypes.c_int, vp]
+    lib.glamr_trajpred_forward_ragged.argtypes = [vp, ctypes.c_int] + [vp] * 11 + [sz, vp]
+    lib.glamr_trajpred_windows_ragged_workspace_floats.restype = sz
+    lib.glamr_trajpred_windows_ragged_workspace_floats.argtypes = [ctypes.c_int, vp, ctypes.c_int]
+    lib.glamr_trajpred_windows_forward_ragged.argtypes = [vp, ctypes.c_int, ctypes.c_int] + [vp] * 10 + [sz, vp]
     lib._nets_declared = True
+
+
+def _np_ptr(a):
+    return a.ctypes.data_as(ctypes.c_void_p)
+
+
+def _infiller_class(rb):
+    """which of the infiller's Linears (50, 30, 2 and 1 rows per track) a call of rb tracks runs above the skinny-GEMM limit"""
+    return sum(s * rb > SKINNY_MAX_M for s in (50, 30, 2, 1))
+
+
+def ragged_plan(seq_len, row_batch=None, sample_num=1, traj_window=TRAJ_WINDOW, multi_step_traj=False):
+    """Host plan of a ragged prior call (MotionTrajJointModel.inference with `seq_len`).
+
+    Input row b is a track of seq_len[b] frames; row_batch[b] is the batch size of the single-track call it reproduces: runs of
+    row_batch[b] consecutive rows of equal length are one block, the persons of one equal-length call.  Each row becomes
+    `sample_num` expanded rows e = b * sample_num + s, which reproduce a call of row_batch[b] * sample_num tracks.  The library
+    needs the rows ordered by the kernels their Linears run (include/glamr_b200.h): `inf_order` / `pred_order` are the expanded
+    rows in the infiller's and the predictor's order, `inf_off` / `pred_off` the packed frame offsets in that order and
+    `pred_woff` the window offsets of the windowed predictor."""
+    lens = [int(t) for t in seq_len]
+    B, S = len(lens), int(sample_num)
+    rb = [1] * B if row_batch is None else [int(r) for r in row_batch]
+    if len(rb) != B or B == 0 or S < 1:
+        raise ValueError(f'seq_len and row_batch need one entry per row, got {B} and {len(rb)}')
+    blocks, b = [], 0
+    while b < B:
+        P = rb[b]
+        if P < 1 or b + P > B or any(rb[q] != P or lens[q] != lens[b] for q in range(b, b + P)):
+            raise ValueError(f'rows {b}..{b + P - 1}: row_batch {P} must name a block of {P} consecutive rows of equal length')
+        blocks.append((b, P))
+        b += P
+    short = [t for t in lens if t <= PAST]
+    if short:
+        # the error type the single-track call raises for such a track (its library call refuses it)
+        raise L.GlamrError(f'ragged_plan: tracks of {short} frames have no infiller window (the infiller needs more than {PAST} frames)')
+    E = B * S
+    lens_e = np.repeat(np.asarray(lens, dtype=np.int32), S)
+    rb_e = np.repeat(np.asarray(rb, dtype=np.int32) * S, S)
+    nwin_e = -(-(lens_e - PAST) // CUR)
+    C_e = -(-lens_e // int(traj_window))
+    inf_order = np.array(sorted(range(E), key=lambda e: (_infiller_class(int(rb_e[e])), -int(lens_e[e]), e)), dtype=np.int64)
+
+    def pred_class(e):
+        f, r = (int(C_e[e]) * int(traj_window), int(C_e[e])) if multi_step_traj else (int(lens_e[e]), 1)
+        return (f * int(rb_e[e]) > SKINNY_MAX_M) + (r * int(rb_e[e]) > SKINNY_MAX_M)
+    pred_order = np.array(sorted(range(E), key=lambda e: (pred_class(e), e)), dtype=np.int64)
+    off = lambda order, n: np.concatenate([[0], np.cumsum(n[order])]).astype(np.int32)
+    return {'B': B, 'S': S, 'E': E, 'blocks': blocks, 'lens': lens_e, 'row_batch': rb_e, 'nwin': nwin_e, 'C': C_e,
+            'inf_order': inf_order, 'pred_order': pred_order, 'inf_off': off(inf_order, lens_e), 'pred_off': off(pred_order, lens_e),
+            'pred_woff': off(pred_order, C_e), 'multi_step_traj': bool(multi_step_traj), 'traj_window': int(traj_window)}
+
+
+def draw_ragged_eps(plan, device, infiller=True, traj=True):
+    """The prior's eps for the expanded rows of `plan`, drawn as the serial calls draw them: for each block in row order, the
+    infiller's randn((windows, P * S, 128)) and then the predictor's randn((P * S, 128)) (single pass) or
+    randn((windows, P * S, 128)) (windowed); `infiller` / `traj` False: that network's eps are given and not drawn (None).
+    -> (infiller eps [E, max windows, 128], predictor eps per expanded row: [E, 128] or a list of [C_e, 128])"""
+    S = plan['S']
+    inf = torch.zeros((plan['E'], int(plan['nwin'].max()), NZ), device=device) if infiller else None
+    rows = [None] * plan['E']
+    for b0, P in plan['blocks']:
+        e0, n = b0 * S, P * S
+        nwin, C = int(plan['nwin'][e0]), int(plan['C'][e0])
+        if infiller:
+            inf[e0:e0 + n, :nwin] = torch.randn((nwin, n, NZ), device=device).transpose(0, 1)
+        if traj and plan['multi_step_traj']:
+            rows[e0:e0 + n] = list(torch.randn((C, n, NZ), device=device).transpose(0, 1))
+        elif traj:
+            rows[e0:e0 + n] = list(torch.randn((n, NZ), device=device))
+    if not traj:
+        return inf, None
+    return inf, (rows if plan['multi_step_traj'] else torch.stack(rows))
 
 
 class _GraphCache:
@@ -353,6 +437,7 @@ class MTConfig:
 
 class MotionTrajJointModel:
     supports_person_batch = True     # inference() accepts [B, T, 69] with B > 1 (GlobalReconOptimizer.infer_motion_traj_all)
+    supports_ragged_batch = True     # inference() accepts seq_len [B]: tracks of different lengths in one call
 
     def __init__(self, cfg=None, device=torch.device('cuda'), log=None, smpl=None, states=None):
         """cfg: config id / object of the joint model (its checkpoint locations, `multi_step_trajpred` and
@@ -386,11 +471,21 @@ class MotionTrajJointModel:
     def get_traj_latent(self, seq_len):
         return self.traj_predictor.get_latent(seq_len)
 
-    def inference(self, batch, sample_num=1, recon=False):
+    def inference(self, batch, sample_num=1, recon=False, row_batch=None):
         """motion_traj_joint_model.py:141-145 (+ pred_trajectory :73-133, 'infer' mode).  With multi_step_trajpred the
-        trajectory's window latents come from `in_traj_window_latent` [windows, B * sample_num, 128] when given."""
+        trajectory's window latents come from `in_traj_window_latent` [windows, B * sample_num, 128] when given.
+
+        With `batch['seq_len']` [B], row b of `in_body_pose` [B, T_max, 69] / `frame_mask` [B, T_max] is a track of seq_len[b]
+        frames: all tracks run in one ragged call, and row b's outputs over its first seq_len[b] frames are bit-identical to
+        `inference` on that track alone (frames past its end are zero).  Row b uses the first windows of `in_motion_latent`
+        [B, windows, 128] (or of a shared [windows, 128]) and of `in_traj_window_latent` [windows, B * sample_num, 128] that its
+        length needs; `in_traj_latent` is [1 or B * sample_num, 128].  Latents that are not given are drawn in the order and shapes
+        of the single-track calls (draw_ragged_eps).  `row_batch` (internal: GlobalReconOptimizer) names blocks of equal-length
+        rows whose outputs must equal one call on the whole block instead (ragged_plan)."""
         if recon:
             raise NotImplementedError('recon mode needs the posterior encoders (training-side, out of scope)')
+        if batch.get('seq_len') is not None:
+            return self._inference_ragged(batch, sample_num, row_batch)
         data = self.mfiller.inference(batch, sample_num, recon=False, multi_step=True)
         motion = data['infer_out_body_pose']                                        # [B,S,T,69]
         B, S, T = motion.shape[:3]
@@ -404,3 +499,140 @@ class MotionTrajJointModel:
         data['infer_out_orient'] = out['infer_out_orient'].view(B, S, T, 3)
         data['infer_out_local_traj_tp'] = out['infer_out_local_traj_tp'].view(T, B, S, 11)
         return data
+
+    def ragged_plan(self, seq_len, row_batch=None, sample_num=1):
+        return ragged_plan(seq_len, row_batch, sample_num, self.traj_predictor.seq_len, self.multi_step_trajpred)
+
+    def draw_ragged_latents(self, seq_len, row_batch=None):
+        """eps of a sample_num 1 ragged call drawn as its serial calls draw them, as the latent keys `inference` takes"""
+        plan = self.ragged_plan(seq_len, row_batch)
+        inf, traj = draw_ragged_eps(plan, self.device)
+        out = {'in_motion_latent': inf}
+        if self.multi_step_trajpred:
+            wl = torch.zeros((int(plan['C'].max()), plan['E'], NZ), device=self.device)
+            for e, t in enumerate(traj):
+                wl[:t.shape[0], e] = t
+            out['in_traj_window_latent'] = wl
+        else:
+            out['in_traj_latent'] = traj
+        return out
+
+    def _ragged_eps(self, plan, batch):
+        """expanded-row eps from the batch's latents, or drawn (draw_ragged_eps) when none is given"""
+        dev, S, E = self.device, plan['S'], plan['E']
+        keys = ('in_motion_latent', 'in_traj_latent', 'in_traj_window_latent')
+        given = {k: batch[k].to(dev, torch.float32) for k in keys if batch.get(k) is not None}
+        tkey = 'in_traj_window_latent' if plan['multi_step_traj'] else 'in_traj_latent'
+        inf, traj = draw_ragged_eps(plan, dev, 'in_motion_latent' not in given, tkey not in given)
+        nmax = int(plan['nwin'].max())
+        ml = given.get('in_motion_latent')
+        if ml is not None:
+            ml = ml.unsqueeze(0).expand(plan['B'], -1, -1) if ml.dim() == 2 else ml
+            if ml.shape[1] < nmax:
+                raise ValueError(f'{nmax} windows need {nmax} latents, got {ml.shape[1]}')
+            inf = ml[:, :nmax].repeat_interleave(S, dim=0).contiguous()
+        if tkey not in given:
+            return inf, traj
+        if plan['multi_step_traj']:
+            wl = given[tkey]
+            if wl.shape[0] < int(plan['C'].max()) or wl.shape[1] != E:
+                raise ValueError(f'in_traj_window_latent: need [>= {int(plan["C"].max())}, {E}, {NZ}], got {tuple(wl.shape)}')
+            traj = [wl[:int(plan['C'][e]), e] for e in range(E)]
+        else:
+            tl = given[tkey]
+            traj = tl.expand(E, -1) if tl.shape[0] == 1 else tl
+            if traj.shape[0] != E:
+                raise ValueError(f'in_traj_latent: need [1 or {E}, {NZ}], got {tuple(tl.shape)}')
+        return inf, traj
+
+    def _inference_ragged(self, batch, sample_num, row_batch):
+        dev = self.device
+        pose_in = batch['in_body_pose'].to(dev, torch.float32)
+        frame_mask = batch['frame_mask'].to(dev, torch.float32)
+        B, Tmax = pose_in.shape[:2]
+        seq_len = [int(t) for t in (batch['seq_len'].tolist() if isinstance(batch['seq_len'], torch.Tensor) else batch['seq_len'])]
+        if len(seq_len) != B or max(seq_len) > Tmax:
+            raise ValueError(f'seq_len {seq_len} does not fit in_body_pose {tuple(pose_in.shape)}')
+        plan = self.ragged_plan(seq_len, row_batch, sample_num)
+        S, E = plan['S'], plan['E']
+        eps_inf, eps_traj = self._ragged_eps(plan, batch)
+        lens = plan['lens']
+        # frame (e, t) of expanded row e = b S + s is input frame b Tmax + t; packed rows in each network's order
+        src = lambda order: np.concatenate([(e // S) * Tmax + np.arange(lens[e]) for e in order])
+        dst = lambda order: np.concatenate([e * Tmax + np.arange(lens[e]) for e in order])
+        io, po = plan['inf_order'], plan['pred_order']
+        d_io, d_po = dst(io), dst(po)
+        srt = np.argsort(d_io, kind='stable')
+        host = np.concatenate([src(io), srt[np.searchsorted(d_io[srt], d_po)], d_po])       # + the infiller row of each predictor row
+        idx = torch.from_numpy(host).to(dev, non_blocking=False)
+        M = int(lens.sum())
+        ints = torch.from_numpy(np.concatenate([plan['inf_off'], plan['pred_off'], plan['pred_woff']]).astype(np.int32)).to(dev)
+        eps_inf = eps_inf[torch.from_numpy(io).to(dev)].contiguous()
+        if eps_traj is not None:
+            eps_traj = torch.stack([eps_traj[e] for e in po]) if not plan['multi_step_traj'] else torch.cat([eps_traj[e] for e in po])
+            eps_traj = eps_traj.contiguous()
+        lib = self.mfiller.net.lib
+        self.mfiller.net.workspace(lib.glamr_infiller_ragged_workspace_floats(E))
+        lens_p = np.ascontiguousarray(lens[po], dtype=np.int32)
+        tws = lib.glamr_trajpred_windows_ragged_workspace_floats(E, _np_ptr(lens_p), plan['traj_window']) if plan['multi_step_traj'] \
+            else lib.glamr_trajpred_ragged_workspace_floats(E, _np_ptr(lens_p))
+        self.traj_predictor.net.workspace(tws)
+        self.smpl._workspace(M, fk_only=True)
+        key = ('ragged', tuple(seq_len), None if row_batch is None else tuple(int(r) for r in row_batch), S,
+               Tmax, eps_traj is None)
+        with torch.cuda.device(dev):
+            body, local, trans, orient = self.mfiller.graphs.run(
+                key, lambda *a: self._ragged_forward(plan, *a), (pose_in, frame_mask, idx, ints, eps_inf, eps_traj))
+        T = Tmax
+        data = dict(batch)
+        data['infer_out_body_pose'] = body.view(B, S, T, 69)
+        data['batch_size'] = B
+        data['infer_out_trans'] = trans.view(B, S, T, 3)
+        data['infer_out_orient'] = orient.view(B, S, T, 3)
+        data['infer_out_pose'] = torch.cat([data['infer_out_orient'], data['infer_out_body_pose']], dim=-1)
+        data['infer_out_local_traj_tp'] = local.view(B, S, T, 11).permute(2, 0, 1, 3).contiguous()
+        return data
+
+    def _ragged_forward(self, plan, pose_in, frame_mask, idx, ints, eps_inf, eps_traj):
+        """the ragged infiller sweep, SMPL FK and the ragged predictor, device tensors only -> [E, T_max, *] outputs"""
+        dev, E = self.device, plan['E']
+        B, Tmax = pose_in.shape[:2]
+        M = int(plan['lens'].sum())
+        g_src, g_pred, g_dst = idx[:M], idx[M:2 * M], idx[2 * M:]
+        off_i, off_p, woff_p = ints[:E + 1], ints[E + 1:2 * E + 2], ints[2 * E + 2:]
+        io, po = plan['inf_order'], plan['pred_order']
+        lens_i = np.ascontiguousarray(plan['lens'][io], dtype=np.int32)
+        rb_i = np.ascontiguousarray(plan['row_batch'][io], dtype=np.int32)
+        lens_p = np.ascontiguousarray(plan['lens'][po], dtype=np.int32)
+        rb_p = np.ascontiguousarray(plan['row_batch'][po], dtype=np.int32)
+        pose = pose_in.reshape(B * Tmax, 69)[g_src].contiguous()                             # [M,69], infiller order
+        key_pad = (~(frame_mask.reshape(B * Tmax)[g_src] == 1)).to(torch.uint8).contiguous()
+        stream = torch.cuda.current_stream().cuda_stream
+        net = self.mfiller.net
+        ws = net.workspace(net.lib.glamr_infiller_ragged_workspace_floats(E))
+        L.check(net.lib.glamr_infiller_forward_ragged(net.h, E, _np_ptr(lens_i), _np_ptr(rb_i), off_i.data_ptr(), pose.data_ptr(),
+                                                      key_pad.data_ptr(), eps_inf.data_ptr(), eps_inf.shape[1], ws.data_ptr(), ws.numel(),
+                                                      stream), 'glamr_infiller_forward_ragged')
+        body = pose[g_pred].contiguous()                                                     # predictor order
+        jp = self.traj_predictor.get_joint_pos(body).contiguous()
+        local = torch.empty((M, 11), dtype=torch.float32, device=dev)
+        trans = torch.empty((M, 3), dtype=torch.float32, device=dev)
+        orient = torch.empty((M, 3), dtype=torch.float32, device=dev)
+        tnet = self.traj_predictor.net
+        eps_p = None if eps_traj is None else eps_traj.data_ptr()
+        if plan['multi_step_traj']:
+            ws = tnet.workspace(tnet.lib.glamr_trajpred_windows_ragged_workspace_floats(E, _np_ptr(lens_p), plan['traj_window']))
+            L.check(tnet.lib.glamr_trajpred_windows_forward_ragged(
+                tnet.h, E, plan['traj_window'], _np_ptr(lens_p), _np_ptr(rb_p), off_p.data_ptr(), woff_p.data_ptr(), jp.data_ptr(), eps_p,
+                local.data_ptr(), trans.data_ptr(), orient.data_ptr(), ws.data_ptr(), ws.numel(), stream), 'glamr_trajpred_windows_forward_ragged')
+        else:
+            ws = tnet.workspace(tnet.lib.glamr_trajpred_ragged_workspace_floats(E, _np_ptr(lens_p)))
+            L.check(tnet.lib.glamr_trajpred_forward_ragged(
+                tnet.h, E, _np_ptr(lens_p), _np_ptr(rb_p), off_p.data_ptr(), jp.data_ptr(), eps_p, None, None, local.data_ptr(),
+                trans.data_ptr(), orient.data_ptr(), ws.data_ptr(), ws.numel(), stream), 'glamr_trajpred_forward_ragged')
+        outs = []
+        for x, w in ((body, 69), (local, 11), (trans, 3), (orient, 3)):
+            o = torch.zeros((E * Tmax, w), dtype=torch.float32, device=dev)
+            o.index_copy_(0, g_dst, x)
+            outs.append(o)
+        return tuple(outs)

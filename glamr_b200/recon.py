@@ -492,7 +492,9 @@ class GlobalReconOptimizer:
     def infer_motion_traj_all(self, persons):
         """The reference runs the learned prior once per person with batch size 1 (:230-232 -> :353-392).  When every
         person exists for the same number of frames and the prior object declares `supports_person_batch`, the persons
-        form one batch [P, T, 69] instead (SURVEY.md §8(f)-1): same per-person arithmetic, P times fewer launches."""
+        form one batch [P, T, 69] instead (SURVEY.md §8(f)-1): same per-person arithmetic, P times fewer launches.  Persons of
+        different lengths go into one ragged call when the prior declares `supports_ragged_batch`, with each person's outputs and
+        eps those of its own call."""
         if self.mt_model is None:
             return
         ds = list(persons.values())
@@ -503,9 +505,42 @@ class GlobalReconOptimizer:
             out = self.mt_model.inference(batch, sample_num=1)
             for b, d in enumerate(ds):
                 self._take_prior_output(d, out, b)
+        elif len(ds) > 1 and getattr(self.mt_model, 'supports_ragged_batch', False):
+            # persons of different exist lengths: one ragged call whose row p reproduces person p's own call, eps included (the
+            # prior draws them person by person in the serial calls' order and shapes)
+            self._ragged_prior(ds, [1] * len(ds))
         else:
             for d in ds:
                 self.infer_motion_traj(d)
+
+    def _prior_rows(self, persons):
+        """the persons and the row_batch of each in a ragged prior call that reproduces infer_motion_traj_all: one block of P for
+        P persons of one exist length, else one row per person"""
+        ds = list(persons.values())
+        lens = {int(d['exist_len']) for d in ds}
+        P = len(ds)
+        block = P > 1 and len(lens) == 1 and getattr(self.mt_model, 'supports_person_batch', False)
+        return ds, [P if block else 1] * P
+
+    def _ragged_prior(self, ds, row_batch, latents=None):
+        """one ragged prior call over the exist ranges of the persons `ds` (of one or several data dicts); each person's outputs
+        and, without `latents`, its eps are those of its serial call"""
+        seq_len = [int(d['exist_len']) for d in ds]
+        Tm = max(seq_len)
+        pose = torch.zeros((len(ds), Tm, 69), device=self.device)
+        mask = torch.zeros((len(ds), Tm), device=self.device)
+        for b, d in enumerate(ds):
+            pose[b, :seq_len[b]] = d['smpl_pose_nofill'][_exist_range(d)]
+            mask[b, :seq_len[b]] = d['visible'][_exist_range(d)]
+        batch = {'in_body_pose': pose, 'frame_mask': mask, 'seq_len': seq_len, **(latents or {})}
+        out = self.mt_model.inference(batch, sample_num=1, row_batch=row_batch)
+        for b, d in enumerate(ds):
+            n = seq_len[b]
+            self._take_prior_output(d, {'infer_out_body_pose': out['infer_out_body_pose'][:, :, :n],
+                                        'infer_out_local_traj_tp': out['infer_out_local_traj_tp'][:n],
+                                        'infer_out_pose': out['infer_out_pose'][:, :, :n],
+                                        'infer_out_orient': out['infer_out_orient'][:, :, :n],
+                                        'infer_out_trans': out['infer_out_trans'][:, :, :n]}, b)
 
     def _take_prior_output(self, d, out, b):
         """:368-392 for batch row b of the prior's output"""
@@ -684,6 +719,13 @@ class GlobalReconOptimizer:
             d['person_transform_world'] = G.make_transform(d['smpl_orient_world'], d['root_trans_world'], 'axis_angle')
 
     def init_data(self, in_dict):
+        st = self._init_data_head(in_dict)
+        if self.flag_infer_motion_traj:
+            self.infer_motion_traj_all(st['persons'])
+        return self._init_data_tail(st)
+
+    def _init_data_head(self, in_dict):
+        """init_data up to the learned prior -> the state _init_data_tail finishes from"""
         if self.est_type != 'hybrik':
             raise ValueError(f'est_type {self.est_type} not supported')
         dev = self.device
@@ -699,8 +741,14 @@ class GlobalReconOptimizer:
             d['smpl_pose_nofill'] = d['smpl_pose'].clone()
             d['smpl_pose_nofill'][:int(d['fr_start'])] = 0.0
             d['smpl_pose_nofill'][int(d['fr_end']):] = 0.0
-        if self.flag_infer_motion_traj:
-            self.infer_motion_traj_all(persons)
+        return {'in_dict': in_dict, 'num_fr': num_fr, 'cam_pose': cam_pose, 'cam_pose_inv': cam_pose_inv, 'persons': persons,
+                'init_state': (self._init_host, self._init_visf, self._init_tables_f)}
+
+    def _init_data_tail(self, st):
+        """init_data after the learned prior"""
+        dev, in_dict, num_fr, persons = self.device, st['in_dict'], st['num_fr'], st['persons']
+        cam_pose, cam_pose_inv = st['cam_pose'], st['cam_pose_inv']
+        self._init_host, self._init_visf, self._init_tables_f = st['init_state']
         if not (self.flag_infer_motion_traj and self.flag_pred_traj):
             for d in persons.values():
                 self.init_default_traj(d)
@@ -1092,8 +1140,8 @@ class GlobalReconOptimizer:
         """Optimise every (sequence, seed) pair of `in_dicts` x `seeds` as one group of one problem.  The sequences share this
         optimiser's config and may differ in frames, persons, exist ranges and visibility.  ``outs[i][k]`` is what
         ``np.random.seed(s); torch.manual_seed(s); optimize(copy.deepcopy(in_dicts[i]))`` returns for s = seeds[k], bit for bit:
-        every pair's init_data (and the learned prior in it) runs as in the serial path after setting the RNGs the same way, then
-        the data dicts are attached as the groups of one problem (glamr_b200/problem.py) and the stages run once for all of them.
+        every pair's init_data runs as in the serial path after setting the RNGs the same way, with the learned prior of all pairs
+        in one ragged call when the prior supports it (_init_groups), then the data dicts are attached as the groups of one problem (glamr_b200/problem.py) and the stages run once for all of them.
         Each group's camera, terms and gradient are reduced exactly as in its own one-group problem, from its own normalisers.
         ``self.batch_loss_histories[i][k]`` is that pair's loss history of the last stage.  Scratch grows with the frame-persons of
         all groups (sum of persons x frames).  No continue_opt; one GPU only (run_dataset shards sequences over ranks)."""
@@ -1113,16 +1161,36 @@ class GlobalReconOptimizer:
         return outs
 
     def _init_groups(self, in_dicts, seeds):
-        """init_data of every (sequence, seed) pair, serially with the RNGs set as run_dataset sets them -> [[data dict]]"""
-        batch = []
+        """init_data of every (sequence, seed) pair with the RNGs set as run_dataset sets them -> [[data dict]].  With a prior that
+        takes ragged batches, init_data is split at the prior: each pair runs up to it, draws its eps as its serial prior call would
+        and keeps its RNG states; one ragged prior call then serves every person of every pair (rows in the classes of their serial
+        calls: a block of P for P equal-length persons, one row per person otherwise); and each pair finishes from its RNG states."""
+        ragged = self.flag_infer_motion_traj and getattr(self.mt_model, 'supports_ragged_batch', False)
+        heads = []
         for in_dict in in_dicts:
-            seq = []
             for s in seeds:
                 np.random.seed(s)
                 torch.manual_seed(s)
-                seq.append(self.init_data(copy.deepcopy(in_dict)))
-            batch.append(seq)
-        return batch
+                if not ragged:
+                    heads.append(self.init_data(copy.deepcopy(in_dict)))
+                    continue
+                st = self._init_data_head(copy.deepcopy(in_dict))
+                st['ds'], st['row_batch'] = self._prior_rows(st['persons'])
+                st['latents'] = self.mt_model.draw_ragged_latents([int(d['exist_len']) for d in st['ds']], st['row_batch'])
+                st['rng'] = (np.random.get_state(), torch.get_rng_state(), torch.cuda.get_rng_state(self.device))
+                heads.append(st)
+        if ragged:
+            self._ragged_prior([d for st in heads for d in st['ds']], [r for st in heads for r in st['row_batch']],
+                               _cat_latents([st['latents'] for st in heads]))
+            datas = []
+            for st in heads:
+                np.random.set_state(st['rng'][0])
+                torch.set_rng_state(st['rng'][1])
+                torch.cuda.set_rng_state(st['rng'][2], self.device)
+                datas.append(self._init_data_tail(st))
+            heads = datas
+        S = len(seeds)
+        return [heads[i * S:(i + 1) * S] for i in range(len(in_dicts))]
 
     def _optimize_groups(self, batch):
         """the stages of optimize for the groups of `batch` ([[data dict]] from _init_groups) as one problem; each pair's loss history
@@ -1141,6 +1209,21 @@ class GlobalReconOptimizer:
         lh, S = self.loss_history, len(batch[0])
         hists = [lh] if len(datas) == 1 else [lh[:, g] for g in range(len(datas))]
         self.batch_loss_histories = [hists[i * S:(i + 1) * S] for i in range(len(batch))]
+
+
+def _cat_latents(parts):
+    """the latents of several ragged prior calls (MotionTrajJointModel.draw_ragged_latents) as those of one call on all their rows"""
+    out = {}
+    for k, dim in (('in_motion_latent', 0), ('in_traj_latent', 0), ('in_traj_window_latent', 1)):
+        xs = [p[k] for p in parts if k in p]
+        if not xs:
+            continue
+        if k != 'in_traj_latent':
+            n = max(x.shape[1 - dim] for x in xs)
+            xs = [torch.nn.functional.pad(x, (0, 0, 0, n - x.shape[1])) if dim == 0 else
+                  torch.nn.functional.pad(x, (0, 0, 0, 0, 0, n - x.shape[0])) for x in xs]
+        out[k] = torch.cat(xs, dim=dim)
+    return out
 
 
 def _exist_range(d):

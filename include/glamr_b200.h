@@ -179,6 +179,36 @@ int glamr_trajpred_windows_forward(const glamr_net_t* n, int T, int B, int W, co
                                    float* out_local_traj, float* out_trans, float* out_orient_aa, float* workspace,
                                    size_t workspace_floats, void* stream);
 
+/* Tracks of different lengths in one call.  B tracks are packed without padding: track b is rows offsets[b] .. offsets[b+1] - 1 of
+ * every [rows, ...] buffer (offsets [B+1] int32 on the DEVICE, offsets[0] = 0).  lens [B] and row_batch [B] are HOST int32 arrays:
+ * the tracks' lengths, and for each track the batch size of the single-track call it reproduces (1 for a lone track, P for each
+ * track of a block of P equal-length tracks).  Track b's outputs are bit-identical to that call's outputs for it: every Linear
+ * runs on the kernel that call's M selects.  So the tracks must come in an order in which those kernels change at most once per
+ * Linear; any other order returns GLAMR_EINVAL:
+ *   infiller: by non-decreasing class c(rb) = #{S in 50, 30, 2, 1 : S * rb > 256}, and by non-increasing length within a class;
+ *   trajectory predictor: by non-decreasing (F * rb > 256) + (R * rb > 256), where F = T, R = 1 for the single pass and
+ *   F = C W, R = C with C = ceil(T / W) for the windowed one.
+ * Infiller: pose_io [rows,69] (overwritten with the infilled pose)  key_pad [rows] uint8 (1 = invisible)
+ *   eps [B][eps_windows][128]: track b's window i reads eps[b][i]; eps_windows >= ceil((T_b - 10) / 30) for every b, T_b > 10. */
+size_t glamr_infiller_ragged_workspace_floats(int B);
+int glamr_infiller_forward_ragged(const glamr_net_t* n, int B, const int32_t* lens, const int32_t* row_batch, const int32_t* offsets,
+                                  float* pose_io, const uint8_t* key_pad, const float* eps, int eps_windows, float* workspace,
+                                  size_t workspace_floats, void* stream);
+/* Single pass:  in_joint_pos [rows,69]   eps [B,128] or NULL   init_xy [B,2] / init_heading [B] or NULL
+ *   out_local_traj [rows,11]   out_trans [rows,3]   out_orient_aa [rows,3] */
+size_t glamr_trajpred_ragged_workspace_floats(int B, const int32_t* lens);
+int glamr_trajpred_forward_ragged(const glamr_net_t* n, int B, const int32_t* lens, const int32_t* row_batch, const int32_t* offsets,
+                                  const float* in_joint_pos, const float* eps, const float* init_xy, const float* init_heading,
+                                  float* out_local_traj, float* out_trans, float* out_orient_aa, float* workspace,
+                                  size_t workspace_floats, void* stream);
+/* Windowed: track b contributes C_b = ceil(T_b / W) windows.  win_offsets [B+1] (DEVICE) = prefix sums of C_b.
+ *   eps [sum C_b, 128] (track b's window c at row win_offsets[b] + c) or NULL   other buffers as the single pass */
+size_t glamr_trajpred_windows_ragged_workspace_floats(int B, const int32_t* lens, int W);
+int glamr_trajpred_windows_forward_ragged(const glamr_net_t* n, int B, int W, const int32_t* lens, const int32_t* row_batch,
+                                          const int32_t* offsets, const int32_t* win_offsets, const float* in_joint_pos, const float* eps,
+                                          float* out_local_traj, float* out_trans, float* out_orient_aa, float* workspace,
+                                          size_t workspace_floats, void* stream);
+
 /* ------------------------------------------------------------------------------------------------------------
  * Global optimisation  --  stands behind GlobalReconOptimizer.forward / compute_loss / optimize_main
  * (global_recon/models/global_recon_model.py:428-570), the residual registry global_recon/models/loss_func.py:314-340
