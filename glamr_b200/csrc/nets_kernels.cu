@@ -495,6 +495,12 @@ __global__ void concat_time_kernel(int Ta, int Tb, int B, int D, const float* __
   }
 }
 
+// rows 0 .. B-1 of out [*,256] := tok_a, rows B .. 2B-1 := tok_b (the posterior's two query tokens at time 0 and 1, time-major)
+__global__ void token_rows_kernel(int B, const float* __restrict__ tok_a, const float* __restrict__ tok_b, float* __restrict__ out) {
+  const int row = blockIdx.x, c = threadIdx.x;
+  out[(size_t)row * 256 + c] = (row < B ? tok_a : tok_b)[c];
+}
+
 // z = mu + eps * exp(0.5 logvar)  (lib/utils/dist.py:8-26); eps may be NULL (-> mu) or broadcast over the batch
 __global__ void sample_z_kernel(int B, int nz, const float* __restrict__ mu, int ld_mu, const float* __restrict__ logvar, int ld_lv,
                                 const float* __restrict__ eps, int eps_ld, float* __restrict__ z) {
@@ -822,8 +828,10 @@ extern "C" size_t glamr_infiller_workspace_floats(int B) { return (size_t)B * 50
 
 // One 50-frame window of MotionInfillerVAE.inference_one_step for d.B sequences (layout and kernel choice: WinDisp) -> *dec_out, the
 // 30 decoded frames [30 B, 69] (arena memory).  in_pose [50 B, 69]  key_pad_mask [B,50]  eps rows eps_ld apart (0: one row for all) or NULL
+// gt_cur NULL: mode 'infer', z drawn from the learned prior.  Otherwise mode 'recon' (time-major rows only): gt_cur [30,B,69] is the
+// ground-truth body pose of the window's 30 current frames, and z is the mean of the posterior q(z | X, C); eps is not read.
 static int infiller_window(const glamr_net* n, const WinDisp& d, const float* in_pose, const uint8_t* key_pad_mask, const float* eps,
-                           int eps_ld, float** dec_out_p, Arena& A, cudaStream_t s) {
+                           int eps_ld, const float* gt_cur, float** dec_out_p, Arena& A, cudaStream_t s) {
   const int B = d.B;
   const bool bm = d.rb != nullptr;
   int e = 0;
@@ -867,21 +875,47 @@ static int infiller_window(const glamr_net* n, const WinDisp& d, const float* in
   if ((rc = lin(s, d, S, 256, 512, cat, 512, cpe_w, cpe_b, x, 256, 0))) return rc;
   for (int l = 0; l < 2; ++l)
     if ((rc = encoder_layer(s, A, d, enc[l], S, x, key_pad_mask))) return rc;
-  // ---- learned prior over z (:354-362): two tokens attend to the context
-  GLAMR_CUDA_TRY(cudaMemcpyAsync(tok, mu_tok, 256 * sizeof(float), cudaMemcpyDeviceToDevice, s));
-  GLAMR_CUDA_TRY(cudaMemcpyAsync(tok + 256, lv_tok, 256 * sizeof(float), cudaMemcpyDeviceToDevice, s));
-  pe_concat(2 * B, B, 2, 256, tok, 0, 1, 0);
-  GLAMR_LAUNCH_CHECK();
-  if ((rc = lin(s, d, 2, 256, 512, cat, 512, ppe_w, ppe_b, px, 256, 0))) return rc;
-  if ((rc = decoder_layer(s, A, d, pri, 2, S, px, x, key_pad_mask))) return rc;
-  // the mu token's rows, then the logvar token's: rows 0 .. B-1 and B .. 2B-1 time-major, every other row batch-major
-  const float* pmu = px;
-  const float* plv = bm ? px + 256 : px + (size_t)B * 256;
-  const int ldp = bm ? 512 : 256;
-  if ((rc = lin(s, d, 1, 128, 256, pmu, ldp, pmw, pmb, mu, 128, 0))) return rc;
-  if ((rc = lin(s, d, 1, 128, 256, plv, ldp, plw, plb, lv, 128, 0))) return rc;
-  sample_z_kernel<<<(B * 128 + 127) / 128, 128, 0, s>>>(B, 128, mu, 128, lv, 128, eps, eps_ld, z);
-  GLAMR_LAUNCH_CHECK();
+  if (gt_cur) {
+    // ---- posterior (DataEncoder.forward, :204-233): [mu token | logvar token | in_fc(30 ground-truth frames)] with the PE of
+    // positions 0..31, two decoder layers (self-attention unmasked, cross-attention to the context), z = q_z_mu_net(row 0) (:375-376;
+    // the logvar head reaches no output of this mode)
+    if (bm) return GLAMR_EINVAL;
+    const std::string de = "data_encoder.";
+    const float* q_in_w = W(n, de + "in_fc.weight", 256 * 69, &e), * q_in_b = W(n, de + "in_fc.bias", 256, &e);
+    const float* qpe_w = W(n, de + "pos_enc.fc.weight", 256 * 512, &e), * qpe_b = W(n, de + "pos_enc.fc.bias", 256, &e);
+    DecLayer qdec[2] = {dec_layer(n, de + "temporal_net.layers.0", &e), dec_layer(n, de + "temporal_net.layers.1", &e)};
+    const float* q_mu_tok = W(n, de + "mu_token", 256, &e), * q_lv_tok = W(n, de + "logvar_token", 256, &e);
+    const float* qmw = W(n, de + "q_z_mu_net.weight", 128 * 256, &e), * qmb = W(n, de + "q_z_mu_net.bias", 128, &e);
+    if (e) return GLAMR_EINVAL;
+    const int Sq = 2 + Sc;
+    float* qx = A.take((size_t)Sq * B * 256);
+    if (!qx) return GLAMR_ENOSPACE;
+    token_rows_kernel<<<2 * B, 256, 0, s>>>(B, q_mu_tok, q_lv_tok, qx);
+    GLAMR_LAUNCH_CHECK();
+    if ((rc = lin(s, d, Sc, 256, 69, gt_cur, 69, q_in_w, q_in_b, qx + (size_t)2 * B * 256, 256, 0))) return rc;
+    pe_concat(Sq * B, B, Sq, 256, qx, 0, 0, 0);
+    GLAMR_LAUNCH_CHECK();
+    if ((rc = lin(s, d, Sq, 256, 512, cat, 512, qpe_w, qpe_b, qx, 256, 0))) return rc;
+    for (int l = 0; l < 2; ++l)
+      if ((rc = decoder_layer(s, A, d, qdec[l], Sq, S, qx, x, key_pad_mask))) return rc;
+    if ((rc = lin(s, d, 1, 128, 256, qx, 256, qmw, qmb, z, 128, 0))) return rc;
+  } else {
+    // ---- learned prior over z (:354-362): two tokens attend to the context
+    GLAMR_CUDA_TRY(cudaMemcpyAsync(tok, mu_tok, 256 * sizeof(float), cudaMemcpyDeviceToDevice, s));
+    GLAMR_CUDA_TRY(cudaMemcpyAsync(tok + 256, lv_tok, 256 * sizeof(float), cudaMemcpyDeviceToDevice, s));
+    pe_concat(2 * B, B, 2, 256, tok, 0, 1, 0);
+    GLAMR_LAUNCH_CHECK();
+    if ((rc = lin(s, d, 2, 256, 512, cat, 512, ppe_w, ppe_b, px, 256, 0))) return rc;
+    if ((rc = decoder_layer(s, A, d, pri, 2, S, px, x, key_pad_mask))) return rc;
+    // the mu token's rows, then the logvar token's: rows 0 .. B-1 and B .. 2B-1 time-major, every other row batch-major
+    const float* pmu = px;
+    const float* plv = bm ? px + 256 : px + (size_t)B * 256;
+    const int ldp = bm ? 512 : 256;
+    if ((rc = lin(s, d, 1, 128, 256, pmu, ldp, pmw, pmb, mu, 128, 0))) return rc;
+    if ((rc = lin(s, d, 1, 128, 256, plv, ldp, plw, plb, lv, 128, 0))) return rc;
+    sample_z_kernel<<<(B * 128 + 127) / 128, 128, 0, s>>>(B, 128, mu, 128, lv, 128, eps, eps_ld, z);
+    GLAMR_LAUNCH_CHECK();
+  }
   // ---- decoder (:383-395): z repeated over the 30 current frames, PE offset 10
   pe_concat(Mc, B, Sc, 128, z, 1, 0, 10);
   GLAMR_LAUNCH_CHECK();
@@ -905,7 +939,7 @@ extern "C" int glamr_infiller_window_forward(const glamr_net* n, int B, const fl
   cudaStream_t s = (cudaStream_t)stream;
   Arena A{workspace, workspace_floats, 0};
   float* dec_out = nullptr;
-  const int rc = infiller_window(n, WinDisp{B, nullptr}, in_pose, key_pad_mask, eps, eps_rows == 1 ? 0 : 128, &dec_out, A, s);
+  const int rc = infiller_window(n, WinDisp{B, nullptr}, in_pose, key_pad_mask, eps, eps_rows == 1 ? 0 : 128, nullptr, &dec_out, A, s);
   if (rc) return rc;
   concat_time_kernel<<<64, 256, 0, s>>>(10, 30, B, 69, in_pose, dec_out, out_pose);
   GLAMR_LAUNCH_CHECK();
@@ -937,8 +971,58 @@ __global__ void window_commit_kernel(int B, int s0, int nfr, const float* __rest
   if (i < nfr * row) pose[(size_t)s0 * row + i] = out[i];
 }
 
+// the ground truth of window s0's 30 current frames: gwin [30,B,69] = frames s0 + 10 .. s0 + 39 of gt [T,B,69], zero past T
+__global__ void window_gt_kernel(int T, int B, int s0, const float* __restrict__ gt, float* __restrict__ gwin) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  const int row = B * 69;
+  if (i >= 30 * row) return;
+  const int t = s0 + 10 + i / row;
+  gwin[i] = t < T ? gt[(size_t)t * row + i % row] : 0.0f;
+}
+
 extern "C" size_t glamr_infiller_sequence_workspace_floats(int B) {
   return glamr_infiller_workspace_floats(B) + (size_t)90 * B * 69 + (size_t)(B * 50 + 3) / 4 + 192;
+}
+extern "C" size_t glamr_infiller_recon_workspace_floats(int B) {
+  if (B <= 0) return 0;
+  return glamr_infiller_sequence_workspace_floats(B) + (((size_t)30 * B * 69 + 63) & ~(size_t)63);
+}
+
+// The sweep of both modes: gt NULL runs 'infer' with eps, otherwise 'recon' with the ground truth gt [T,B,69] (eps not read).
+static int infiller_sweep(const glamr_net* n, int T, int B, float* pose_io, const float* gt, const uint8_t* key_pad_all, const float* eps,
+                          int eps_rows, float* workspace, size_t workspace_floats, cudaStream_t s) {
+  float* win = workspace;
+  float* out = win + (size_t)50 * B * 69;
+  uint8_t* kp = reinterpret_cast<uint8_t*>(out + (size_t)40 * B * 69);
+  float* rest = reinterpret_cast<float*>((reinterpret_cast<uintptr_t>(kp + (size_t)B * 50) + 255) & ~(uintptr_t)255);
+  float* gwin = nullptr;
+  if (gt) {
+    gwin = rest;
+    rest += ((size_t)30 * B * 69 + 63) & ~(size_t)63;
+  }
+  const size_t rest_floats = workspace_floats - (size_t)(rest - workspace);
+  const int nwin = (T - 10 + 29) / 30;
+  const int prep_blocks = (50 * B * 69 + 255) / 256;
+  for (int i = 0; i < nwin; ++i) {
+    const int s0 = i * 30;
+    window_prep_kernel<<<prep_blocks, 256, 0, s>>>(T, B, s0, pose_io, key_pad_all, win, kp);
+    GLAMR_LAUNCH_CHECK();
+    if (gt) {
+      window_gt_kernel<<<(30 * B * 69 + 255) / 256, 256, 0, s>>>(T, B, s0, gt, gwin);
+      GLAMR_LAUNCH_CHECK();
+    }
+    Arena A{rest, rest_floats, 0};
+    float* dec = nullptr;
+    const float* eps_i = gt ? nullptr : eps + (size_t)i * eps_rows * 128;
+    const int rc = infiller_window(n, WinDisp{B, nullptr}, win, kp, eps_i, eps_rows == 1 ? 0 : 128, gwin, &dec, A, s);
+    if (rc) return rc;
+    concat_time_kernel<<<64, 256, 0, s>>>(10, 30, B, 69, win, dec, out);
+    GLAMR_LAUNCH_CHECK();
+    const int nfr = (s0 + 40 < T ? s0 + 40 : T) - s0;
+    window_commit_kernel<<<(nfr * B * 69 + 255) / 256, 256, 0, s>>>(B, s0, nfr, out, pose_io);
+    GLAMR_LAUNCH_CHECK();
+  }
+  return GLAMR_OK;
 }
 
 //   pose_io [T,B,69]: the input body pose, overwritten with the infilled pose   key_pad_all [B,T] uint8 (1 = frame invisible)
@@ -947,25 +1031,16 @@ extern "C" int glamr_infiller_forward(const glamr_net* n, int T, int B, float* p
                                       int eps_rows, float* workspace, size_t workspace_floats, void* stream) {
   if (!n || T <= 10 || B <= 0 || !pose_io || !key_pad_all || !eps || !workspace || (eps_rows != 1 && eps_rows != B)) return GLAMR_EINVAL;
   if (workspace_floats < glamr_infiller_sequence_workspace_floats(B)) return GLAMR_ENOSPACE;
-  cudaStream_t s = (cudaStream_t)stream;
-  float* win = workspace;
-  float* out = win + (size_t)50 * B * 69;
-  uint8_t* kp = reinterpret_cast<uint8_t*>(out + (size_t)40 * B * 69);
-  float* rest = reinterpret_cast<float*>((reinterpret_cast<uintptr_t>(kp + (size_t)B * 50) + 255) & ~(uintptr_t)255);
-  const size_t rest_floats = workspace_floats - (size_t)(rest - workspace);
-  const int nwin = (T - 10 + 29) / 30;
-  const int prep_blocks = (50 * B * 69 + 255) / 256;
-  for (int i = 0; i < nwin; ++i) {
-    const int s0 = i * 30;
-    window_prep_kernel<<<prep_blocks, 256, 0, s>>>(T, B, s0, pose_io, key_pad_all, win, kp);
-    GLAMR_LAUNCH_CHECK();
-    const int rc = glamr_infiller_window_forward(n, B, win, kp, eps + (size_t)i * eps_rows * 128, eps_rows, out, rest, rest_floats, stream);
-    if (rc) return rc;
-    const int nfr = (s0 + 40 < T ? s0 + 40 : T) - s0;
-    window_commit_kernel<<<(nfr * B * 69 + 255) / 256, 256, 0, s>>>(B, s0, nfr, out, pose_io);
-    GLAMR_LAUNCH_CHECK();
-  }
-  return GLAMR_OK;
+  return infiller_sweep(n, T, B, pose_io, nullptr, key_pad_all, eps, eps_rows, workspace, workspace_floats, (cudaStream_t)stream);
+}
+
+//   pose_io [T,B,69]: the input body pose, overwritten with the reconstructed pose   gt_body_pose [T,B,69]: the ground truth the
+//   posterior encodes   key_pad_all [B,T] uint8 (1 = frame invisible)
+extern "C" int glamr_infiller_recon_forward(const glamr_net* n, int T, int B, float* pose_io, const float* gt_body_pose,
+                                            const uint8_t* key_pad_all, float* workspace, size_t workspace_floats, void* stream) {
+  if (!n || T <= 10 || B <= 0 || !pose_io || !gt_body_pose || !key_pad_all || !workspace) return GLAMR_EINVAL;
+  if (workspace_floats < glamr_infiller_recon_workspace_floats(B)) return GLAMR_ENOSPACE;
+  return infiller_sweep(n, T, B, pose_io, gt_body_pose, key_pad_all, nullptr, 1, workspace, workspace_floats, (cudaStream_t)stream);
 }
 
 // ------------------------------------------------------------------------------------------------ tracks of their own length
@@ -1069,7 +1144,7 @@ extern "C" int glamr_infiller_forward_ragged(const glamr_net* n, int B, const in
     GLAMR_LAUNCH_CHECK();
     Arena A{rest, rest_floats, 0};
     float* dec = nullptr;
-    const int rc = infiller_window(n, WinDisp{Bi, rb_slot.data()}, win, kp, epsw, 128, &dec, A, s);
+    const int rc = infiller_window(n, WinDisp{Bi, rb_slot.data()}, win, kp, epsw, 128, nullptr, &dec, A, s);
     if (rc) return rc;
     window_commit_ragged_kernel<<<(Bi * 40 * 69 + 255) / 256, 256, 0, s>>>(Bi, m, s0, offsets, win, dec, pose_io);
     GLAMR_LAUNCH_CHECK();

@@ -32,6 +32,9 @@ def _declare(lib):
     lib.glamr_infiller_sequence_workspace_floats.restype = ctypes.c_size_t
     lib.glamr_infiller_forward.argtypes = [ctypes.c_void_p, ctypes.c_int, ctypes.c_int] + [ctypes.c_void_p] * 3 + [ctypes.c_int, ctypes.c_void_p, ctypes.c_size_t,
                                                                                                      ctypes.c_void_p]
+    lib.glamr_infiller_recon_workspace_floats.restype = ctypes.c_size_t
+    lib.glamr_infiller_recon_workspace_floats.argtypes = [ctypes.c_int]
+    lib.glamr_infiller_recon_forward.argtypes = [ctypes.c_void_p, ctypes.c_int, ctypes.c_int] + [ctypes.c_void_p] * 4 + [ctypes.c_size_t, ctypes.c_void_p]
     lib.glamr_trajpred_workspace_floats.restype = ctypes.c_size_t
     lib.glamr_net_set_tensor.argtypes = [ctypes.c_void_p, ctypes.c_char_p, ctypes.c_void_p, ctypes.c_size_t]
     lib.glamr_infiller_window_forward.argtypes = [ctypes.c_void_p, ctypes.c_int] + [ctypes.c_void_p] * 3 + [ctypes.c_int, ctypes.c_void_p,
@@ -178,12 +181,14 @@ class _Net:
         _declare(self.lib)
         self.h = ctypes.c_void_p()
         L.check(self.lib.glamr_net_create(ctypes.byref(self.h)), 'glamr_net_create')
+        self.names = set()
         with torch.cuda.device(self.device):
             for name, val in state.items():
                 arr = np.ascontiguousarray(val.detach().cpu().numpy() if isinstance(val, torch.Tensor) else np.asarray(val), dtype=np.float32)
                 if arr.size == 0 or arr.dtype != np.float32:
                     continue
                 L.check(self.lib.glamr_net_set_tensor(self.h, name.encode(), arr.ctypes.data_as(ctypes.c_void_p), arr.size), f'set_tensor {name}')
+                self.names.add(name)
         self._ws = None
 
     def workspace(self, floats):
@@ -214,10 +219,33 @@ class MotionInfillerVAE:
         return torch.randn((int(np.ceil((seq_len - PAST) / CUR)), NZ))
 
     def inference(self, batch, sample_num=1, recon=False, multi_step=True):
-        if recon or not multi_step:
-            raise NotImplementedError('only the multi-step sampling path (recon=False) is implemented on CUDA')
+        """multi-step inference (:643-652): `sample_num` infer sweeps, then with `recon` one reconstruction sweep.
+
+        `pose` [B,T,72] (with `pose_mask` [B,T,72]) is the ground truth: the infer outputs carry its root orientation, the input body
+        pose defaults to (pose * pose_mask)[..., 3:] when `in_body_pose` is not given, and `recon` encodes it with the posterior
+        (z = the posterior mean) into `recon_out_pose` [B,T,72] / `recon_out_body_pose` [B,T,69].  Both sweeps start from the input
+        body pose; the caller's tensors are never written."""
+        if not multi_step:
+            raise NotImplementedError('only the multi-step path (multi_step=True) is implemented on CUDA')
+        gt = batch.get('pose')
+        if gt is not None and batch.get('pose_mask') is None:
+            raise ValueError('`pose` needs `pose_mask` (the input body pose is (pose * pose_mask)[..., 3:])')
+        if recon:
+            if gt is None:
+                raise ValueError('recon=True needs the ground-truth `pose` [B, T, 72] that the posterior encodes')
+            if batch.get('seq_len') is not None:
+                raise NotImplementedError('recon=True is not implemented for tracks of different lengths (`seq_len`)')
+            if not any(k.startswith('data_encoder.') for k in self.net.names):
+                raise ValueError('recon=True needs the posterior encoder weights (data_encoder.*), which this net does not have')
         dev = self.device
-        pose_in = batch['in_body_pose'].to(dev, torch.float32).contiguous()
+        if gt is not None:
+            gt = gt.to(dev, torch.float32)
+        if batch.get('in_body_pose') is not None:
+            pose_in = batch['in_body_pose'].to(dev, torch.float32).contiguous()
+        elif gt is not None:
+            pose_in = (gt * batch['pose_mask'].to(dev, torch.float32))[..., 3:].contiguous()
+        else:
+            raise KeyError('in_body_pose')
         frame_mask = batch['frame_mask'].to(dev, torch.float32).contiguous()
         latent = batch.get('in_motion_latent')
         latent = None if latent is None else latent.to(dev, torch.float32).contiguous()
@@ -228,9 +256,29 @@ class MotionInfillerVAE:
             body = self.graphs.run(key, lambda a, b, c: self._windows(a, b, c, sample_num), (pose_in, frame_mask, latent))
         data = dict(batch)
         data['infer_out_body_pose'] = body
-        data['infer_out_pose'] = torch.cat([torch.zeros_like(body[..., :3]), body], dim=-1)
+        root = torch.zeros_like(body[..., :3]) if gt is None else gt[:, None, :, :3].expand(-1, sample_num, -1, -1)
+        data['infer_out_pose'] = torch.cat([root, body], dim=-1)
         data['batch_size'], data['seq_len'] = B0, T
+        if recon:
+            gt_body = gt[..., 3:].contiguous()
+            self.net.workspace(self.net.lib.glamr_infiller_recon_workspace_floats(B0))
+            with torch.cuda.device(dev):
+                rbody = self.graphs.run(('recon', B0, T), self._recon_windows, (pose_in, gt_body, frame_mask))
+            data['recon_out_body_pose'] = rbody
+            data['recon_out_pose'] = torch.cat([gt[..., :3], rbody], dim=-1)
         return data
+
+    def _recon_windows(self, pose_in, gt_body, frame_mask):
+        """the reconstruction sweep (inference_multi_step with recon=True): one library call, [B, T, 69] out"""
+        B, T = pose_in.shape[:2]
+        pose = pose_in.transpose(0, 1).contiguous().clone()                                       # [T,B,69], overwritten in place
+        gt_tb = gt_body.transpose(0, 1).contiguous()
+        key_pad_all = (~(frame_mask == 1)).to(torch.uint8).contiguous()                           # [B,T]
+        lib = self.net.lib
+        ws = self.net.workspace(lib.glamr_infiller_recon_workspace_floats(B))
+        L.check(lib.glamr_infiller_recon_forward(self.net.h, T, B, pose.data_ptr(), gt_tb.data_ptr(), key_pad_all.data_ptr(), ws.data_ptr(),
+                                                 ws.numel(), torch.cuda.current_stream().cuda_stream), 'glamr_infiller_recon_forward')
+        return pose.transpose(0, 1).contiguous()
 
     def _windows(self, pose_in, frame_mask, latent, sample_num):
         """motion_infiller_vae.py:618-632: autoregressive 50-frame windows, stride 30 -- one library call for the whole sweep
@@ -483,7 +531,8 @@ class MotionTrajJointModel:
         of the single-track calls (draw_ragged_eps).  `row_batch` (internal: GlobalReconOptimizer) names blocks of equal-length
         rows whose outputs must equal one call on the whole block instead (ragged_plan)."""
         if recon:
-            raise NotImplementedError('recon mode needs the posterior encoders (training-side, out of scope)')
+            raise NotImplementedError('recon mode needs the trajectory predictor\'s posterior encoder, which is not implemented on CUDA '
+                                      '(MotionInfillerVAE.inference(recon=True) reconstructs the motion)')
         if batch.get('seq_len') is not None:
             return self._inference_ragged(batch, sample_num, row_batch)
         data = self.mfiller.inference(batch, sample_num, recon=False, multi_step=True)

@@ -64,6 +64,27 @@ def infiller_param_shapes():
     return s
 
 
+def infiller_posterior_param_shapes():
+    """the infiller's posterior encoder q(z | X, C) (DataEncoder, motion_infiller_vae.py:126-249), which only reconstruction runs.
+    Kept apart from infiller_param_shapes(): make_state draws the sorted names from one stream, so a new name there would move
+    every other stand-in weight."""
+    s = {}
+    s.update(_linear('data_encoder.in_fc', D, 69))
+    s.update(_linear('data_encoder.pos_enc.fc', D, 2 * D))
+    for l in range(2):
+        s.update(_dec_layer(f'data_encoder.temporal_net.layers.{l}'))
+    s['data_encoder.mu_token'] = (D,)
+    s['data_encoder.logvar_token'] = (D,)
+    s.update(_linear('data_encoder.q_z_mu_net', NZ, D))
+    s.update(_linear('data_encoder.q_z_logvar_net', NZ, D))
+    return s
+
+
+def make_infiller_posterior_state(seed=1236):
+    """stand-in posterior weights from a seed of their own; merged into make_prior_states()[0] they make a full infiller"""
+    return make_state(infiller_posterior_param_shapes(), seed)
+
+
 def trajpred_param_shapes():
     s = {}
     s.update(_mlp('context_encoder.in_mlp', 69, [512, 256]))

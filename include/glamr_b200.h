@@ -164,6 +164,14 @@ int glamr_infiller_window_forward(const glamr_net_t* n, int B, const float* in_p
 size_t glamr_infiller_sequence_workspace_floats(int B);
 int glamr_infiller_forward(const glamr_net_t* n, int T, int B, float* pose_io, const uint8_t* key_pad_all, const float* eps,
                            int eps_rows, float* workspace, size_t workspace_floats, void* stream);
+/* The same sweep in reconstruction mode (inference_multi_step with recon=True, motion_infiller_vae.py:551-557,618-632): each window
+ * encodes the ground truth of its 30 current frames with the posterior DataEncoder (:204-233, the data_encoder.* parameters, which
+ * must be registered) and decodes z = the posterior mean.  No eps.
+ *   pose_io [T,B,69]: input body pose, overwritten with the reconstructed pose   gt_body_pose [T,B,69]   key_pad_all as above
+ *   workspace >= glamr_infiller_recon_workspace_floats(B) floats */
+size_t glamr_infiller_recon_workspace_floats(int B);
+int glamr_infiller_recon_forward(const glamr_net_t* n, int T, int B, float* pose_io, const float* gt_body_pose,
+                                 const uint8_t* key_pad_all, float* workspace, size_t workspace_floats, void* stream);
 /*   in_joint_pos [T,B,69] (23 joints from SMPL.get_joints)   eps as above   init_xy [B,2] / init_heading [B] or NULL
  *   out_local_traj [T,B,11]   out_trans [T,B,3]   out_orient_aa [T,B,3] */
 int glamr_trajpred_forward(const glamr_net_t* n, int T, int B, const float* in_joint_pos, const float* eps, int eps_rows,
